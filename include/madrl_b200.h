@@ -118,7 +118,8 @@ void* madrl_ww_state_ptr(madrl_ww* h);
 /* seed(): new key, draw counters reset to 0 (waterworld.py:135-137 creates a fresh generator). */
 int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream);
 /* Launch geometry override (0 = library default): resident blocks per SM.  Blocks are one warp (= one
- * env) since round 2; `warps_per_block` is accepted for ABI stability and ignored. */
+ * env); `warps_per_block` is range-checked ([0,4]) for ABI stability and otherwise ignored.  The same
+ * holds for madrl_pursuit_set_launch and madrl_hostage_set_launch. */
 int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the

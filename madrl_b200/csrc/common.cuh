@@ -51,10 +51,25 @@ __device__ __forceinline__ void store_stream(T* p, T v) {
   __stcs(p, v);
 }
 
-// Experiment: launch the warp-per-env kernels as 32-thread blocks.  The env index then derives from
-// blockIdx alone, so ptxas can prove the persistent loop and every branch on warp-uniform values
-// uniform: the BRA.DIV guards in front of the warp collectives disappear, loop bookkeeping moves to
-// the uniform datapath and the register count drops (Waterworld C2: 72 regs + spills -> 56, none).
+// Vector type of an (x, y) pair of `real`.
+template <typename real> struct Vec2;
+template <> struct Vec2<float> { typedef float2 type; };
+template <> struct Vec2<double> { typedef double2 type; };
+
+// Butterfly sum over the full warp: every lane gets the total.  (postproc.cu's `warp_sum` is a
+// different reduction whose result lands in lane 0 only.)
+template <typename real>
+__device__ __forceinline__ real warp_allreduce_sum(real v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL_MASK, v, o);
+  return v;
+}
+
+// The warp-per-env kernels are launched as 32-thread blocks (one env per block; see engine_launch in
+// engine.cuh).  The env index then derives from blockIdx alone, so ptxas can prove the persistent loop
+// and every branch on warp-uniform values uniform: the BRA.DIV guards in front of the warp collectives
+// disappear, loop bookkeeping moves to the uniform datapath and the register count drops (Waterworld
+// C2: 72 regs + spills -> 56, none).
 
 // Kernels are launched through one macro and the PTX-level helpers below sit behind one guard so
 // that the test-only warp emulator (tests/emu: the kernels compiled by g++ against a fake

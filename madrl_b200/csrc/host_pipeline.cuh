@@ -48,7 +48,7 @@ struct HostPipe {
 // steps is one contiguous slice of each).
 struct StepBytes { size_t act, obs, rew, done, info; };
 
-// launch(t0, Tc, act_dev, obs_dev, rew_dev, done_dev, info_dev, stream) -> rc runs Tc lockstep steps.
+// launch(Tc, act_dev, obs_dev, rew_dev, done_dev, info_dev, stream) -> rc runs the next Tc lockstep steps.
 template <class Launch>
 int host_rollout(HostPipe& hp, int T, const StepBytes& sb, const void* act_h, void* obs_h, void* rew_h, void* done_h,
                  void* info_h, int obs_last_only, Launch launch) {
@@ -72,7 +72,7 @@ int host_rollout(HostPipe& hp, int T, const StepBytes& sb, const void* act_h, vo
   int c = 0;
   for (size_t t0 = 0; t0 < TT; t0 += Tc, ++c) {
     const size_t n = (t0 + Tc <= TT) ? Tc : TT - t0;
-    rc = launch((int)t0, (int)n, st + t0 * sb.act, st + o_obs + t0 * sb.obs, st + o_rew + t0 * sb.rew,
+    rc = launch((int)n, st + t0 * sb.act, st + o_obs + t0 * sb.obs, st + o_rew + t0 * sb.rew,
                 st + o_done + t0 * sb.done, st + o_info + t0 * sb.info, hp.compute);
     if (rc) return rc;
     MADRL_CUDA_CHECK(cudaEventRecord(hp.done[c], hp.compute));

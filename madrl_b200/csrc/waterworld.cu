@@ -24,8 +24,8 @@
 #include <new>
 
 #include "common.cuh"
+#include "engine.cuh"
 #include "philox.cuh"
-#include "host_pipeline.cuh"
 
 namespace madrl {
 
@@ -73,17 +73,6 @@ struct WWParams {
   uint8_t* peer_done[8];
   int32_t* peer_info[8];
 };
-
-template <typename real> struct Vec2;
-template <> struct Vec2<float> { typedef float2 type; };
-template <> struct Vec2<double> { typedef double2 type; };
-
-template <typename real>
-__device__ __forceinline__ real warp_sum(real v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(FULL_MASK, v, o);
-  return v;
-}
 
 // 0 <= sv < best for best > 0, in one comparison for float: non-negative floats order like their bit patterns
 // and every negative one has the sign bit set, i.e. compares above any positive `best` as an unsigned integer.
@@ -219,7 +208,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
             wx += w * sx_l[kc]; wy += w * sy_l[kc];
           }
         }
-        wx = warp_sum(wx); wy = warp_sum(wy);
+        wx = warp_allreduce_sum(wx); wy = warp_allreduce_sum(wy);
         if (lane == pi) { pax = wx; pay = wy; }
       }
     }
@@ -298,7 +287,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
             if (y[0] != cy) vy[0] = 0;
             x[0] = cx; y[0] = cy;
           }
-          pen = p.control_penalty * (p.reward_global ? warp_sum(sq) : sq);
+          pen = p.control_penalty * (p.reward_global ? warp_allreduce_sum(sq) : sq);
         }
         // ---- obstacle rebound (velocity only): ww:247-270 ----------------------------------------
 #pragma unroll
@@ -491,7 +480,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
           }
           }
           if constexpr (POLICY) {   // sum over the sensors; lane pi keeps pursuer pi's next action
-            pwx = warp_sum(pwx); pwy = warp_sum(pwy);
+            pwx = warp_allreduce_sum(pwx); pwy = warp_allreduce_sum(pwy);
             if (lane == pi) { pax = pwx; pay = pwy; }
           }
         }
@@ -623,20 +612,19 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
 // =================================================================================================
 using namespace madrl;
 
-struct madrl_ww {
+struct madrl_ww : EngineCore {
   madrl_ww_config cfg;
   madrl_ww_layout lay;
-  char* state;
-  bool owns_state;
-  int device, sms;
-  int warps_per_block, blocks_per_sm;
-  madrl::HostPipe pipe;   // staging + streams of the host-buffer entry points (lazily created)
-  void* term_obs;         // madrl_ww_set_terminal_obs (NULL = off)
   // peer gather buffers (multi-GPU fused exchange); n_peers == 0: disabled
   int n_peers, peer_rank, peer_tmax;
   void* peer_rew[8];
   void* peer_done[8];
   void* peer_info[8];
+
+  StepBytes step_bytes() const {
+    const size_t E = cfg.n_envs, Np = cfg.n_pursuers, rb = lay.real_bytes;
+    return {E * Np * 2 * rb, E * Np * lay.obs_dim * rb, E * Np * rb, E, E * 2 * 4};
+  }
 };
 
 static int ww_validate(const madrl_ww_config* c) {
@@ -675,73 +663,15 @@ extern "C" int madrl_ww_state_layout(const madrl_ww_config* c, madrl_ww_layout* 
   return MADRL_OK;
 }
 
-template <typename real>
-static int ww_upload_sensors(madrl_ww* h) {
-  const int K = h->cfg.n_sensors;
-  real* tab = new (std::nothrow) real[2 * (size_t)K];
-  if (!tab) return MADRL_ENOMEM;
-  // ww:29-31  angles = linspace(0, 2pi, K+1)[:-1]
-  const double step = (2.0 * M_PI - 0.0) / (double)K;
-  for (int k = 0; k < K; ++k) {
-    const double a = (double)k * step + 0.0;
-    tab[k] = (real)cos(a);
-    tab[K + k] = (real)sin(a);
-  }
-  cudaError_t e = cudaMemcpy(h->state + h->lay.sensors, tab, sizeof(real) * 2 * K, cudaMemcpyHostToDevice);
-  delete[] tab;
-  MADRL_CUDA_CHECK(e);
-  return MADRL_OK;
-}
-
 extern "C" int madrl_ww_create(const madrl_ww_config* c, void* state_dev, madrl_ww** out) {
-  MADRL_REQUIRE(out != nullptr, "out is NULL");
-  madrl_ww_layout lay;
-  int rc = madrl_ww_state_layout(c, &lay);
-  if (rc) return rc;
-  madrl_ww* h = new (std::nothrow) madrl_ww();
-  if (!h) return MADRL_ENOMEM;
-  h->cfg = *c;
-  h->lay = lay;
-  h->warps_per_block = 0;
-  h->blocks_per_sm = 0;
-  h->n_peers = 0; h->peer_rank = 0; h->peer_tmax = 0;
-  cudaError_t e = cudaGetDevice(&h->device);
-  if (e != cudaSuccess) { set_error("cudaGetDevice: %s", cudaGetErrorString(e)); delete h; return MADRL_ECUDA; }
-  h->sms = sm_count(h->device);
-  if (h->sms <= 0) { delete h; return MADRL_ECUDA; }
-  if (state_dev) {
-    h->state = (char*)state_dev;
-    h->owns_state = false;
-  } else {
-    e = cudaMalloc((void**)&h->state, lay.total_bytes);
-    if (e != cudaSuccess) { set_error("cudaMalloc(%zu): %s", lay.total_bytes, cudaGetErrorString(e)); delete h; return MADRL_ENOMEM; }
-    h->owns_state = true;
-  }
-  e = cudaMemset(h->state, 0, lay.total_bytes);
-  if (e != cudaSuccess) { set_error("cudaMemset: %s", cudaGetErrorString(e)); madrl_ww_destroy(h); return MADRL_ECUDA; }
-  rc = c->fp64 ? ww_upload_sensors<double>(h) : ww_upload_sensors<float>(h);
-  if (rc) { madrl_ww_destroy(h); return rc; }
-  *out = h;
-  return MADRL_OK;
+  return engine_create(c, state_dev, out, madrl_ww_state_layout, upload_sensors<madrl_ww>);
 }
 
-extern "C" int madrl_ww_destroy(madrl_ww* h) {
-  if (!h) return MADRL_OK;
-  if (h->owns_state && h->state) cudaFree(h->state);
-  h->pipe.destroy();
-  delete h;
-  return MADRL_OK;
-}
+extern "C" int madrl_ww_destroy(madrl_ww* h) { return engine_destroy(h); }
 
 extern "C" void* madrl_ww_state_ptr(madrl_ww* h) { return h ? h->state : nullptr; }
 
-extern "C" int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream) {
-  MADRL_REQUIRE(h != nullptr, "handle is NULL");
-  h->cfg.seed = seed;
-  MADRL_CUDA_CHECK(cudaMemsetAsync(h->state + h->lay.rng_counter, 0, 8 * (size_t)h->cfg.n_envs,
-                                   (cudaStream_t)stream));
-  return MADRL_OK;
-}
+extern "C" int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream) { return engine_seed(h, seed, stream); }
 
 extern "C" int madrl_ww_set_peers(madrl_ww* h, int n_peers, int rank, int t_max, void* const* rew_peers,
                                   void* const* done_peers, void* const* info_peers) {
@@ -760,49 +690,17 @@ extern "C" int madrl_ww_set_peers(madrl_ww* h, int n_peers, int rank, int t_max,
 }
 
 extern "C" int madrl_ww_set_terminal_obs(madrl_ww* h, void* term_obs_dev) {
-  MADRL_REQUIRE(h != nullptr, "handle is NULL");
-  h->term_obs = term_obs_dev;
-  return MADRL_OK;
+  return engine_set_terminal_obs(h, term_obs_dev);
 }
 
 extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm) {
-  MADRL_REQUIRE(h != nullptr, "handle is NULL");
-  MADRL_REQUIRE(warps_per_block >= 0 && warps_per_block <= 4, "warps_per_block must be in [0,4]");
-  MADRL_REQUIRE(blocks_per_sm >= 0 && blocks_per_sm <= 32, "blocks_per_sm must be in [0,32]");
-  h->warps_per_block = warps_per_block;
-  h->blocks_per_sm = blocks_per_sm;
-  return MADRL_OK;
-}
-
-// Largest representable t with correctly-rounded sqrt(t) <= thr: `sqrt(d2) <= thr` (what
-// scipy's cdist + `<=` computes in the reference) is then exactly `d2 <= t`.
-template <typename real>
-static real exact_sq_threshold(double thr_d) {
-  const real thr = (real)thr_d;
-  real t = thr * thr;
-  const real up = (real)INFINITY, dn = -(real)INFINITY;
-  while (std::sqrt(t) <= thr) t = std::nextafter(t, up);
-  while (std::sqrt(t) > thr) t = std::nextafter(t, dn);
-  return t;
+  return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
 template <typename real, int OPL, int KCH, int KC, bool PEER, bool POLICY>
 static int ww_launch_inst2(madrl_ww* h, const WWParams<real>& p, cudaStream_t stream) {
-  const auto kfn = ww_kernel<real, OPL, KCH, KC, PEER, POLICY>;
-  int resident = 0;
   const size_t smem = OPL >= 2 ? (size_t)p.Nall * CandSlot<real>::kStride : 0;   // candidate slots
-  if (smem > 48 * 1024)
-    MADRL_CUDA_CHECK(cudaFuncSetAttribute(kfn,
-                                          cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  MADRL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kfn, 32, smem));
-  if (resident < 1) resident = 1;
-  if (h->blocks_per_sm > 0 && h->blocks_per_sm < resident) resident = h->blocks_per_sm;
-  int grid = p.E;                                    // one warp (= one 32-thread block) per env ...
-  if (grid > h->sms * resident) grid = h->sms * resident;  // ... or a single persistent wave
-  MADRL_LAUNCH(kfn, grid, 32, smem, stream, p);
-  g_launches.fetch_add(1);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
+  return engine_launch(h, ww_kernel<real, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p);
 }
 
 template <typename real, int OPL, int KCH, int KC>
@@ -929,45 +827,17 @@ extern "C" int madrl_ww_step(madrl_ww* h, const void* actions_dev, void* obs_dev
 
 // ---- host-buffer entry points -------------------------------------------------------------------
 extern "C" int madrl_ww_reset_host(madrl_ww* h, const uint8_t* mask_host, void* obs_host) {
-  MADRL_REQUIRE(h != nullptr && obs_host != nullptr, "handle/obs is NULL");
-  const size_t E = h->cfg.n_envs, rb = h->lay.real_bytes;
-  const size_t obs_b = E * h->cfg.n_pursuers * h->lay.obs_dim * rb;
-  const size_t mask_off = align_up(obs_b, 256);
-  int rc = h->pipe.ensure(mask_off + E);
-  if (rc) return rc;
-  char* st = (char*)h->pipe.stage;
-  uint8_t* mask_dev = nullptr;
-  if (mask_host) {
-    mask_dev = (uint8_t*)(st + mask_off);
-    MADRL_CUDA_CHECK(cudaMemcpyAsync(mask_dev, mask_host, E, cudaMemcpyHostToDevice, 0));
-    // rows of unmasked envs must survive: seed the staging buffer with the caller's obs
-    MADRL_CUDA_CHECK(cudaMemcpyAsync(st, obs_host, obs_b, cudaMemcpyHostToDevice, 0));
-  }
-  rc = madrl_ww_reset(h, mask_dev, st, nullptr);
-  if (rc) return rc;
-  MADRL_CUDA_CHECK(cudaMemcpyAsync(obs_host, st, obs_b, cudaMemcpyDeviceToHost, 0));
-  MADRL_CUDA_CHECK(cudaStreamSynchronize(0));
-  return MADRL_OK;
+  return engine_reset_host(h, mask_host, obs_host,
+                           [h](uint8_t* mask, char* obs) { return madrl_ww_reset(h, mask, obs, nullptr); });
 }
 
 extern "C" int madrl_ww_rollout_host2(madrl_ww* h, int T, const void* actions_host, void* obs_host,
                                       void* rew_host, uint8_t* done_host, int32_t* info_host,
                                       int auto_reset, int flags) {
-  MADRL_REQUIRE(h != nullptr, "handle is NULL");
-  MADRL_REQUIRE(T >= 1, "T must be >= 1");
-  MADRL_REQUIRE(actions_host && obs_host && rew_host && done_host && info_host, "NULL trajectory buffer");
-  MADRL_REQUIRE((flags & ~MADRL_HOST_OBS_LAST) == 0, "unknown flags %d", flags);
-  const size_t E = h->cfg.n_envs, Np = h->cfg.n_pursuers, rb = h->lay.real_bytes;
-  const StepBytes sb = {E * Np * 2 * rb, E * Np * h->lay.obs_dim * rb, E * Np * rb, E, E * 2 * 4};
-  void* const keep = h->term_obs;    // chunk-relative offsets: the side tensor is a device-API feature
-  h->term_obs = nullptr;
-  const int rc_ = host_rollout(h->pipe, T, sb, actions_host, obs_host, rew_host, done_host, info_host,
-                      flags & MADRL_HOST_OBS_LAST,
-                      [&](int, int Tc, char* a, char* o, char* r, char* d, char* i, cudaStream_t st) {
-                        return madrl_ww_rollout(h, Tc, a, o, r, (uint8_t*)d, (int32_t*)i, auto_reset, st);
-                      });
-  h->term_obs = keep;
-  return rc_;
+  return engine_rollout_host(h, T, actions_host, obs_host, rew_host, done_host, info_host, flags,
+                             [&](int Tc, char* a, char* o, char* r, char* d, char* i, cudaStream_t st) {
+                               return madrl_ww_rollout(h, Tc, a, o, r, (uint8_t*)d, (int32_t*)i, auto_reset, st);
+                             });
 }
 
 extern "C" int madrl_ww_rollout_host(madrl_ww* h, int T, const void* actions_host, void* obs_host,

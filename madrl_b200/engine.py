@@ -1,0 +1,194 @@
+"""What the three env families share on the Python side.
+
+``BatchedEngine`` is the base of ``BatchedMAWaterWorld``, ``BatchedPursuitEvade`` and
+``BatchedHostageWorld``: one handle of the ``madrl_<abi>_*`` C ABI, its state blob in HBM, and the entry
+points every family has.  A family declares its ABI prefix, its layout struct, the action shape of one
+agent, the info shape of one env and the info keys of ``step()``; its constructor builds the config
+struct and hands it to ``BatchedEngine.__init__``.
+
+``DropInEnv`` is the base of the drop-in env classes (``MAWaterWorld``, ``PursuitEvade``,
+``ContinuousHostageWorld``): a one-env engine built by the family's ``_make_engine``, and rllab's
+batched plug-in hook (``vectorized`` / ``vec_env_executor``; rllab/sandbox/rocky/tf/envs/base.py:97-103).
+"""
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _lib
+from ._lib import _ptr
+from .core import AbstractMAEnv, EzPickle
+
+
+class BatchedEngine(object):
+    _abi = None       # C ABI prefix: madrl_<_abi>_*
+    _Layout = None    # ctypes struct filled by madrl_<_abi>_state_layout
+    _act_tail = ()    # action shape of one acting agent
+    _info_tail = ()   # info shape of one env
+    _info_keys = ()   # step() info keys: one per info column, or a single key for the whole row
+
+    def __init__(self, cfg, n_acting, device, dtype, act_dtype, create_args=()):
+        """`n_acting`: agents that act and observe per env; `dtype`: observations and rewards;
+        `act_dtype`: actions; `create_args`: family arguments of madrl_<abi>_create before the blob."""
+        if not torch.cuda.is_available():
+            raise _lib.EngineError("madrl_b200 needs a CUDA device (there is no CPU fallback)")
+        self._L = _lib.lib()
+        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None \
+            else torch.device(device)
+        if self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        self.cfg, self._n_acting, self.dtype, self._act_dtype = cfg, n_acting, dtype, act_dtype
+        self.layout = self._Layout()
+        _lib.check(self._fn("state_layout")(C.byref(cfg), C.byref(self.layout)))
+        self.obs_dim = int(self.layout.obs_dim)
+        with torch.cuda.device(self.device):
+            self._blob = torch.zeros(int(self.layout.total_bytes), dtype=torch.uint8, device=self.device)
+            h = C.c_void_p()
+            _lib.check(self._fn("create")(C.byref(cfg), *create_args, _ptr(self._blob), C.byref(h)))
+        self._h = h
+
+    def _fn(self, name):
+        return getattr(self._L, "madrl_%s_%s" % (self._abi, name))
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._fn("destroy")(h)
+
+    def _view(self, off, dtype, shape):
+        n = int(np.prod(shape)) * torch.empty((), dtype=dtype).element_size()
+        return self._blob[off:off + n].view(dtype).view(*shape)
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def set_terminal_obs(self, term_obs):
+        """Keep the terminal observations of done steps: `term_obs` (same shape / dtype as the obs tensor
+        of the following auto-reset rollouts) receives, at the [t, e] slots where `done` is set, the
+        observation the env returned BEFORE it was reset in place (StandardizedEnv needs it,
+        madrl_environments/__init__.py:283-291).  None switches it off."""
+        if term_obs is not None:
+            assert term_obs.is_contiguous() and term_obs.device == self.device, "term_obs must be a contiguous device tensor"
+        self._term_keepalive = term_obs
+        _lib.check(self._fn("set_terminal_obs")(self._h, _ptr(term_obs)))
+
+    def set_launch(self, warps_per_block=0, blocks_per_sm=0):
+        _lib.check(self._fn("set_launch")(self._h, warps_per_block, blocks_per_sm))
+
+    def seed(self, seed=None):
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("seed")(self._h, 0 if seed is None else int(seed), self._stream()))
+        return [seed]
+
+    def reset(self, mask=None, out=None):
+        """reset() of the masked envs (all if None) -> obs [E, A, D]."""
+        shape = (self.n_envs, self._n_acting, self.obs_dim)
+        obs = out if out is not None else torch.zeros(shape, dtype=self.dtype, device=self.device)
+        if out is not None:
+            _lib.require_tensor(out, "out", self.dtype, shape, self.device)
+        if mask is not None:
+            mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("reset")(self._h, _ptr(mask), _ptr(obs), self._stream()))
+        return obs
+
+    def _trajectory_shapes(self, T):
+        """(dtype, shape) of obs, rew, done and info of a T-step rollout."""
+        E, A = self.n_envs, self._n_acting
+        return ((self.dtype, (T, E, A, self.obs_dim)), (self.dtype, (T, E, A)), (torch.uint8, (T, E)),
+                (torch.int32, (T, E) + self._info_tail))
+
+    def _outputs(self, T, out):
+        """The trajectory buffers of a T-step device rollout: `out` after checking dtype / shape /
+        contiguity / placement, or new ones."""
+        if out is None:   # spelled out: this is on the per-step path of the single-env drop-ins
+            E, A, dev = self.n_envs, self._n_acting, self.device
+            return (torch.empty((T, E, A, self.obs_dim), dtype=self.dtype, device=dev),
+                    torch.empty((T, E, A), dtype=self.dtype, device=dev),
+                    torch.empty((T, E), dtype=torch.uint8, device=dev),
+                    torch.empty((T, E) + self._info_tail, dtype=torch.int32, device=dev))
+        obs, rew, done, info = out
+        for t, n, (dt, s) in zip(out, ("obs", "rew", "done", "info"), self._trajectory_shapes(T)):
+            _lib.require_tensor(t, n, dt, s, self.device)
+        return obs, rew, done, info
+
+    def rollout(self, actions, auto_reset=True, out=None):
+        """T lockstep steps in one kernel launch.  actions [T, E, A, *act_tail] ->
+        (obs [T,E,A,D], rew [T,E,A], done [T,E] uint8, info [T,E,*info_tail] int32)."""
+        actions = actions.to(device=self.device, dtype=self._act_dtype).contiguous()
+        T = actions.shape[0]
+        assert actions.shape == (T, self.n_envs, self._n_acting) + self._act_tail, actions.shape
+        obs, rew, done, info = self._outputs(T, out)
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("rollout")(self._h, T, _ptr(actions), _ptr(obs), _ptr(rew),
+                                           _ptr(done), _ptr(info), int(auto_reset), self._stream()))
+        return obs, rew, done, info
+
+    def _rollout_heuristic(self, T, obs0, auto_reset, out, record_actions, actions_out, *extra):
+        """madrl_<abi>_rollout_heuristic; `extra`: the family's arguments before the stream."""
+        E, A = self.n_envs, self._n_acting
+        _lib.require_tensor(obs0, "obs0", self.dtype, (E, A, self.obs_dim), self.device)
+        obs, rew, done, info = self._outputs(T, out)
+        act_shape = (T, E, A) + self._act_tail
+        if actions_out is not None:   # caller-owned buffer for the actions taken (no allocation in a rollout loop)
+            act = _lib.require_tensor(actions_out, "actions_out", self._act_dtype, act_shape, self.device)
+        else:
+            act = torch.empty(act_shape, dtype=self._act_dtype, device=self.device) if record_actions else None
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("rollout_heuristic")(self._h, T, _ptr(obs0), _ptr(act), _ptr(obs), _ptr(rew),
+                                                     _ptr(done), _ptr(info), int(auto_reset), *extra,
+                                                     self._stream()))
+        return act, obs, rew, done, info
+
+    def step(self, actions, auto_reset=False):
+        """One lockstep step.  actions [E, A, *act_tail] (or anything reshapeable to it)."""
+        a = torch.as_tensor(actions, device=self.device, dtype=self._act_dtype).reshape(
+            (1, self.n_envs, self._n_acting) + self._act_tail)
+        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset)
+        if len(self._info_keys) == 1:
+            return obs[0], rew[0], done[0], {self._info_keys[0]: info[0]}
+        return obs[0], rew[0], done[0], {k: info[0, :, i] for i, k in enumerate(self._info_keys)}
+
+    def rollout_host(self, actions, obs, rew, done, info, auto_reset=True, obs_last=False):
+        """rollout() with HOST tensors (pinned for full PCIe speed); the copies are inside the call,
+        chunked and overlapped with the compute (csrc/host_pipeline.cuh).  `obs_last=True`: only the last
+        step's observations come back (obs is [E, A, D]) -- the policy-on-device mode."""
+        T = actions.shape[0]
+        E, A = self.n_envs, self._n_acting
+        _lib.require_tensor(actions, "actions", self._act_dtype, (T, E, A) + self._act_tail, 'cpu')
+        shapes = self._trajectory_shapes(T)
+        if obs_last:
+            shapes = ((self.dtype, (E, A, self.obs_dim)),) + shapes[1:]
+        for t, n, (dt, s) in zip((obs, rew, done, info), ("obs", "rew", "done", "info"), shapes):
+            _lib.require_tensor(t, n, dt, s, 'cpu')
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("rollout_host2")(self._h, T, _ptr(actions), _ptr(obs), _ptr(rew), _ptr(done),
+                                                 _ptr(info), int(auto_reset), 1 if obs_last else 0))
+        return obs, rew, done, info
+
+
+class DropInEnv(AbstractMAEnv, EzPickle):
+    """Base of the drop-in env classes.  A family sets `_reward_mech`, `_seed_value` and `_env_id` and
+    defines `_make_engine(n_envs, **kw)`, which builds its batched engine from the env's attributes."""
+
+    vectorized = True  # rllab batched plug-in hook (tf/envs/base.py:97-103)
+
+    def setup(self):
+        """(Re)build the engine from the current attributes (set_param_values contract)."""
+        self._engine = self._make_engine(1, env_id_base=self._env_id)
+
+    @property
+    def reward_mech(self):
+        return self._reward_mech
+
+    def get_param_values(self):
+        return self.__dict__
+
+    def seed(self, seed=None):
+        self._seed_value = 0 if seed is None else int(seed)
+        self._engine.seed(self._seed_value)
+        return [seed]
+
+    def vec_env_executor(self, n_envs, max_path_length):
+        from .vec_executor import BatchedVecExecutor
+        return BatchedVecExecutor(self, n_envs, max_path_length)

@@ -19,10 +19,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr())
+from ._lib import _ptr
 
 
 def _stream(dev):

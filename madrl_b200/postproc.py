@@ -17,10 +17,7 @@ import numpy as np
 import torch
 
 from . import _lib
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
+from ._lib import _ptr
 
 
 def _stream(dev):

@@ -11,12 +11,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from .core import AbstractMAEnv, Agent, EzPickle
+from .core import Agent, EzPickle
+from .engine import BatchedEngine, DropInEnv
 from .spaces import Box, Discrete
-
-
-def _ptr(t):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 class DiscreteAgent(Agent):
@@ -38,7 +35,30 @@ class DiscreteAgent(Agent):
         return Discrete(5)
 
 
-class BatchedPursuitEvade(object):
+def map_pool_array(map_pool):
+    """The map pool as a C-contiguous int32 [n_maps, xs, ys] array (one [xs, ys] map is a pool of one)."""
+    mp = np.ascontiguousarray(np.asarray(map_pool), dtype=np.int32)
+    return mp[None] if mp.ndim == 2 else mp
+
+
+def pe_config(n_envs, map_pool, n_evaders=1, n_pursuers=1, obs_range=3, flatten=True, layer_norm=10, n_catch=2,
+              catchr=0.01, term_pursuit=5.0, urgency_reward=0.0, include_id=True, surround=True,
+              constraint_window=1.0, sample_maps=False, reward_mech='global', random_opponents=False,
+              max_opponents=10, seed=0, env_id_base=0, max_path_length=0):
+    """The madrl_pursuit_config of BatchedPursuitEvade's arguments; `map_pool` as map_pool_array returns it."""
+    return _lib.PEConfig(
+        n_envs=n_envs, env_id_base=env_id_base, n_pursuers=n_pursuers, n_evaders=n_evaders,
+        xs=map_pool.shape[1], ys=map_pool.shape[2], n_maps=map_pool.shape[0], obs_range=obs_range,
+        flatten=int(bool(flatten)), n_catch=n_catch, surround=int(bool(surround)),
+        reward_global=int(reward_mech == 'global'), include_id=int(bool(include_id)),
+        sample_maps=int(bool(sample_maps)), max_path_length=int(max_path_length or 0),
+        max_opponents=int(max_opponents) if random_opponents else 0,   # pursuit_evade.py:81-82,177-181
+        layer_norm=float(layer_norm), catchr=float(catchr), term_pursuit=float(term_pursuit),
+        urgency_reward=float(urgency_reward), constraint_window=float(constraint_window),
+        seed=int(seed))
+
+
+class BatchedPursuitEvade(BatchedEngine):
     """E lockstep PursuitEvade instances resident in HBM.
 
     Keyword names follow pursuit_evade.py:49-148.  Evader motion uses the env's counter-based
@@ -46,53 +66,26 @@ class BatchedPursuitEvade(object):
     instance, utils/Controllers.py:11, so there is no reference stream to reproduce).
     """
 
+    _abi, _Layout, _act_tail, _info_tail, _info_keys = "pursuit", _lib.PELayout, (), (), ("removed",)
+
     def __init__(self, n_envs, map_pool, n_evaders=1, n_pursuers=1, obs_range=3, flatten=True,
                  layer_norm=10, n_catch=2, catchr=0.01, term_pursuit=5.0, urgency_reward=0.0,
                  include_id=True, surround=True, constraint_window=1.0, sample_maps=False,
                  reward_mech='global', random_opponents=False, max_opponents=10, device=None, seed=0,
                  env_id_base=0, max_path_length=0):
-        if not torch.cuda.is_available():
-            raise _lib.EngineError("madrl_b200 needs a CUDA device (there is no CPU fallback)")
-        self._L = _lib.lib()
-        self.device = torch.device("cuda", torch.cuda.current_device()) if device is None \
-            else torch.device(device)
-        if self.device.index is None:
-            self.device = torch.device("cuda", torch.cuda.current_device())
-        mp = np.ascontiguousarray(np.asarray(map_pool), dtype=np.int32)
-        if mp.ndim == 2:
-            mp = mp[None]
+        mp = map_pool_array(map_pool)
+        cfg = pe_config(n_envs, mp, n_evaders=n_evaders, n_pursuers=n_pursuers, obs_range=obs_range,
+                        flatten=flatten, layer_norm=layer_norm, n_catch=n_catch, catchr=catchr,
+                        term_pursuit=term_pursuit, urgency_reward=urgency_reward, include_id=include_id,
+                        surround=surround, constraint_window=constraint_window, sample_maps=sample_maps,
+                        reward_mech=reward_mech, random_opponents=random_opponents, max_opponents=max_opponents,
+                        seed=seed, env_id_base=env_id_base, max_path_length=max_path_length)
         self.map_pool = mp
         self.n_envs, self.n_pursuers, self.n_evaders = n_envs, n_pursuers, n_evaders
         self.obs_range, self.reward_mech, self.flatten = obs_range, reward_mech, bool(flatten)
-        self.cfg = _lib.PEConfig(
-            n_envs=n_envs, env_id_base=env_id_base, n_pursuers=n_pursuers, n_evaders=n_evaders,
-            xs=mp.shape[1], ys=mp.shape[2], n_maps=mp.shape[0], obs_range=obs_range,
-            flatten=int(bool(flatten)), n_catch=n_catch, surround=int(bool(surround)),
-            reward_global=int(reward_mech == 'global'), include_id=int(bool(include_id)),
-            sample_maps=int(bool(sample_maps)), max_path_length=int(max_path_length or 0),
-            max_opponents=int(max_opponents) if random_opponents else 0,   # pursuit_evade.py:81-82,177-181
-            layer_norm=float(layer_norm), catchr=float(catchr), term_pursuit=float(term_pursuit),
-            urgency_reward=float(urgency_reward), constraint_window=float(constraint_window),
-            seed=int(seed))
-        self.layout = _lib.PELayout()
-        _lib.check(self._L.madrl_pursuit_state_layout(C.byref(self.cfg), C.byref(self.layout)))
-        self.obs_dim = int(self.layout.obs_dim)
-        self.n_agents = int(self.layout.n_agents)
-        with torch.cuda.device(self.device):
-            self._blob = torch.zeros(int(self.layout.total_bytes), dtype=torch.uint8, device=self.device)
-            h = C.c_void_p()
-            _lib.check(self._L.madrl_pursuit_create(C.byref(self.cfg), C.c_void_p(mp.ctypes.data),
-                                                    _ptr(self._blob), C.byref(h)))
-        self._h = h
-
-    def __del__(self):
-        h, self._h = getattr(self, "_h", None), None
-        if h:
-            self._L.madrl_pursuit_destroy(h)
-
-    def _view(self, off, dtype, shape):
-        n = int(np.prod(shape)) * torch.empty((), dtype=dtype).element_size()
-        return self._blob[off:off + n].view(dtype).view(*shape)
+        super().__init__(cfg, n_pursuers, device, torch.float32, torch.int32,
+                         create_args=(C.c_void_p(mp.ctypes.data),))
+        self.n_agents = int(self.layout.n_agents)   # pursuers + evaders (the state records), not the acting agents
 
     @property
     def state(self):
@@ -105,22 +98,6 @@ class BatchedPursuitEvade(object):
                     rng_counter=self._view(L.rng_counter, torch.int64, (E,)),
                     stale=self._view(L.stale, torch.int16, (E, Np, RR)))
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
-    def set_terminal_obs(self, term_obs):
-        """Keep the terminal observations of done steps: `term_obs` (same shape / dtype as the obs tensor
-        of the following auto-reset rollouts) receives, at the [t, e] slots where `done` is set, the
-        observation the env returned BEFORE it was reset in place (StandardizedEnv needs it,
-        madrl_environments/__init__.py:283-291).  None switches it off."""
-        if term_obs is not None:
-            assert term_obs.is_contiguous() and term_obs.device == self.device, "term_obs must be a contiguous device tensor"
-        self._term_keepalive = term_obs
-        _lib.check(self._L.madrl_pursuit_set_terminal_obs(self._h, _ptr(term_obs)))
-
-    def set_launch(self, warps_per_block=0, blocks_per_sm=0):
-        _lib.check(self._L.madrl_pursuit_set_launch(self._h, warps_per_block, blocks_per_sm))
-
     def set_params(self, catchr=None, constraint_window=None):
         """Curriculum updates (pursuit_evade.py:264-272)."""
         if catchr is not None:
@@ -128,52 +105,6 @@ class BatchedPursuitEvade(object):
         if constraint_window is not None:
             self.cfg.constraint_window = float(constraint_window)
         _lib.check(self._L.madrl_pursuit_set_params(self._h, self.cfg.catchr, self.cfg.constraint_window))
-
-    def seed(self, seed=None):
-        s = 0 if seed is None else int(seed)
-        with torch.cuda.device(self.device):
-            _lib.check(self._L.madrl_pursuit_seed(self._h, s, self._stream()))
-        return [seed]
-
-    def reset(self, mask=None, out=None):
-        E, Np, D = self.n_envs, self.n_pursuers, self.obs_dim
-        obs = out if out is not None else torch.zeros((E, Np, D), dtype=torch.float32, device=self.device)
-        if out is not None:
-            _lib.require_tensor(out, "out", torch.float32, (E, Np, D), self.device)
-        if mask is not None:
-            mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
-        with torch.cuda.device(self.device):
-            _lib.check(self._L.madrl_pursuit_reset(self._h, _ptr(mask), _ptr(obs), self._stream()))
-        return obs
-
-    def _require_outputs(self, T, out, device):
-        """dtype / shape / contiguity / placement of caller-supplied trajectory buffers."""
-        obs, rew, done, info = out
-        E, A, D = self.n_envs, self.n_pursuers, self.obs_dim
-        _lib.require_tensor(obs, "obs", torch.float32, (T, E, A, D), device)
-        _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), device)
-        _lib.require_tensor(done, "done", torch.uint8, (T, E), device)
-        _lib.require_tensor(info, "info", torch.int32, (T, E) + (), device)
-        return obs, rew, done, info
-
-    def rollout(self, actions, auto_reset=True, out=None):
-        """actions int32 [T, E, Np] -> (obs [T,E,Np,D] f32, rew [T,E,Np] f32, done [T,E] u8,
-        removed [T,E] i32)."""
-        actions = actions.to(device=self.device, dtype=torch.int32).contiguous()
-        T = actions.shape[0]
-        E, Np, D = self.n_envs, self.n_pursuers, self.obs_dim
-        assert actions.shape == (T, E, Np), actions.shape
-        if out is None:
-            obs = torch.empty((T, E, Np, D), dtype=torch.float32, device=self.device)
-            rew = torch.empty((T, E, Np), dtype=torch.float32, device=self.device)
-            done = torch.empty((T, E), dtype=torch.uint8, device=self.device)
-            info = torch.empty((T, E), dtype=torch.int32, device=self.device)
-        else:
-            obs, rew, done, info = self._require_outputs(T, out, self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self._L.madrl_pursuit_rollout(self._h, T, _ptr(actions), _ptr(obs), _ptr(rew),
-                                                     _ptr(done), _ptr(info), int(auto_reset), self._stream()))
-        return obs, rew, done, info
 
     def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, py2_division=True,
                           actions_out=None):
@@ -184,51 +115,11 @@ class BatchedPursuitEvade(object):
         the previous rollout).  `py2_division`: the window centre `xs / 2` (heuristics/pursuit.py:23) as
         Python 2 -- the reference's language -- computes it (R // 2); False = Python 3 true division.
         Returns (actions int32 [T,E,Np] or None, obs, rew, done, removed)."""
-        E, Np, D = self.n_envs, self.n_pursuers, self.obs_dim
-        _lib.require_tensor(obs0, "obs0", torch.float32, (E, Np, D), self.device)
-        if out is None:
-            obs = torch.empty((T, E, Np, D), dtype=torch.float32, device=self.device)
-            rew = torch.empty((T, E, Np), dtype=torch.float32, device=self.device)
-            done = torch.empty((T, E), dtype=torch.uint8, device=self.device)
-            info = torch.empty((T, E), dtype=torch.int32, device=self.device)
-        else:
-            obs, rew, done, info = self._require_outputs(T, out, self.device)
-        if actions_out is not None:   # caller-owned buffer for the actions taken (no allocation in a rollout loop)
-            act = _lib.require_tensor(actions_out, "actions_out", torch.int32, (T, E, Np), self.device)
-        else:
-            act = torch.empty((T, E, Np), dtype=torch.int32, device=self.device) if record_actions else None
-        with torch.cuda.device(self.device):
-            _lib.check(self._L.madrl_pursuit_rollout_heuristic(
-                self._h, T, _ptr(obs0), _ptr(act), _ptr(obs), _ptr(rew), _ptr(done), _ptr(info), int(auto_reset),
-                int(bool(py2_division)), self._stream()))
-        return act, obs, rew, done, info
-
-    def step(self, actions, auto_reset=False):
-        a = torch.as_tensor(actions, device=self.device).to(torch.int32).reshape(1, self.n_envs, self.n_pursuers)
-        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset)
-        return obs[0], rew[0], done[0], dict(removed=info[0])
-
-    def rollout_host(self, actions, obs, rew, done, info, auto_reset=True, obs_last=False):
-        """rollout() with HOST tensors (pinned for full PCIe speed); the copies are inside the call,
-        chunked and overlapped with the compute (csrc/host_pipeline.cuh).  `obs_last=True`: only the last
-        step's observations come back (obs is [E, A, D]) -- the policy-on-device mode."""
-        T = actions.shape[0]
-        E, A, D = self.n_envs, self.n_pursuers, self.obs_dim
-        _lib.require_tensor(actions, "actions", torch.int32, (T, E) + (self.n_pursuers,), 'cpu')
-        _lib.require_tensor(obs, "obs", torch.float32, (E, A, D) if obs_last else (T, E, A, D), 'cpu')
-        _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), 'cpu')
-        _lib.require_tensor(done, "done", torch.uint8, (T, E), 'cpu')
-        _lib.require_tensor(info, "info", torch.int32, (T, E) + (), 'cpu')
-        with torch.cuda.device(self.device):
-            _lib.check(self._L.madrl_pursuit_rollout_host2(self._h, T, _ptr(actions), _ptr(obs), _ptr(rew), _ptr(done),
-                                                      _ptr(info), int(auto_reset), 1 if obs_last else 0))
-        return obs, rew, done, info
+        return self._rollout_heuristic(T, obs0, auto_reset, out, record_actions, actions_out, int(bool(py2_division)))
 
 
-class PursuitEvade(AbstractMAEnv, EzPickle):
+class PursuitEvade(DropInEnv):
     """Drop-in for the reference class: ``PursuitEvade(map_pool, **kwargs)``."""
-
-    vectorized = True
 
     def __init__(self, map_pool, **kwargs):
         EzPickle.__init__(self, map_pool, **kwargs)
@@ -276,37 +167,25 @@ class PursuitEvade(AbstractMAEnv, EzPickle):
         self.act_dims = [5 for _ in range(self.n_pursuers)]
         self.setup()
 
-    def _ctor_params(self):
-        return dict(n_evaders=self.n_evaders, n_pursuers=self.n_pursuers, obs_range=self.obs_range,
-                    flatten=self.flatten, layer_norm=self.layer_norm, n_catch=self.n_catch,
-                    catchr=self.catchr, term_pursuit=self.term_pursuit,
-                    urgency_reward=self.urgency_reward, include_id=self.include_id,
-                    surround=self.surround, constraint_window=self.constraint_window,
-                    sample_maps=self.sample_maps, reward_mech=self._reward_mech,
-                    random_opponents=self.random_opponents, max_opponents=self.max_opponents)
+    def _make_engine(self, n_envs, **kw):
+        # looks up the module-level class at call time, so that a test double can stand in for it
+        return BatchedPursuitEvade(n_envs, self.map_pool, n_evaders=self.n_evaders, n_pursuers=self.n_pursuers,
+                                   obs_range=self.obs_range, flatten=self.flatten, layer_norm=self.layer_norm,
+                                   n_catch=self.n_catch, catchr=self.catchr, term_pursuit=self.term_pursuit,
+                                   urgency_reward=self.urgency_reward, include_id=self.include_id,
+                                   surround=self.surround, constraint_window=self.constraint_window,
+                                   sample_maps=self.sample_maps, reward_mech=self._reward_mech,
+                                   random_opponents=self.random_opponents, max_opponents=self.max_opponents,
+                                   seed=self._seed_value, **self._engine_kwargs, **kw)
 
     def setup(self):
         self.pursuers = [DiscreteAgent(self.obs_range, flatten=self.flatten) for _ in range(self.n_pursuers)]
-        self._engine = BatchedPursuitEvade(1, self.map_pool, seed=self._seed_value,
-                                           env_id_base=self._env_id, **self._ctor_params(),
-                                           **self._engine_kwargs)
+        super().setup()
         self._n_live = self.n_evaders
 
     @property
     def agents(self):
         return self.pursuers
-
-    @property
-    def reward_mech(self):
-        return self._reward_mech
-
-    def seed(self, seed=None):
-        self._seed_value = 0 if seed is None else int(seed)
-        self._engine.seed(self._seed_value)
-        return [seed]
-
-    def get_param_values(self):
-        return self.__dict__
 
     def n_agents(self):
         return self.n_pursuers
@@ -367,7 +246,3 @@ class PursuitEvade(AbstractMAEnv, EzPickle):
         self.n_pursuers = d['n_pursuers']
         self.catchr = d['catchr']
         self.setup()
-
-    def vec_env_executor(self, n_envs, max_path_length):
-        from .vec_executor import PursuitVecExecutor
-        return PursuitVecExecutor(self, n_envs, max_path_length)

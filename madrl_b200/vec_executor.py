@@ -1,4 +1,4 @@
-"""GPU-batched stand-ins for rllab's ``VecEnvExecutor``
+"""GPU-batched stand-in for rllab's ``VecEnvExecutor``
 (rllab/sandbox/rocky/tf/envs/vec_env_executor.py:8-48): same methods and return types
 (``reset() -> list``, ``step(action_n) -> (obs list, rewards ndarray, dones ndarray,
 env_infos dict of arrays)``, ``num_envs``, ``action_space``, ``observation_space``,
@@ -7,16 +7,20 @@ env_infos dict of arrays)``, ``num_envs``, ``action_space``, ``observation_space
 import numpy as np
 import torch
 
+from .spaces import Discrete
 
-class _BatchedVecExecutor(object):
-    info_keys = ()
 
-    def __init__(self, proto_env, engine, n_envs, max_path_length):
+class BatchedVecExecutor(object):
+    """`n_envs` copies of the drop-in env `proto_env` on one batched engine (the env's `_make_engine`)."""
+
+    def __init__(self, proto_env, n_envs, max_path_length):
         self._proto = proto_env
-        self._engine = engine
+        self._engine = proto_env._make_engine(n_envs, max_path_length=max_path_length)
         self._n = n_envs
         self.max_path_length = max_path_length
         self.ts = np.zeros(n_envs, dtype='int')
+        # discrete moves (Pursuit) are int32, continuous ones float64 until the engine casts them to its dtype
+        self._act_dtype = np.int32 if isinstance(self.action_space, Discrete) else np.float64
 
     @property
     def num_envs(self):
@@ -35,11 +39,10 @@ class _BatchedVecExecutor(object):
         self.ts[:] = 0
         return [obs[i] for i in range(self._n)]
 
-    def _actions(self, action_n):
-        raise NotImplementedError
-
     def step(self, action_n):
-        obs, rew, done, info = self._engine.step(self._actions(action_n), auto_reset=True)
+        # engine.step reshapes the actions to [n_envs, agents, *action shape]
+        a = torch.as_tensor(np.asarray(action_n, dtype=self._act_dtype))
+        obs, rew, done, info = self._engine.step(a, auto_reset=True)
         obs = obs.cpu().numpy().astype(np.float64)
         dones = done.cpu().numpy().astype(bool)
         self.ts += 1
@@ -49,39 +52,3 @@ class _BatchedVecExecutor(object):
 
     def terminate(self):
         pass
-
-
-class WaterworldVecExecutor(_BatchedVecExecutor):
-    def __init__(self, proto_env, n_envs, max_path_length):
-        from .waterworld import BatchedMAWaterWorld
-        eng = BatchedMAWaterWorld(n_envs, seed=proto_env._seed_value, max_path_length=max_path_length,
-                                  **proto_env._ctor_params(), **proto_env._engine_kwargs)
-        super().__init__(proto_env, eng, n_envs, max_path_length)
-
-    def _actions(self, action_n):
-        a = np.asarray(action_n, dtype=np.float64).reshape(self._n, self._proto.n_pursuers, 2)
-        return torch.as_tensor(a)
-
-
-class PursuitVecExecutor(_BatchedVecExecutor):
-    def __init__(self, proto_env, n_envs, max_path_length):
-        from .pursuit import BatchedPursuitEvade
-        eng = BatchedPursuitEvade(n_envs, proto_env.map_pool, seed=proto_env._seed_value,
-                                  max_path_length=max_path_length, **proto_env._ctor_params(),
-                                  **proto_env._engine_kwargs)
-        super().__init__(proto_env, eng, n_envs, max_path_length)
-
-    def _actions(self, action_n):
-        return torch.as_tensor(np.asarray(action_n, dtype=np.int32).reshape(self._n, self._proto.n_pursuers))
-
-
-class HostageVecExecutor(_BatchedVecExecutor):
-    def __init__(self, proto_env, n_envs, max_path_length):
-        from .hostage import BatchedHostageWorld
-        eng = BatchedHostageWorld(n_envs, seed=proto_env._seed_value, max_path_length=max_path_length,
-                                  **proto_env._ctor_params(), **proto_env._engine_kwargs)
-        super().__init__(proto_env, eng, n_envs, max_path_length)
-
-    def _actions(self, action_n):
-        a = np.asarray(action_n, dtype=np.float64).reshape(self._n, self._proto.n_good, 2)
-        return torch.as_tensor(a)

@@ -1,13 +1,18 @@
 """TEST INFRASTRUCTURE: ctypes drivers for the warp-emulator build of the kernels
 (tests/emu/build_emu.py).  The emulator library exports the product's C ABI; "device" pointers are
-host pointers, so the entry points are called directly with NumPy arrays.  Argument names and
-defaults mirror madrl_b200.{waterworld,pursuit,hostage}.Batched* so the tests read like the GPU ones.
+host pointers, so the entry points are called directly with NumPy arrays.  The engines take the
+arguments of madrl_b200.{waterworld,pursuit,hostage}.Batched* and build their config structs with the
+same functions (ww_config / pe_config / hw_config), so the tests read like the GPU ones and check the
+product's argument mapping.
 """
 import ctypes as C
 
 import numpy as np
 
 from madrl_b200 import _lib as L
+from madrl_b200.hostage import hw_config
+from madrl_b200.pursuit import map_pool_array, pe_config
+from madrl_b200.waterworld import ww_config
 
 from . import build_emu
 
@@ -35,24 +40,9 @@ def races(reset=True):
 
 
 def _declare(lib):
-    vp, i32, u64 = C.c_void_p, C.c_int, C.c_uint64
+    L._declare_engines(lib)
     lib.madrl_last_error.restype = C.c_char_p
     lib.madrl_emu_race_count.restype = C.c_long
-    for fam, cfg, lay in (("ww", L.WWConfig, L.WWLayout), ("hostage", L.HWConfig, L.HWLayout),
-                          ("pursuit", L.PEConfig, L.PELayout)):
-        g = lambda n: getattr(lib, "madrl_%s_%s" % (fam, n))   # noqa: E731
-        g("state_layout").argtypes = [C.POINTER(cfg), C.POINTER(lay)]
-        g("create").argtypes = [C.POINTER(cfg), vp, vp, C.POINTER(vp)] if fam == "pursuit" else \
-            [C.POINTER(cfg), vp, C.POINTER(vp)]
-        g("destroy").argtypes = [vp]
-        g("seed").argtypes = [vp, u64, vp]
-        g("set_launch").argtypes = [vp, i32, i32]
-        g("reset").argtypes = [vp, vp, vp, vp]
-        g("rollout").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp]
-        g("rollout_host").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32]
-        g("reset_host").argtypes = [vp, vp, vp]
-    lib.madrl_ww_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
-    lib.madrl_pursuit_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
 
 
 def _p(a):
@@ -175,27 +165,13 @@ def pursuit_heuristic_actions(obs, obs_range, flatten, fallback, py2_division=Tr
 class EmuWaterworld(_Engine):
     fam, LayoutT, info_shape, act_shape = "ww", L.WWLayout, (2,), (2,)
 
-    def __init__(self, n_envs, n_pursuers, n_evaders, n_coop=2, n_poison=10, radius=0.015,
-                 obstacle_radius=0.2, obstacle_loc=np.array([0.5, 0.5]), ev_speed=0.01,
-                 poison_speed=0.01, n_sensors=30, sensor_range=0.2, action_scale=0.01,
-                 poison_reward=-1., food_reward=1., encounter_reward=.05, control_penalty=-.5,
-                 reward_mech='local', addid=True, speed_features=True, seed=0, env_id_base=0,
-                 max_path_length=0, fp64=True, defines=()):
+    def __init__(self, n_envs, *args, fp64=True, defines=(), **kw):
+        """The arguments of BatchedMAWaterWorld (without device / dtype)."""
         self.lib = load(defines)
-        self.n_envs, self.n_agents, self.n_pursuers, self.n_evaders = n_envs, n_pursuers, n_pursuers, n_evaders
+        self.cfg = ww_config(n_envs, *args, fp64=fp64, **kw)
+        self.n_envs, self.n_pursuers, self.n_evaders = n_envs, self.cfg.n_pursuers, self.cfg.n_evaders
+        self.n_agents = self.n_pursuers
         self.obs_dtype = self.act_dtype = np.float64 if fp64 else np.float32
-        rand = obstacle_loc is None
-        ox, oy = (0.0, 0.0) if rand else (float(obstacle_loc[0]), float(obstacle_loc[1]))
-        self.cfg = L.WWConfig(
-            n_envs=n_envs, env_id_base=env_id_base, n_pursuers=n_pursuers, n_evaders=n_evaders,
-            n_poison=n_poison, n_sensors=n_sensors, n_coop=n_coop,
-            reward_global=int(reward_mech == 'global'), addid=int(bool(addid)),
-            speed_features=int(bool(speed_features)), random_obstacle=int(rand), timestep_limit=1000,
-            max_path_length=int(max_path_length or 0), fp64=int(fp64), radius=radius,
-            obstacle_radius=obstacle_radius, obstacle_x=ox, obstacle_y=oy, ev_speed=ev_speed,
-            poison_speed=poison_speed, sensor_range=sensor_range, action_scale=action_scale,
-            poison_reward=poison_reward, food_reward=food_reward, encounter_reward=encounter_reward,
-            control_penalty=control_penalty, seed=int(seed))
         self._finish(())
 
     def state(self, e):
@@ -212,27 +188,12 @@ class EmuWaterworld(_Engine):
 class EmuHostage(_Engine):
     fam, LayoutT, info_shape, act_shape = "hostage", L.HWLayout, (2,), (2,)
 
-    def __init__(self, n_envs, n_good, n_hostages, n_bad, n_coop_save, n_coop_avoid, radius=0.015,
-                 key_loc=None, bad_speed=0.01, n_sensors=30, sensor_range=0.2, action_scale=0.01,
-                 save_reward=5., hit_reward=-1., encounter_reward=0.01, not_saved_reward=-3,
-                 bomb_reward=-5., bomb_radius=0.05, key_radius=0.0075, control_penalty=-.1,
-                 reward_mech='global', addid=True, seed=0, env_id_base=0, max_path_length=0, fp64=True,
-                 defines=()):
+    def __init__(self, n_envs, *args, fp64=True, defines=(), **kw):
+        """The arguments of BatchedHostageWorld (without device / dtype)."""
         self.lib = load(defines)
-        self.n_envs, self.n_agents, self.n_hostages = n_envs, n_good, n_hostages
+        self.cfg = hw_config(n_envs, *args, fp64=fp64, **kw)
+        self.n_envs, self.n_agents, self.n_hostages = n_envs, self.cfg.n_good, self.cfg.n_hostages
         self.obs_dtype = self.act_dtype = np.float64 if fp64 else np.float32
-        rand_key = key_loc is None
-        kx, ky = (0.0, 0.0) if rand_key else [float(v) for v in np.asarray(key_loc).reshape(-1)[:2]]
-        self.cfg = L.HWConfig(
-            n_envs=n_envs, env_id_base=env_id_base, n_good=n_good, n_hostages=n_hostages, n_bad=n_bad,
-            n_coop_save=n_coop_save, n_coop_avoid=n_coop_avoid, n_sensors=n_sensors,
-            reward_global=int(reward_mech == 'global'), addid=int(bool(addid)), random_key=int(rand_key),
-            timestep_limit=1000, max_path_length=int(max_path_length or 0), fp64=int(fp64), radius=radius,
-            key_x=kx, key_y=ky, bad_speed=bad_speed, sensor_range=float(sensor_range),
-            action_scale=action_scale, save_reward=save_reward, hit_reward=hit_reward,
-            encounter_reward=encounter_reward, not_saved_reward=float(not_saved_reward),
-            bomb_reward=bomb_reward, bomb_radius=bomb_radius, key_radius=key_radius,
-            control_penalty=control_penalty, seed=int(seed))
         self._finish(())
 
     def state(self, e):
@@ -247,27 +208,14 @@ class EmuPursuit(_Engine):
     fam, LayoutT, info_shape, act_shape = "pursuit", L.PELayout, (), ()
     obs_dtype, act_dtype = np.float32, np.int32
 
-    def __init__(self, n_envs, map_pool, n_evaders=1, n_pursuers=1, obs_range=3, flatten=True,
-                 layer_norm=10, n_catch=2, catchr=0.01, term_pursuit=5.0, urgency_reward=0.0,
-                 include_id=True, surround=True, constraint_window=1.0, sample_maps=False,
-                 reward_mech='global', random_opponents=False, max_opponents=10, seed=0, env_id_base=0,
-                 max_path_length=0, defines=()):
+    def __init__(self, n_envs, map_pool, *args, defines=(), **kw):
+        """The arguments of BatchedPursuitEvade (without device)."""
         self.lib = load(defines)
-        mp = np.ascontiguousarray(np.asarray(map_pool), dtype=np.int32)
-        if mp.ndim == 2:
-            mp = mp[None]
-        self.map_pool = mp
-        self.n_envs, self.n_agents, self.n_pursuers, self.n_evaders = n_envs, n_pursuers, n_pursuers, n_evaders
-        self.cfg = L.PEConfig(
-            n_envs=n_envs, env_id_base=env_id_base, n_pursuers=n_pursuers, n_evaders=n_evaders,
-            xs=mp.shape[1], ys=mp.shape[2], n_maps=mp.shape[0], obs_range=obs_range,
-            flatten=int(bool(flatten)), n_catch=n_catch, surround=int(bool(surround)),
-            reward_global=int(reward_mech == 'global'), include_id=int(bool(include_id)),
-            sample_maps=int(bool(sample_maps)), max_path_length=int(max_path_length or 0),
-            max_opponents=int(max_opponents) if random_opponents else 0,
-            layer_norm=float(layer_norm), catchr=float(catchr), term_pursuit=float(term_pursuit),
-            urgency_reward=float(urgency_reward), constraint_window=float(constraint_window), seed=int(seed))
-        self._finish((_p(mp),))
+        self.map_pool = map_pool_array(map_pool)
+        self.cfg = pe_config(n_envs, self.map_pool, *args, **kw)
+        self.n_envs, self.n_pursuers, self.n_evaders = n_envs, self.cfg.n_pursuers, self.cfg.n_evaders
+        self.n_agents = self.n_pursuers
+        self._finish((_p(self.map_pool),))
 
     def state(self, e):
         Ly, E, Np = self.layout, self.n_envs, self.n_pursuers
@@ -331,9 +279,7 @@ def _pe_facade(n_envs, map_pool, device=None, **kw):
     f._act_tail = (f.emu.n_pursuers,)
 
     def set_params(catchr, constraint_window):
-        lib = f.emu.lib
-        lib.madrl_pursuit_set_params.argtypes = [C.c_void_p, C.c_double, C.c_double]
-        f.emu._check(lib.madrl_pursuit_set_params(f.emu._h, float(catchr), float(constraint_window)))
+        f.emu._check(f.emu.lib.madrl_pursuit_set_params(f.emu._h, float(catchr), float(constraint_window)))
     f.set_params = set_params
     import torch
     type(f).state = property(lambda self: {'gone': torch.tensor([self.emu.state(e)['gone'] for e in range(self.n_envs)])})

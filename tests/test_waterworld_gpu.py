@@ -188,7 +188,7 @@ def test_sharding_is_invisible_and_launch_geometry_is_irrelevant():
     half = E // 2
     for base in (0, half):
         sh = make(cfg, half, torch.float32, seed=7, env_id_base=base)
-        sh.set_launch(warps_per_block=3, blocks_per_sm=1)  # multi-env-per-warp path
+        sh.set_launch(warps_per_block=3, blocks_per_sm=1)  # override accepted; warps_per_block is ignored
         sh.reset()
         out = [x.cpu() for x in sh.rollout(act[:, base:base + half].contiguous())]
         for a, b in zip(ref, out):
