@@ -69,7 +69,7 @@ __device__ __forceinline__ real warp_allreduce_sum(real v) {
 // engine.cuh).  The env index then derives from blockIdx alone, so ptxas can prove the persistent loop
 // and every branch on warp-uniform values uniform: the BRA.DIV guards in front of the warp collectives
 // disappear, loop bookkeeping moves to the uniform datapath and the register count drops (Waterworld
-// C2: 72 regs + spills -> 56, none).
+// C2: 72 regs + spills -> 63, none: 32 resident one-warp blocks per SM, the hardware's block limit).
 
 // Kernels are launched through one macro and the PTX-level helpers below sit behind one guard so
 // that the test-only warp emulator (tests/emu: the kernels compiled by g++ against a fake
@@ -155,6 +155,63 @@ template <> struct CandSlot<double> {
 
 // Pull a line towards L1/L2 without occupying a register (next step's action).
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
+
+// Rows staged in shared memory leave through TMA bulk stores (cp.async.bulk, issued by one lane).
+// The lanes that wrote the rows fence their shared stores into the async proxy and sync
+// with the issuing lane; the issuer waits for the group to have READ its source before the buffer is
+// refilled, and for full completion before anything rewrites or re-reads the same global bytes.
+__device__ __forceinline__ void sts_real(uint32_t a, float v) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory"); }
+__device__ __forceinline__ void sts_real(uint32_t a, double v) { asm volatile("st.shared.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+template <typename real> __device__ __forceinline__ real lds_real(uint32_t a);
+template <> __device__ __forceinline__ float lds_real<float>(uint32_t a) { return lds_f32(a); }
+template <> __device__ __forceinline__ double lds_real<double>(uint32_t a) {
+  double v;
+  asm volatile("ld.shared.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void fence_async_shared() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// `bytes` (a multiple of 16) from shared `src` to global `dst` (both 16-byte aligned) as one bulk group,
+// L2 evict-first like store_stream.
+__device__ __forceinline__ void bulk_store_stream(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("{ .reg .b64 pol;\n\t"
+               "createpolicy.fractional.L2::evict_first.b64 pol, 1.0;\n\t"
+               "cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, pol;\n\t"
+               "cp.async.bulk.commit_group; }" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
+// Every bulk group / all but the most recent one have finished reading their shared source.
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_read_all_but_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
+// Every bulk group has completed, and its global writes are ordered before this thread's later
+// generic-proxy accesses.
+__device__ __forceinline__ void bulk_wait_all() {
+  asm volatile("cp.async.bulk.wait_group 0;\n\tfence.proxy.async.global;" ::: "memory");
+}
+#else   // MADRL_EMU_PTX_HELPERS
+// Host versions of the bulk-store helpers above for the test emulator, built on the shared-memory
+// primitives its <cuda_runtime.h> provides (emu_at, smem_access: the per-byte race checker).  The
+// copy happens at issue, recorded as a shared read by the issuing lane, so refilling a staging buffer
+// without a __syncwarp after the issue is reported as a race; the waits and fences are no-ops.  The
+// alignment cp.async.bulk requires (16-byte addresses and size) is checked.
+static inline void sts_real(uint32_t a, float v) { smem_access(a, 4, SMEM_WRITE); memcpy(emu_at(a), &v, 4); }
+static inline void sts_real(uint32_t a, double v) { smem_access(a, 8, SMEM_WRITE); memcpy(emu_at(a), &v, 8); }
+template <typename real> static inline real lds_real(uint32_t a) {
+  smem_access(a, sizeof(real), SMEM_READ);
+  real v;
+  memcpy(&v, emu_at(a), sizeof v);
+  return v;
+}
+static inline void fence_async_shared() {}
+static inline void bulk_store_stream(void* dst, uint32_t src, uint32_t bytes) {
+  if (((uintptr_t)dst | src | bytes) & 15u) {
+    fprintf(stderr, "madrl_emu: misaligned bulk store dst=%p src=%u bytes=%u\n", dst, src, bytes);
+    abort();
+  }
+  smem_access(src, bytes, SMEM_READ);
+  memcpy(dst, emu_at(src), bytes);
+}
+static inline void bulk_wait_read_all() {}
+static inline void bulk_wait_read_all_but_1() {}
+static inline void bulk_wait_all() {}
 #endif  // MADRL_EMU_PTX_HELPERS
 
 // StandardizedEnv sees the TERMINAL observation of an episode before the reset one

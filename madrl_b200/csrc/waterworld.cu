@@ -5,16 +5,16 @@
 // Design (see DESIGN.md):
 //   * One WARP owns one env for the WHOLE T-step rollout.  The env's state lives in REGISTERS:
 //     lane l holds objects l, l+32, ... (position + velocity); objects are ordered pursuers,
-//     evaders, poisons.  There is no shared memory and no block barrier anywhere: warps are
-//     completely independent, so the SM's schedulers overlap the phases of different envs.
-//     HBM sees the state once per launch (a coalesced per-env record) and, per step, only
-//     actions in and obs / reward / done / info out.
+//     evaders, poisons.  There is no block barrier anywhere (blocks are one warp, and shared memory
+//     is the warp's own): warps are completely independent, so the SM's schedulers overlap the
+//     phases of different envs.  HBM sees the state once per launch (a coalesced per-env record)
+//     and, per step, only actions in and obs / reward / done / info out.
 //   * Per step and pursuer, lanes act first as OBJECTS (relative position, squared distance,
 //     collision test and exact conservative range cull, all reduced with __ballot_sync), then as
 //     SENSORS (lane k = sensor k) looping over the few surviving candidates, whose geometry is
 //     broadcast with __shfl_sync; nearest-object-per-sensor keeps the lowest index among equal
-//     minima (np.argmin).  The 7 feature rows of the pursuer are stored as coalesced
-//     feature-major runs straight from registers.
+//     minima (np.argmin).  The pursuer's feature values are staged in shared memory and leave,
+//     with the env-step's other rows or on their own, as TMA bulk stores (obs_row_stage).
 //   * sqrt-free thresholds: every `cdist(...) <= thr` of the reference is evaluated as
 //     d2 <= thr2 with thr2 the largest representable value whose correctly-rounded sqrt is
 //     <= thr (computed on the host), which is exactly equivalent.
@@ -34,6 +34,7 @@ struct WWParams {
   int E, env_id_base, Np, Ne, Npo, K, n_coop, D, Nall;
   int reward_global, addid, speed_features, random_obstacle, timestep_limit, max_path_length;
   int T, mode, auto_reset;  // mode 0 = rollout, 1 = reset
+  int stage_step;            // observation staging: 1 = the env-step's Np rows at once, 0 = row by row (obs_row_stage)
   // element strides of one lockstep step in the trajectory tensors (host-computed so that the
   // per-step pointer bumps are plain 64-bit adds on constant-bank operands)
   size_t obs_step, agent_step;   // E*Np*D and E*Np
@@ -111,9 +112,61 @@ __device__ __noinline__ Spawn<real> spawn_object(uint64_t seed, uint32_t env_id,
   return s;
 }
 
+// Observation rows leave through shared memory (after the candidate slots) and TMA bulk stores.  When an
+// env-step's Np rows fit (stage_step), they are staged together, tail triples included, and leave as one
+// bulk store at the end of the step.  Otherwise each row's feature values go through a two-slot ring:
+// while one slot's bulk store still reads its source, the next row is staged in the other, and the tail
+// triple, known only after every pursuer has sensed, is stored directly.  n values are staged at the
+// global address modulo 16, so that their 16-byte-aligned global interior and its shared source are
+// both 16-byte aligned; hence the 16 bytes of slack.
+__host__ __device__ __forceinline__ uint32_t obs_stage_bytes(int n, int real_bytes) {
+  return (((uint32_t)n * (uint32_t)real_bytes + 15u) & ~15u) + 16u;
+}
+// Staging an env-step keeps 32 one-warp blocks per SM: 32 x (6 KB + the 1 KB reserved per block) fit
+// the H100's 227 KB of shared memory per SM.
+constexpr size_t kStepStageMaxBytes = 6 * 1024;
+
+// Shared address of element 0 of `row` (a row of the env-step starting at `obs_t`), after waiting for
+// the bulk store that last read that memory: the previous step's (whole-step staging, first row of
+// the step) or the one two rows ago (ring slot `slot_off`).
+template <typename real>
+__device__ __forceinline__ uint32_t obs_row_stage(bool whole_step, uint32_t stage, uint32_t slot_off,
+                                                  const real* obs_t, const real* row, int lane) {
+  if (whole_step) {
+    if (row == obs_t) {
+      if (lane == 0) bulk_wait_read_all();
+      __syncwarp();
+    }
+    return stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)((row - obs_t) * sizeof(real));
+  }
+  if (lane == 0) bulk_wait_read_all_but_1();
+  __syncwarp();
+  return stage + slot_off + ((uint32_t)(uintptr_t)row & 15u);
+}
+
+// The n values staged at `slot` -> global `row`: the 16-byte-aligned interior as one bulk store
+// (HBM then sees whole sectors from one writer), the <= 16 bytes outside it on either side by
+// direct stores of one lane per element.  Full writes, no read-back, so the rows are bit-identical
+// to per-lane stores.
+template <typename real>
+__device__ __forceinline__ void obs_row_store(uint32_t slot, real* row, int n, int lane) {
+  fence_async_shared();   // this lane's shared stores -> visible to the async proxy ...
+  __syncwarp();           // ... before lane 0 issues the copy; the edge lanes read other lanes' values
+  const uintptr_t g0 = (uintptr_t)row, g1 = g0 + (uintptr_t)n * sizeof(real);
+  const uintptr_t a0 = (g0 + 15u) & ~(uintptr_t)15u, a1 = g1 & ~(uintptr_t)15u;
+  const bool bulk = a1 > a0;
+  if (lane == 0 && bulk) bulk_store_stream((void*)a0, slot + (uint32_t)(a0 - (g0 & ~(uintptr_t)15u)), (uint32_t)(a1 - a0));
+  const int head = bulk ? (int)((a0 - g0) / sizeof(real)) : n;
+  const int tail = bulk ? (int)((g1 - a1) / sizeof(real)) : 0;
+  if (lane < head + tail) {
+    const int i = lane < head ? lane : n - tail + (lane - head);
+    store_stream(row + i, lds_real<real>(slot + ((uint32_t)g0 & 15u) + (uint32_t)(i * sizeof(real))));
+  }
+}
+
 // OPL = objects per lane (ceil(n_obj / 32)); KCH = sensors per lane (ceil(K / 32));
 // KC = compile-time sensor count (0 = runtime p.K): with KC known the 7 feature-row stores of a
-// pursuer use immediate offsets from one running pointer instead of 64-bit address arithmetic.
+// pursuer use immediate offsets from one shared address.
 // PEER = compile the fused multi-GPU exchange in (a separate instantiation, so the single-GPU kernel
 // carries none of its registers).
 // POLICY = the actions come from the in-kernel heuristic policy instead of the action tensor (again a
@@ -133,8 +186,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
   constexpr bool SMEM = OPL >= 2;
   const unsigned lt_mask = lanemask_lt();
   extern __shared__ __align__(16) unsigned char ww_smem[];
-  // this warp's candidate slots (32-bit shared address)
-  uint32_t slots = SMEM ? smem_addr(ww_smem) : 0u;
+  // this warp's candidate slots (OPL >= 2), then its observation staging (32-bit shared address)
+  uint32_t slots = smem_addr(ww_smem);
   asm volatile("" : "+r"(slots));   // keep it in a register: ptxas otherwise re-derives it from SR_CgaCtaId at every use
 
   // ---- per-lane constants: this lane as OBJECT (classes, thresholds) and as SENSOR -----------
@@ -161,6 +214,9 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
   // per sensor): no layout branch per pursuer; every other combination takes the KC = 0 instantiation
   const bool speed = KC > 0 ? true : (p.speed_features != 0);
   const int n_feat = speed ? 7 : 4;
+  const uint32_t stage = slots + (SMEM ? (uint32_t)Nall * CandSlot<real>::kStride : 0u);
+  const uint32_t slot_bytes = obs_stage_bytes(n_feat * K, sizeof(real));
+  uint32_t slot_off = 0u;   // row-by-row staging: ring slot of the next row, 0 or slot_bytes
   typedef typename Vec2<real>::type V2;
 
   for (int e = warp_global; e < p.E; e += warp_stride) {
@@ -184,8 +240,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
     int tt = p.timestep[e], ts = p.path_len[e];
     uint64_t ctr = p.ctr[e];
 
-    // running output pointers (this lane's column of the env's first pursuer row at step t)
-    real* obs_t = p.obs + (size_t)e * p.Np * p.D + lane;
+    // running output pointers: the env's first pursuer row at step t (warp-uniform), this lane's reward
+    real* obs_t = p.obs + (size_t)e * p.Np * p.D;
     real* rew_t = p.rew + (size_t)e * p.Np + lane;
     size_t te = (size_t)e;   // index of (t, e) in the [T][E] done / info tensors
     int pass = (p.mode == 1) ? 1 : 0;  // pass 1 = reset pass: fresh draws, zero action, obs only
@@ -361,6 +417,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
             MADRL_WW_SCAN(endU, endE, bE, aE)
             MADRL_WW_SCAN(endE, endP, bP, aP)
 #undef MADRL_WW_SCAN
+            const uint32_t srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
             for (int kc = 0; kc < KCH; ++kc) {
               const real sx = sx_l[kc], sy = sy_l[kc];
@@ -368,7 +425,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
               const int k = lane + 32 * kc;
               const bool hO = bO[kc] < INF, hE = bE[kc] < up, hP = bP[kc] < up, hU = bU[kc] < up;
               const real z = (real)0;
-              real* o = obs_row + 32 * kc;   // this lane's column
+              const uint32_t o = srow + (uint32_t)(k * sizeof(real));   // this lane's column
+              constexpr uint32_t R = sizeof(real);
               if constexpr (POLICY) {
                 if (k < K) {
                   const real w = (real)0.5 * (hU ? bU[kc] : z) + ((tE ? (real)1.5 : (real)1) * (hE ? bE[kc] : z) - (hO ? bO[kc] : z)) -
@@ -383,19 +441,19 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
                 CandSlot<real>::vel(aP[kc], oPx, oPy);
                 CandSlot<real>::vel(aU[kc], oUx, oUy);
                 if (k < K) {
-                  store_stream(o + 0 * K, hO ? bO[kc] : z);
-                  store_stream(o + 1 * K, hE ? bE[kc] : z);
-                  store_stream(o + 2 * K, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
-                  store_stream(o + 3 * K, hP ? bP[kc] : z);
-                  store_stream(o + 4 * K, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
-                  store_stream(o + 5 * K, hU ? bU[kc] : z);
-                  store_stream(o + 6 * K, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
+                  sts_real(o + 0 * K * R, hO ? bO[kc] : z);
+                  sts_real(o + 1 * K * R, hE ? bE[kc] : z);
+                  sts_real(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
+                  sts_real(o + 3 * K * R, hP ? bP[kc] : z);
+                  sts_real(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
+                  sts_real(o + 5 * K * R, hU ? bU[kc] : z);
+                  sts_real(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
                 }
               } else if (k < K) {
-                store_stream(o + 0 * K, hO ? bO[kc] : z);
-                store_stream(o + 1 * K, hE ? bE[kc] : z);
-                store_stream(o + 2 * K, hP ? bP[kc] : z);
-                store_stream(o + 3 * K, hU ? bU[kc] : z);
+                sts_real(o + 0 * K * R, hO ? bO[kc] : z);
+                sts_real(o + 1 * K * R, hE ? bE[kc] : z);
+                sts_real(o + 2 * K * R, hP ? bP[kc] : z);
+                sts_real(o + 3 * K * R, hU ? bU[kc] : z);
               }
             }
             __syncwarp();   // the next pursuer's staging overwrites the slots
@@ -429,6 +487,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
 #undef MADRL_WW_SCAN
             }
           }
+          const uint32_t srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
           for (int kc = 0; kc < KCH; ++kc) {
             const real sx = sx_l[kc], sy = sy_l[kc];
@@ -436,7 +495,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
             const int k = lane + 32 * kc;
             const bool hO = bO[kc] < INF, hE = bE[kc] < INF, hP = bP[kc] < INF, hU = bU[kc] < INF;
             const real z = (real)0;
-            real* o = obs_row + 32 * kc;   // this lane's column
+            const uint32_t o = srow + (uint32_t)(k * sizeof(real));   // this lane's column
+            constexpr uint32_t R = sizeof(real);
             if constexpr (POLICY) {
               if (k < K) {
                 const real w = (real)0.5 * (hU ? bU[kc] : z) + ((tE ? (real)1.5 : (real)1) * (hE ? bE[kc] : z) - (hO ? bO[kc] : z)) -
@@ -463,21 +523,25 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
                 }
               }
               if (k < K) {
-                store_stream(o + 0 * K, hO ? bO[kc] : z);
-                store_stream(o + 1 * K, hE ? bE[kc] : z);
-                store_stream(o + 2 * K, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
-                store_stream(o + 3 * K, hP ? bP[kc] : z);
-                store_stream(o + 4 * K, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
-                store_stream(o + 5 * K, hU ? bU[kc] : z);
-                store_stream(o + 6 * K, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
+                sts_real(o + 0 * K * R, hO ? bO[kc] : z);
+                sts_real(o + 1 * K * R, hE ? bE[kc] : z);
+                sts_real(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
+                sts_real(o + 3 * K * R, hP ? bP[kc] : z);
+                sts_real(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
+                sts_real(o + 5 * K * R, hU ? bU[kc] : z);
+                sts_real(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
               }
             } else if (k < K) {
-              store_stream(o + 0 * K, hO ? bO[kc] : z);
-              store_stream(o + 1 * K, hE ? bE[kc] : z);
-              store_stream(o + 2 * K, hP ? bP[kc] : z);
-              store_stream(o + 3 * K, hU ? bU[kc] : z);
+              sts_real(o + 0 * K * R, hO ? bO[kc] : z);
+              sts_real(o + 1 * K * R, hE ? bE[kc] : z);
+              sts_real(o + 2 * K * R, hP ? bP[kc] : z);
+              sts_real(o + 3 * K * R, hU ? bU[kc] : z);
             }
           }
+          }
+          if (!p.stage_step) {
+            obs_row_store(stage + slot_off, obs_row, n_feat * K, lane);
+            slot_off = slot_bytes - slot_off;
           }
           if constexpr (POLICY) {   // sum over the sensors; lane pi keeps pursuer pi's next action
             pwx = warp_allreduce_sum(pwx); pwy = warp_allreduce_sum(pwy);
@@ -516,11 +580,20 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
         // ww:411-428 tail of every pursuer's row: [touched an evader, touched a poison, id]; lane i
         // writes pursuer i's.  whoEnc / whoP are exactly the any-collision masks (ww:376, ww:293).
         if (lane < p.Np) {
-          real* tp = obs_t + (size_t)lane * (p.D - 1) + n_feat * K;   // obs_t already carries +lane
-          store_stream(tp, (real)((whoEnc >> lane) & 1u));
-          store_stream(tp + 1, (real)((whoP >> lane) & 1u));
-          if (p.addid) store_stream(tp + 2, (real)(lane + 1));
+          const real vE = (real)((whoEnc >> lane) & 1u), vP = (real)((whoP >> lane) & 1u), id = (real)(lane + 1);
+          const int i = lane * p.D + n_feat * K;
+          if (p.stage_step) {
+            const uint32_t a = stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)(i * sizeof(real));
+            sts_real(a, vE);
+            sts_real(a + (uint32_t)sizeof(real), vP);
+            if (p.addid) sts_real(a + 2 * (uint32_t)sizeof(real), id);
+          } else {
+            store_stream(obs_t + i, vE);
+            store_stream(obs_t + i + 1, vP);
+            if (p.addid) store_stream(obs_t + i + 2, id);
+          }
         }
+        if (p.stage_step) obs_row_store(stage, obs_t, p.Np * p.D, lane);
         if (!pass && lane < p.Np) {
           real r = pen;
           if (p.reward_global) {
@@ -578,8 +651,12 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
           // VecEnvExecutor.step: a done env is reset in place and its obs slot receives the
           // reset observation (rllab/sandbox/rocky/tf/envs/vec_env_executor.py:24-27)
           need_reset = done && p.auto_reset;
+          if (need_reset) {   // the rows' bulk stores must land before they are read back or rewritten by the reset pass
+            if (lane == 0) bulk_wait_all();
+            __syncwarp();
+          }
           if (need_reset && p.term_obs != nullptr)
-            keep_terminal_rows(obs_t - lane, p.term_obs + ((obs_t - lane) - p.obs), p.Np * p.D, lane);
+            keep_terminal_rows(obs_t, p.term_obs + (obs_t - p.obs), p.Np * p.D, lane);
         }
         pass = need_reset ? 1 : 0;
       } while (need_reset);
@@ -603,6 +680,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
       p.timestep[e] = tt; p.path_len[e] = ts; p.ctr[e] = ctr;
     }
   }
+  if (lane == 0) bulk_wait_all();   // the last bulk store has read its source before the block exits
 }
 
 }  // namespace madrl
@@ -697,9 +775,13 @@ extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
+template <typename real>
+static size_t ww_cand_bytes(int opl, int n_obj) { return opl >= 2 ? (size_t)n_obj * CandSlot<real>::kStride : 0; }
+
 template <typename real, int OPL, int KCH, int KC, bool PEER, bool POLICY>
 static int ww_launch_inst2(madrl_ww* h, const WWParams<real>& p, cudaStream_t stream) {
-  const size_t smem = OPL >= 2 ? (size_t)p.Nall * CandSlot<real>::kStride : 0;   // candidate slots
+  const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(real))
+                                                                        : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(real)));
   return engine_launch(h, ww_kernel<real, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p);
 }
 
@@ -769,6 +851,7 @@ static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* ob
   }
 
   const int opl = (p.Nall + 31) / 32, kch = (p.K + 31) / 32;
+  p.stage_step = ww_cand_bytes<real>(opl, p.Nall) + obs_stage_bytes(p.Np * p.D, sizeof(real)) <= kStepStageMaxBytes;
 #define MADRL_WW_CASE(O, KH, KC_) return ww_launch_inst<real, O, KH, KC_>(h, p, stream)
   if (p.K == 30 && p.speed_features) {   // the reference's defaults (n_sensors = 30, speed features): compile-time K and layout
     if (opl == 1) MADRL_WW_CASE(1, 1, 30);

@@ -1,0 +1,131 @@
+"""Waterworld observation write path against the card's streaming-write rate (one GPU command).
+
+    python scripts/ww_write_path.py [--lib NAME=PATH ...] [--rounds R]
+
+Prints the card (name, power limit, SM clock), then times with CUDA events
+  * `fill_` of a float32 tensor the size of one headline launch's observations ([256, 4096, 5, 213]):
+    the rate at which this card streams writes to HBM, the ceiling of a kernel that mostly writes;
+  * the headline rollout (C2: 4096 envs, 5 pursuers, T = 256) and C4 (4096 envs, 20 pursuers, T = 64),
+    reported as kernel time and observation bytes / kernel time next to the fill rate.
+Every `--lib` build (default: the library MADRL_B200_LIB names, else the in-tree one; a PATH is loaded
+through MADRL_B200_LIB, e.g. one made by scripts/build_variant.py from another checkout) is timed in a
+child process of its own, the builds alternating for R rounds, and the median and min-max spread over
+the rounds are printed per build.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+SHAPES = {"c2": dict(cfg=dict(n_pursuers=5, n_evaders=5, n_poison=10, n_sensors=30), E=4096, T=256),
+          "c4": dict(cfg=dict(n_pursuers=20, n_evaders=50, n_poison=50, n_sensors=30), E=4096, T=64)}
+
+
+def card():
+    import torch
+    q = "name,power.limit,clocks.sm,clocks.max.sm"
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=" + q, "--format=csv,noheader", "-i",
+                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
+        return dict(zip(q.split(","), [s.strip() for s in out.strip().split(",")]))
+    except (OSError, subprocess.SubprocessError):
+        return {"name": torch.cuda.get_device_name(), "power.limit": "unknown", "clocks.sm": "unknown"}
+
+
+def event_ms(fn, warmup, reps):
+    """Median over `reps` calls of fn's device time (CUDA events around each call)."""
+    import torch
+    for _ in range(warmup):
+        fn()
+    torch.cuda.synchronize()
+    ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(reps)]
+    for s, e in ev:
+        s.record()
+        fn()
+        e.record()
+    torch.cuda.synchronize()
+    return sorted(s.elapsed_time(e) for s, e in ev)[reps // 2]
+
+
+def fill_rate(reps):
+    import torch
+    x = torch.empty((256, 4096, 5, 213), dtype=torch.float32, device="cuda")
+    ms = event_ms(lambda: x.fill_(1.0), 3, reps)
+    nbytes = x.numel() * 4
+    del x
+    torch.cuda.empty_cache()
+    return {"bytes": nbytes, "ms": ms, "gbs": nbytes / (ms * 1e-3) / 1e9}
+
+
+def rollout_rate(name, reps):
+    import torch
+    sys.path.insert(0, ROOT)
+    from madrl_b200 import BatchedMAWaterWorld
+    s = SHAPES[name]
+    E, T, Np = s["E"], s["T"], s["cfg"]["n_pursuers"]
+    eng = BatchedMAWaterWorld(E, device="cuda", seed=0, **s["cfg"])
+    eng.reset()
+    g = torch.Generator(device="cuda")
+    g.manual_seed(1234)
+    act = torch.randn(T, E, Np, 2, device="cuda", generator=g) * 0.5
+    out = (torch.empty((T, E, Np, eng.obs_dim), device="cuda"), torch.empty((T, E, Np), device="cuda"),
+           torch.empty((T, E), dtype=torch.uint8, device="cuda"), torch.empty((T, E, 2), dtype=torch.int32, device="cuda"))
+    ms = event_ms(lambda: eng.rollout(act, auto_reset=True, out=out), 3, reps)
+    obs_bytes = out[0].numel() * 4
+    return {"ms": ms, "obs_bytes": obs_bytes, "obs_gbs": obs_bytes / (ms * 1e-3) / 1e9,
+            "agent_steps_per_sec": E * Np * T / (ms * 1e-3)}
+
+
+def child(reps):
+    print(json.dumps({n: rollout_rate(n, reps) for n in SHAPES}), flush=True)
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--lib", action="append", default=[], metavar="NAME=PATH",
+                    help="a build to time (PATH is loaded through MADRL_B200_LIB; 'NAME=' = the in-tree library)")
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--reps", type=int, default=10, help="timed launches per shape and round")
+    ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
+    a = ap.parse_args()
+    if a.child:
+        return child(a.reps)
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("ww_write_path.py needs a CUDA device")
+    libs = [tuple(s.split("=", 1)) for s in a.lib] or [("default", os.environ.get("MADRL_B200_LIB", ""))]
+    print("card:", json.dumps(card()))
+    fill = fill_rate(20)
+    print("fill_ float32 %.2f GB: %.3f ms, %.1f GB/s (streaming-write rate)" % (fill["bytes"] / 1e9, fill["ms"], fill["gbs"]))
+    res = {n: {s: [] for s in SHAPES} for n, _ in libs}
+    for r in range(a.rounds):
+        for n, path in libs:
+            env = dict(os.environ)
+            env.pop("MADRL_B200_LIB", None)
+            if path:
+                env["MADRL_B200_LIB"] = os.path.abspath(path)
+            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--reps", str(a.reps)],
+                               env=env, cwd=ROOT, capture_output=True, text=True)
+            if p.returncode:
+                sys.stderr.write(p.stdout + p.stderr)
+                raise SystemExit("round %d, build %s failed" % (r, n))
+            rec = json.loads(p.stdout.strip().splitlines()[-1])
+            for s in SHAPES:
+                res[n][s].append(rec[s])
+                print("round %d %-8s %s: %.3f ms/launch, obs %.1f GB/s (%.1f%% of fill), %.3g agent-steps/s"
+                      % (r, n, s, rec[s]["ms"], rec[s]["obs_gbs"], 100 * rec[s]["obs_gbs"] / fill["gbs"],
+                         rec[s]["agent_steps_per_sec"]), flush=True)
+    print("summary (median over %d rounds; spread = (max - min) / median of the launch time):" % a.rounds)
+    for n, _ in libs:
+        for s in SHAPES:
+            ms = sorted(x["ms"] for x in res[n][s])
+            med = ms[len(ms) // 2]
+            gbs = res[n][s][0]["obs_bytes"] / (med * 1e-3) / 1e9
+            print("  %-8s %s: %.3f ms (spread %.1f%%), obs %.1f GB/s = %.1f%% of the fill rate"
+                  % (n, s, med, 100 * (ms[-1] - ms[0]) / med, gbs, 100 * gbs / fill["gbs"]))
+
+
+if __name__ == "__main__":
+    main()
