@@ -79,6 +79,16 @@ int madrl_copy_async(void* dst_dev, const void* src_dev, size_t bytes, void* str
 int madrl_stream_write32(void* stream, void* addr_dev, uint32_t value);
 int madrl_stream_wait_geq32(void* stream, void* addr_dev, uint32_t value);
 
+/* Observation formats (madrl_{ww,pursuit,hostage}_set_obs_format).  NATIVE: observations have the handle's
+ * `real` type (float, or double when fp64).  BF16: bfloat16 (2 bytes), fp32 handles only.  Features are computed
+ * in float either way and rounded to nearest even once, at the store: a BF16 observation is bit-identical to the
+ * NATIVE one converted to bfloat16, and state, rewards, dones and infos are the same.  The format applies to
+ * every observation buffer of the calls that follow it: reset, rollout, step, rollout_heuristic (obs0 and obs),
+ * the _host variants and the set_terminal_obs buffer.  It returns MADRL_EINVAL for an unknown format or BF16 on
+ * an fp64 handle.  Waterworld's fused peer exchange (madrl_ww_set_peers) needs NATIVE observations. */
+#define MADRL_OBS_NATIVE 0
+#define MADRL_OBS_BF16 1
+
 /* ------------------------------------------------------------------ MAWaterWorld ------------ */
 typedef struct madrl_ww_config {
   int32_t n_envs;          /* envs in THIS handle (the local shard)                              */
@@ -127,6 +137,7 @@ int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm);
  * of a finished env to the same [t][e] slot of term_obs_dev (same shape as that rollout's obs tensor;
  * other slots are left untouched).  NULL switches it off. */
 int madrl_ww_set_terminal_obs(madrl_ww* h, void* term_obs_dev);
+int madrl_ww_set_obs_format(madrl_ww* h, int format);
 /* Fused per-rollout exchange for env-sharded multi-GPU runs: after this call every rollout also
  * stores its reward / done / info rows into slot `slot` of each of the `n_dest` listed gather
  * buffers (peer-mapped device pointers: CUDA-IPC mappings of other ranks' buffers over NVLink; one
@@ -229,15 +240,17 @@ int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_p
  * of a finished env to the same [t][e] slot of term_obs_dev (same shape as that rollout's obs tensor;
  * other slots are left untouched).  NULL switches it off. */
 int madrl_pursuit_set_terminal_obs(madrl_pursuit* h, void* term_obs_dev);
+/* obs buffers below are float, or bfloat16 after set_obs_format(MADRL_OBS_BF16). */
+int madrl_pursuit_set_obs_format(madrl_pursuit* h, int format);
 /* Curriculum knobs that survive pickling in the reference (pursuit_evade.py:264-272,397-411). */
 int madrl_pursuit_set_params(madrl_pursuit* h, double catchr, double constraint_window);
 /* reset(): obs_dev float [E][Np][obs_dim]. */
-int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, float* obs_dev, void* stream);
+int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, void* obs_dev, void* stream);
 /* actions_dev int32 [T][E][Np] in {0 left,1 right,2 up,3 down,4 stay} (DiscreteAgent.py:28-38);
  * obs_dev float [T][E][Np][obs_dim] (obs_dim = 3R^2+id if flatten else 4R^2 laid out [x][y][ch]);
  * rew_dev float [T][E][Np] (computed in float64, narrowed once);
  * done_dev uint8 [T][E]; info_dev int32 [T][E] = removed. */
-int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, float* obs_dev,
+int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, void* obs_dev,
                           float* rew_dev, uint8_t* done_dev, int32_t* info_dev, int auto_reset,
                           void* stream);
 /* Closed-loop rollout: the pursuers' actions come from the reference's hand-written policy
@@ -251,16 +264,16 @@ int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, f
  * deciding on an observation produced when the env's draw counter stood at c takes word 32 c + q of the
  * (seed, env id, tag 2) Philox stream, mapped to {0..4} like every other range draw.  Other arguments as
  * madrl_pursuit_rollout. */
-int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const float* obs0_dev, int32_t* actions_out_dev,
-                                    float* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
+int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const void* obs0_dev, int32_t* actions_out_dev,
+                                    void* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
                                     int auto_reset, int floor_centre, void* stream);
-int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, float* obs_dev, float* rew_dev,
+int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, void* obs_dev, float* rew_dev,
                        uint8_t* done_dev, int32_t* info_dev, int auto_reset, void* stream);
-int madrl_pursuit_reset_host(madrl_pursuit* h, const uint8_t* mask_host, float* obs_host);
-int madrl_pursuit_rollout_host(madrl_pursuit* h, int T, const int32_t* actions_host, float* obs_host,
+int madrl_pursuit_reset_host(madrl_pursuit* h, const uint8_t* mask_host, void* obs_host);
+int madrl_pursuit_rollout_host(madrl_pursuit* h, int T, const int32_t* actions_host, void* obs_host,
                                float* rew_host, uint8_t* done_host, int32_t* info_host,
                                int auto_reset);
-int madrl_pursuit_rollout_host2(madrl_pursuit* h, int T, const int32_t* actions_host, float* obs_host,
+int madrl_pursuit_rollout_host2(madrl_pursuit* h, int T, const int32_t* actions_host, void* obs_host,
                                 float* rew_host, uint8_t* done_host, int32_t* info_host,
                                 int auto_reset, int flags);
 
@@ -302,6 +315,7 @@ int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, int blocks_p
  * of a finished env to the same [t][e] slot of term_obs_dev (same shape as that rollout's obs tensor;
  * other slots are left untouched).  NULL switches it off. */
 int madrl_hostage_set_terminal_obs(madrl_hostage* h, void* term_obs_dev);
+int madrl_hostage_set_obs_format(madrl_hostage* h, int format);
 /* obs_dev real [E][n_good][obs_dim] */
 int madrl_hostage_reset(madrl_hostage* h, const uint8_t* mask_dev, void* obs_dev, void* stream);
 /* actions_dev real [T][E][n_good][2]; obs_dev real [T][E][n_good][obs_dim]; rew_dev real
@@ -350,12 +364,21 @@ int madrl_gae_f32(int T, int E, int A, const float* rew_dev, const float* value_
  * out [T][E][A][D][B]; carry [E][A][D][B] is the buffer kept between calls; B <= 8. */
 int madrl_frame_stack_f32(int T, int E, int A, int D, int B, const float* obs_dev,
                           const uint8_t* done_dev, float* carry_dev, float* out_dev, void* stream);
+/* bfloat16 observations (madrl_*_set_obs_format): obs, carry and out hold bfloat16. */
+int madrl_frame_stack_bf16(int T, int E, int A, int D, int B, const void* obs_dev,
+                           const uint8_t* done_dev, void* carry_dev, void* out_dev, void* stream);
 /* StandardizedEnv running mean / variance normalisation (madrl_environments/__init__.py:241-291),
  * in place over x [T][n] with float64 state mean/var [n]; center=1 for observations, 0 for rewards
  * (which are divided by the running std and multiplied by `scale`); enable=0 only applies `scale`. */
 int madrl_standardize_f32(int T, size_t n, float* x_dev, double* mean_dev, double* var_dev,
                           double alpha, double eps, int center, double scale, int enable,
                           void* stream);
+/* Same over bfloat16 x: each value is widened, takes the float32 pass's float64 arithmetic and float32
+ * result, and is rounded to bfloat16 once, at the store (bit-identical to the f32 pass on the widened
+ * input, rounded to nearest even). */
+int madrl_standardize_bf16(int T, size_t n, void* x_dev, double* mean_dev, double* var_dev,
+                           double alpha, double eps, int center, double scale, int enable,
+                           void* stream);
 /* Same, for observations of an auto-reset rollout with the terminal observations kept on the side
  * (madrl_*_set_terminal_obs): at a step with done[t][e] set, the running estimate of env e's columns is
  * first updated with term[t] (which is standardised in place too) and then with x[t] -- the reference
@@ -364,6 +387,10 @@ int madrl_standardize_f32(int T, size_t n, float* x_dev, double* mean_dev, doubl
 int madrl_standardize_obs_terminal_f32(int T, int E, size_t per_env, float* x_dev, float* term_dev,
                                        const uint8_t* done_dev, double* mean_dev, double* var_dev,
                                        double alpha, double eps, void* stream);
+/* Same over bfloat16 x and term, rounded as madrl_standardize_bf16. */
+int madrl_standardize_obs_terminal_bf16(int T, int E, size_t per_env, void* x_dev, void* term_dev,
+                                        const uint8_t* done_dev, double* mean_dev, double* var_dev,
+                                        double alpha, double eps, void* stream);
 /* DiagnosticsWrapper episode statistics (madrl_environments/__init__.py:314-369): rew [T][E][A],
  * done uint8 [T][E]; carry float64 [E][A+3] (zero-initialised by the caller, kept between calls);
  * outputs at the steps where an episode closes (ep_end[t][e] = 1; zeros elsewhere):
@@ -404,6 +431,9 @@ int madrl_center_advantages_f32(size_t n, float* adv_dev, int center, int positi
 int madrl_paths_plan(int T, int E, int A, const uint8_t* done_dev, int32_t* seg_start_dev, int32_t* seg_len_dev,
                      int32_t* n_episodes_dev, int32_t* ep_rec_dev, void* stream);
 int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
+                         const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream);
+/* madrl_paths_pack_u32 for rows of D 2-byte elements (bfloat16 observations; D may be odd). */
+int madrl_paths_pack_u16(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
                          const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream);
 
 #ifdef __cplusplus

@@ -15,6 +15,10 @@ class EngineError(RuntimeError):
     pass
 
 
+# observation formats (madrl_*_set_obs_format)
+OBS_NATIVE, OBS_BF16 = 0, 1
+
+
 class WWConfig(C.Structure):
     _fields_ = [
         ("n_envs", C.c_int32), ("env_id_base", C.c_int32),
@@ -111,6 +115,9 @@ def _declare_engines(lib):
         f("reset_host").argtypes = [vp, vp, vp]
         f("rollout_host").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32]
         f("rollout_host2").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, i32]
+        # absent from libraries built before the bfloat16 observation format (timed side by side by scripts/)
+        if hasattr(lib, "madrl_%s_set_obs_format" % fam):
+            f("set_obs_format").argtypes = [vp, i32]
     lib.madrl_ww_set_peers.argtypes = [vp, i32, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.madrl_ww_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.madrl_pursuit_set_params.argtypes = [vp, C.c_double, C.c_double]
@@ -147,6 +154,11 @@ def _declare(lib):
     lib.madrl_paths_pack_u32.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     lib.madrl_moments_f32.argtypes = [C.c_size_t, vp, vp, vp, vp, vp]
     lib.madrl_center_advantages_f32.argtypes = [C.c_size_t, vp, i32, i32, vp, vp, vp]
+    if hasattr(lib, "madrl_frame_stack_bf16"):   # bfloat16 observation passes (absent from older builds)
+        lib.madrl_frame_stack_bf16.argtypes = lib.madrl_frame_stack_f32.argtypes
+        lib.madrl_standardize_bf16.argtypes = lib.madrl_standardize_f32.argtypes
+        lib.madrl_standardize_obs_terminal_bf16.argtypes = lib.madrl_standardize_obs_terminal_f32.argtypes
+        lib.madrl_paths_pack_u16.argtypes = lib.madrl_paths_pack_u32.argtypes
 
 
 def lib():

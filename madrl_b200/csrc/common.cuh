@@ -186,6 +186,18 @@ __device__ __forceinline__ void bulk_wait_read_all_but_1() { asm volatile("cp.as
 __device__ __forceinline__ void bulk_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;\n\tfence.proxy.async.global;" ::: "memory");
 }
+// bfloat16 bits of v, rounded to nearest even (cvt.rn), as a plain uint16_t: no cuda_bf16.h type enters the
+// kernels.  The pair form packs `lo` into bits 0-15 (the lower address) and `hi` into bits 16-31.
+__device__ __forceinline__ uint16_t bf16_rn(float v) {
+  uint16_t r;
+  asm("cvt.rn.bf16.f32 %0, %1;" : "=h"(r) : "f"(v));
+  return r;
+}
+__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
+  uint32_t r;
+  asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+  return r;
+}
 #else   // MADRL_EMU_PTX_HELPERS
 // Host versions of the bulk-store helpers above for the test emulator, built on the shared-memory
 // primitives its <cuda_runtime.h> provides (emu_at, smem_access: the per-byte race checker).  The
@@ -212,7 +224,42 @@ static inline void bulk_store_stream(void* dst, uint32_t src, uint32_t bytes) {
 static inline void bulk_wait_read_all() {}
 static inline void bulk_wait_read_all_but_1() {}
 static inline void bulk_wait_all() {}
+// Round-to-nearest-even on the bit pattern, as cvt.rn.bf16.f32 rounds finite values and infinities.  A NaN
+// maps to some NaN here; which one the hardware returns is not modelled (observations are never NaN).
+static inline uint16_t bf16_rn(float v) {
+  uint32_t u;
+  memcpy(&u, &v, 4);
+  if ((u & 0x7fffffffu) > 0x7f800000u) return (uint16_t)((u >> 16) | 0x40u);
+  return (uint16_t)((u + 0x7fffu + ((u >> 16) & 1u)) >> 16);
+}
+static inline uint32_t bf16x2_rn(float lo, float hi) { return (uint32_t)bf16_rn(lo) | ((uint32_t)bf16_rn(hi) << 16); }
 #endif  // MADRL_EMU_PTX_HELPERS
+
+// Observation element type O of an env kernel: its `real`, or uint16_t = bfloat16 bits (with real = float
+// only; madrl_*_set_obs_format).  Features are computed in `real` either way and converted once, at the
+// store, so a bf16 observation is exactly the rounded fp32 one.
+template <typename O, typename real>
+__device__ __forceinline__ O obs_cvt(real v) {
+  if constexpr (sizeof(O) == 2) return bf16_rn(v);
+  else return v;
+}
+// An observation element read back (the POLICY kernels' obs0) as `real`: bf16 widens exactly.
+template <typename real, typename O>
+__device__ __forceinline__ real obs_widen(O v) {
+  if constexpr (sizeof(O) == 2) return __int_as_float((int)((uint32_t)v << 16));
+  else return v;
+}
+// Shared-memory staging of observation elements (Waterworld's bulk-store rows).
+__device__ __forceinline__ void sts_obs(uint32_t a, float v) { sts_real(a, v); }
+__device__ __forceinline__ void sts_obs(uint32_t a, double v) { sts_real(a, v); }
+__device__ __forceinline__ void sts_obs(uint32_t a, uint16_t v) { sts_u16(a, v); }
+template <typename O> __device__ __forceinline__ O lds_obs(uint32_t a) {
+  if constexpr (sizeof(O) == 2) return (O)lds_u16(a);
+  else return lds_real<O>(a);
+}
+// Convert a `real` feature value to O and stage it.
+template <typename O, typename real>
+__device__ __forceinline__ void stage_obs(uint32_t a, real v) { sts_obs(a, obs_cvt<O>(v)); }
 
 // StandardizedEnv sees the TERMINAL observation of an episode before the reset one
 // (madrl_environments/__init__.py:283-291 step(), then reset()); under auto-reset the rollout's obs slot is

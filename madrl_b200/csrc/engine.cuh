@@ -21,6 +21,10 @@ struct EngineCore {
   int blocks_per_sm = 0;     // set_launch override of resident blocks per SM (0 = as many as fit)
   HostPipe pipe;             // staging + streams of the host-buffer entry points (lazily created)
   void* term_obs = nullptr;  // set_terminal_obs (NULL = off)
+  int obs_format = MADRL_OBS_NATIVE;   // set_obs_format: element type of every observation buffer
+
+  // bytes of one observation element: `native` (the handle's real) or 2 (bfloat16)
+  size_t obs_elem_bytes(size_t native) const { return obs_format == MADRL_OBS_BF16 ? 2 : native; }
 };
 
 template <class H>
@@ -85,6 +89,14 @@ int engine_seed(H* h, uint64_t seed, void* stream) {
 inline int engine_set_terminal_obs(EngineCore* h, void* term_obs_dev) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
   h->term_obs = term_obs_dev;
+  return MADRL_OK;
+}
+
+inline int engine_set_obs_format(EngineCore* h, int format, bool fp64) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(format == MADRL_OBS_NATIVE || format == MADRL_OBS_BF16, "unknown observation format %d", format);
+  MADRL_REQUIRE(!(format == MADRL_OBS_BF16 && fp64), "bfloat16 observations need an fp32 handle (fp64 = 0)");
+  h->obs_format = format;
   return MADRL_OK;
 }
 

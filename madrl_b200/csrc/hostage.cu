@@ -17,7 +17,7 @@
 
 namespace madrl {
 
-template <typename real>
+template <typename real, typename O = real>   // O: observation element type (see obs_cvt)
 struct HWParams {
   int E, env_id_base, Nr, Nc, Nh, K, n_coop_save, D, Nall;
   int reward_global, addid, random_key, timestep_limit, max_path_length;
@@ -39,12 +39,12 @@ struct HWParams {
   const real* sensors;
   // trajectory tensors
   const real* actions;
-  real* obs;
+  O* obs;
   real* rew;
   uint8_t* done;
   int32_t* info;     // [T][E][2] = (ho_saved, cr_encs)
   const uint8_t* mask;
-  real* term_obs;    // optional [T][E][Nr][D]: terminal observations of done steps (see keep_terminal_rows)
+  O* term_obs;       // optional [T][E][Nr][D]: terminal observations of done steps (see keep_terminal_rows)
 };
 
 template <typename real>
@@ -52,9 +52,9 @@ __device__ __forceinline__ real unit_at(uint64_t seed, uint32_t env_id, uint64_t
   return (real)(stream_word(seed, env_id, 0u, n) >> 8) * (real)(1.0 / 16777216.0);
 }
 
-template <typename real, int OPL, int KCH, int KC>
+template <typename real, typename O, int OPL, int KCH, int KC>
 __global__ void __launch_bounds__(32, (OPL <= 2 ? 28 : 16))
-hw_kernel(const __grid_constant__ HWParams<real> p) {
+hw_kernel(const __grid_constant__ HWParams<real, O> p) {
   const real INF = real_inf<real>();
   const int K = KC > 0 ? KC : p.K;
   const int lane = threadIdx.x;
@@ -112,7 +112,7 @@ hw_kernel(const __grid_constant__ HWParams<real> p) {
     int tt = p.timestep[e], ts = p.path_len[e];
     uint64_t ctr = p.ctr[e];
 
-    real* obs_t = p.obs + (size_t)e * p.Nr * p.D + lane;
+    O* obs_t = p.obs + (size_t)e * p.Nr * p.D + lane;
     real* rew_t = p.rew + (size_t)e * p.Nr + lane;
     size_t te = (size_t)e;
     int pass = (p.mode == 1) ? 1 : 0;
@@ -219,7 +219,7 @@ hw_kernel(const __grid_constant__ HWParams<real> p) {
         }
         const bool gate_post = gate_pre || (coll_ke != 0u);
         // ---- sense: one rescuer at a time -----------------------------------------------------------
-        real* obs_row = obs_t;
+        O* obs_row = obs_t;
         for (int pi = 0; pi < p.Nr; ++pi, obs_row += p.D) {
           const real mx = __shfl_sync(FULL_MASK, rpx, pi), my = __shfl_sync(FULL_MASK, rpy, pi);
           const real mvx = __shfl_sync(FULL_MASK, rpvx, pi), mvy = __shfl_sync(FULL_MASK, rpvy, pi);
@@ -295,12 +295,12 @@ hw_kernel(const __grid_constant__ HWParams<real> p) {
               sC = hC ? sx * (oCx - mvx) + sy * (oCy - mvy) : z;
             }
             if (k < K) {
-              real* o = obs_row + 32 * kc;
-              store_stream(o + 0 * K, fC);
-              store_stream(o + 1 * K, sC);
-              store_stream(o + 2 * K, bH[kc] < INF ? bH[kc] : z);
-              store_stream(o + 3 * K, bK[kc] < INF ? bK[kc] : z);
-              store_stream(o + 4 * K, bB[kc] < INF ? bB[kc] : z);
+              O* o = obs_row + 32 * kc;
+              store_stream(o + 0 * K, obs_cvt<O>(fC));
+              store_stream(o + 1 * K, obs_cvt<O>(sC));
+              store_stream(o + 2 * K, obs_cvt<O>(bH[kc] < INF ? bH[kc] : z));
+              store_stream(o + 3 * K, obs_cvt<O>(bK[kc] < INF ? bK[kc] : z));
+              store_stream(o + 4 * K, obs_cvt<O>(bB[kc] < INF ? bB[kc] : z));
             }
           }
         }
@@ -339,13 +339,13 @@ hw_kernel(const __grid_constant__ HWParams<real> p) {
         // tail hw:406-421 of every rescuer's row: coll_ho, coll_cr, coll_key, coll_bomb, gate_open
         // (post), id; lane i writes rescuer i's.  whoEnc / whoC are exactly the any-collision masks.
         if (lane < p.Nr) {
-          real* tp = obs_t + (size_t)lane * (p.D - 1) + 5 * K;   // obs_t already carries +lane
-          store_stream(tp, (real)((whoEnc >> lane) & 1u));
-          store_stream(tp + 1, (real)((whoC >> lane) & 1u));
-          store_stream(tp + 2, (real)((coll_ke >> lane) & 1u));
-          store_stream(tp + 3, (real)((coll_bo >> lane) & 1u));
-          store_stream(tp + 4, gate_post ? (real)1 : (real)0);
-          if (p.addid) store_stream(tp + 5, (real)(lane + 1));
+          O* tp = obs_t + (size_t)lane * (p.D - 1) + 5 * K;   // obs_t already carries +lane
+          store_stream(tp, obs_cvt<O>((real)((whoEnc >> lane) & 1u)));
+          store_stream(tp + 1, obs_cvt<O>((real)((whoC >> lane) & 1u)));
+          store_stream(tp + 2, obs_cvt<O>((real)((coll_ke >> lane) & 1u)));
+          store_stream(tp + 3, obs_cvt<O>((real)((coll_bo >> lane) & 1u)));
+          store_stream(tp + 4, obs_cvt<O>(gate_post ? (real)1 : (real)0));
+          if (p.addid) store_stream(tp + 5, obs_cvt<O>((real)(lane + 1)));
         }
         if (coll_bo) flags |= 2;
         if (coll_ke) flags |= 1;
@@ -423,7 +423,7 @@ struct madrl_hostage : EngineCore {
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Nr = cfg.n_good, rb = lay.real_bytes;
-    return {E * Nr * 2 * rb, E * Nr * lay.obs_dim * rb, E * Nr * rb, E, E * 2 * 4};
+    return {E * Nr * 2 * rb, E * Nr * lay.obs_dim * obs_elem_bytes(rb), E * Nr * rb, E, E * 2 * 4};
   }
 };
 
@@ -477,20 +477,24 @@ extern "C" int madrl_hostage_set_terminal_obs(madrl_hostage* h, void* term_obs_d
   return engine_set_terminal_obs(h, term_obs_dev);
 }
 
+extern "C" int madrl_hostage_set_obs_format(madrl_hostage* h, int format) {
+  return engine_set_obs_format(h, format, h != nullptr && h->cfg.fp64);
+}
+
 extern "C" int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
-template <typename real, int OPL, int KCH, int KC>
-static int hw_launch_inst(madrl_hostage* h, const HWParams<real>& p, cudaStream_t stream) {
-  return engine_launch(h, hw_kernel<real, OPL, KCH, KC>, 0, p.E, stream, p);
+template <typename real, typename O, int OPL, int KCH, int KC>
+static int hw_launch_inst(madrl_hostage* h, const HWParams<real, O>& p, cudaStream_t stream) {
+  return engine_launch(h, hw_kernel<real, O, OPL, KCH, KC>, 0, p.E, stream, p);
 }
 
-template <typename real>
-static int hw_launch(madrl_hostage* h, int mode, int T, const void* actions, void* obs, void* rew,
-                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream) {
+template <typename real, typename O>
+static int hw_launch_t(madrl_hostage* h, int mode, int T, const void* actions, void* obs, void* rew,
+                       uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream) {
   const madrl_hostage_config& c = h->cfg;
-  HWParams<real> p;
+  HWParams<real, O> p;
   p.E = c.n_envs; p.env_id_base = c.env_id_base; p.Nr = c.n_good; p.Nc = c.n_bad; p.Nh = c.n_hostages;
   p.K = c.n_sensors; p.n_coop_save = c.n_coop_save; p.D = h->lay.obs_dim; p.Nall = h->lay.n_obj;
   p.reward_global = c.reward_global; p.addid = c.addid; p.random_key = c.random_key;
@@ -517,11 +521,11 @@ static int hw_launch(madrl_hostage* h, int mode, int T, const void* actions, voi
   p.saved = (uint8_t*)(st + h->lay.saved); p.flags = (int32_t*)(st + h->lay.flags);
   p.timestep = (int32_t*)(st + h->lay.timestep); p.path_len = (int32_t*)(st + h->lay.path_len);
   p.ctr = (uint64_t*)(st + h->lay.rng_counter); p.sensors = (const real*)(st + h->lay.sensors);
-  p.actions = (const real*)actions; p.obs = (real*)obs; p.rew = (real*)rew;
+  p.actions = (const real*)actions; p.obs = (O*)obs; p.rew = (real*)rew;
   p.done = done; p.info = info; p.mask = mask;
-  p.term_obs = (mode == 0) ? (real*)h->term_obs : nullptr;
+  p.term_obs = (mode == 0) ? (O*)h->term_obs : nullptr;
   const int opl = (p.Nall - p.Nr + 31) / 32, kch = (p.K + 31) / 32;
-#define MADRL_HW_CASE(O, KH, KC_) return hw_launch_inst<real, O, KH, KC_>(h, p, stream)
+#define MADRL_HW_CASE(OP, KH, KC_) return hw_launch_inst<real, O, OP, KH, KC_>(h, p, stream)
   if (p.K == 30) {
     if (opl == 1) MADRL_HW_CASE(1, 1, 30);
     if (opl == 2) MADRL_HW_CASE(2, 1, 30);
@@ -541,10 +545,18 @@ static int hw_launch(madrl_hostage* h, int mode, int T, const void* actions, voi
 #undef MADRL_HW_CASE
 }
 
+// fp64 verification build, fp32 with fp32 observations, or fp32 with bfloat16 observations
+static int hw_launch(madrl_hostage* h, int mode, int T, const void* actions, void* obs, void* rew,
+                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream) {
+  if (h->cfg.fp64) return hw_launch_t<double, double>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream);
+  if (h->obs_format == MADRL_OBS_BF16)
+    return hw_launch_t<float, uint16_t>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream);
+  return hw_launch_t<float, float>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream);
+}
+
 extern "C" int madrl_hostage_reset(madrl_hostage* h, const uint8_t* mask_dev, void* obs_dev, void* stream) {
   MADRL_REQUIRE(h != nullptr && obs_dev != nullptr, "handle/obs is NULL");
-  return h->cfg.fp64 ? hw_launch<double>(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream)
-                     : hw_launch<float>(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
+  return hw_launch(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_hostage_rollout(madrl_hostage* h, int T, const void* actions_dev, void* obs_dev, void* rew_dev,
@@ -553,8 +565,7 @@ extern "C" int madrl_hostage_rollout(madrl_hostage* h, int T, const void* action
   MADRL_REQUIRE(T >= 1, "T must be >= 1");
   MADRL_REQUIRE(actions_dev && obs_dev && rew_dev && done_dev && info_dev, "NULL trajectory buffer");
   MADRL_REQUIRE(((uintptr_t)info_dev & 7) == 0, "info_dev must be 8-byte aligned (rows are stored as one 8-byte word)");
-  return h->cfg.fp64 ? hw_launch<double>(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream)
-                     : hw_launch<float>(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
+  return hw_launch(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_hostage_step(madrl_hostage* h, const void* actions_dev, void* obs_dev, void* rew_dev,

@@ -8,6 +8,10 @@
 //                            paths segmented by `done`
 //   madrl_frame_stack_f32    madrl_environments/__init__.py:143-196  ObservationBuffer
 //   madrl_standardize_f32    madrl_environments/__init__.py:204-291  StandardizedEnv
+// The observation passes (frame stack, standardize, path packing) also take bfloat16 observations
+// (madrl_*_set_obs_format): element type O = uint16_t holding bfloat16 bits.  Values are widened to the
+// same float / double arithmetic as the float32 pass and rounded once, at the store, so a bf16 result is
+// the f32 pass's result on the widened input, rounded to nearest even.
 #include "common.cuh"
 
 namespace madrl {
@@ -41,18 +45,19 @@ __global__ void gae_kernel(int T, int E, int A, const float* __restrict__ rew,
 // ObservationBuffer: out[t][..][d][b] = the observation b steps before the newest one; on a step
 // whose `done` flag is set the obs slot holds the reset observation and reset() fills every slot
 // of the buffer with it (__init__.py:186-196).  `carry` [E][A][D][B] holds the buffer between calls.
-template <int B>
-__global__ void frame_stack_kernel(int T, size_t n /* E*A*D */, int AD, const float* __restrict__ obs,
-                                   const uint8_t* __restrict__ done, int E, float* __restrict__ carry,
-                                   float* __restrict__ out) {
+// Values are only moved, so the bf16 variant (O = uint16_t: obs, carry and out in bfloat16) is exact.
+template <int B, typename O>
+__global__ void frame_stack_kernel(int T, size_t n /* E*A*D */, int AD, const O* __restrict__ obs,
+                                   const uint8_t* __restrict__ done, int E, O* __restrict__ carry,
+                                   O* __restrict__ out) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const size_t e = i / AD;
-  float buf[B];
+  O buf[B];
 #pragma unroll
   for (int b = 0; b < B; ++b) buf[b] = carry[i * B + b];
   for (int t = 0; t < T; ++t) {
-    const float x = obs[(size_t)t * n + i];
+    const O x = obs[(size_t)t * n + i];
     if (done[(size_t)t * E + e]) {
 #pragma unroll
       for (int b = 0; b < B; ++b) buf[b] = x;
@@ -61,7 +66,7 @@ __global__ void frame_stack_kernel(int T, size_t n /* E*A*D */, int AD, const fl
       for (int b = 0; b < B - 1; ++b) buf[b] = buf[b + 1];          // __init__.py:178-180
       buf[B - 1] = x;
     }
-    float* o = out + ((size_t)t * n + i) * B;
+    O* o = out + ((size_t)t * n + i) * B;
 #pragma unroll
     for (int b = 0; b < B; ++b) __stcs(o + b, buf[b]);
   }
@@ -87,7 +92,8 @@ __device__ __forceinline__ double inv_std(double v, double eps) {
   return r;
 }
 
-__global__ void standardize_kernel(int T, size_t n, float* __restrict__ x, double* __restrict__ mean,
+template <typename O>
+__global__ void standardize_kernel(int T, size_t n, O* __restrict__ x, double* __restrict__ mean,
                                    double* __restrict__ var, double alpha, double eps, int center,
                                    double scale, int enable) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -95,7 +101,7 @@ __global__ void standardize_kernel(int T, size_t n, float* __restrict__ x, doubl
   double m = mean[i], v = var[i];
   for (int t = 0; t < T; ++t) {
     const size_t k = (size_t)t * n + i;
-    const double xv = (double)x[k];
+    const double xv = (double)obs_widen<float>(x[k]);
     double o = xv;
     if (enable) {
       m = (1.0 - alpha) * m + alpha * xv;
@@ -103,15 +109,16 @@ __global__ void standardize_kernel(int T, size_t n, float* __restrict__ x, doubl
       v = (1.0 - alpha) * v + alpha * d * d;
       o = (center ? (xv - m) : xv) * inv_std(v, eps);
     }
-    x[k] = (float)(scale * o);
+    x[k] = obs_cvt<O>((float)(scale * o));
   }
   mean[i] = m;
   var[i] = v;
 }
 
 // Observation standardiser for auto-reset rollouts with the terminal observations on the side.
-__global__ void standardize_terminal_kernel(int T, int E, size_t per_env, float* __restrict__ x,
-                                            float* __restrict__ term, const uint8_t* __restrict__ done,
+template <typename O>
+__global__ void standardize_terminal_kernel(int T, int E, size_t per_env, O* __restrict__ x,
+                                            O* __restrict__ term, const uint8_t* __restrict__ done,
                                             double* __restrict__ mean, double* __restrict__ var, double alpha,
                                             double eps) {
   const size_t n = (size_t)E * per_env;
@@ -122,17 +129,17 @@ __global__ void standardize_terminal_kernel(int T, int E, size_t per_env, float*
   for (int t = 0; t < T; ++t) {
     const size_t k = (size_t)t * n + i;
     if (done[(size_t)t * E + e]) {                 // step(): the terminal observation comes first
-      const double tv = (double)term[k];
+      const double tv = (double)obs_widen<float>(term[k]);
       m = (1.0 - alpha) * m + alpha * tv;
       const double d = tv - m;
       v = (1.0 - alpha) * v + alpha * d * d;
-      term[k] = (float)((tv - m) * inv_std(v, eps));
+      term[k] = obs_cvt<O>((float)((tv - m) * inv_std(v, eps)));
     }
-    const double xv = (double)x[k];
+    const double xv = (double)obs_widen<float>(x[k]);
     m = (1.0 - alpha) * m + alpha * xv;
     const double d = xv - m;
     v = (1.0 - alpha) * v + alpha * d * d;
-    x[k] = (float)((xv - m) * inv_std(v, eps));
+    x[k] = obs_cvt<O>((float)((xv - m) * inv_std(v, eps)));
   }
   mean[i] = m;
   var[i] = v;
@@ -320,9 +327,11 @@ __global__ void paths_plan_kernel(int T, int E, int A, const uint8_t* __restrict
   n_episodes[e] = n;
 }
 
-__global__ void paths_pack_kernel(int T, int E, int A, int D, const uint32_t* __restrict__ src,
-                                  const uint32_t* __restrict__ first, const int32_t* __restrict__ seg_start,
-                                  const int32_t* __restrict__ seg_len, uint32_t* __restrict__ dst) {
+// W = the row element: uint32_t (4-byte words) or uint16_t (bfloat16 observations; rows of odd length).
+template <typename W>
+__global__ void paths_pack_kernel(int T, int E, int A, int D, const W* __restrict__ src,
+                                  const W* __restrict__ first, const int32_t* __restrict__ seg_start,
+                                  const int32_t* __restrict__ seg_len, W* __restrict__ dst) {
   const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // source row (t, e, a)
   const int lane = threadIdx.x & 31;
   const size_t rows = (size_t)T * E * A;
@@ -334,16 +343,17 @@ __global__ void paths_pack_kernel(int T, int E, int A, int D, const uint32_t* __
   // `first` != NULL: observations are shifted by one step -- the row of time t is the observation the
   // action of time t was taken in: first[e][a] for t = 0, src[t-1] afterwards (on a done step the
   // rollout's obs slot already holds the reset observation, i.e. the next episode's first one)
-  const uint32_t* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
-                             : src + row * D;
-  uint32_t* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
+  const W* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
+                      : src + row * D;
+  W* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
   for (int d = lane; d < D; d += 32) __stcs(out + d, __ldcs(in + d));
 }
 
 // Narrow rows (rewards, actions, infos: D <= 4 words): one THREAD per source row instead of one warp.
-__global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const uint32_t* __restrict__ src,
-                                         const uint32_t* __restrict__ first, const int32_t* __restrict__ seg_start,
-                                         const int32_t* __restrict__ seg_len, uint32_t* __restrict__ dst) {
+template <typename W>
+__global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const W* __restrict__ src,
+                                         const W* __restrict__ first, const int32_t* __restrict__ seg_start,
+                                         const int32_t* __restrict__ seg_len, W* __restrict__ dst) {
   const size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x;   // source row (t, e, a)
   const size_t rows = (size_t)T * E * A;
   if (row >= rows) return;
@@ -351,9 +361,9 @@ __global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const uint3
   const size_t te = row / A;
   const int e = (int)(te % E), t = (int)(te / E);
   const int s = seg_start[te], L = seg_len[te];
-  const uint32_t* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
-                             : src + row * D;
-  uint32_t* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
+  const W* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
+                      : src + row * D;
+  W* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
   for (int d = 0; d < D; ++d) out[d] = in[d];
 }
 
@@ -389,18 +399,41 @@ extern "C" int madrl_gae_f32(int T, int E, int A, const float* rew_dev, const fl
   return MADRL_OK;
 }
 
-extern "C" int madrl_frame_stack_f32(int T, int E, int A, int D, int B, const float* obs_dev,
-                                     const uint8_t* done_dev, float* carry_dev, float* out_dev,
-                                     void* stream) {
+template <typename O>
+static int frame_stack(int T, int E, int A, int D, int B, const O* obs_dev, const uint8_t* done_dev, O* carry_dev,
+                       O* out_dev, void* stream) {
   MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && D >= 1, "bad sizes");
   MADRL_REQUIRE(B >= 1 && B <= 8, "buffer_size must be in [1,8], got %d", B);
   MADRL_REQUIRE(obs_dev && done_dev && carry_dev && out_dev, "NULL buffer");
   const size_t n = (size_t)E * A * D;
   const unsigned grid = (unsigned)((n + 255) / 256);
   cudaStream_t s = (cudaStream_t)stream;
-#define MADRL_FS(BB) case BB: MADRL_LAUNCH(frame_stack_kernel<BB>, grid, 256, 0, s, T, n, A * D, obs_dev, done_dev, E, carry_dev, out_dev); break
+#define MADRL_FS(BB) case BB: MADRL_LAUNCH((frame_stack_kernel<BB, O>), grid, 256, 0, s, T, n, A * D, obs_dev, done_dev, E, carry_dev, out_dev); break
   switch (B) { MADRL_FS(1); MADRL_FS(2); MADRL_FS(3); MADRL_FS(4); MADRL_FS(5); MADRL_FS(6); MADRL_FS(7); MADRL_FS(8); }
 #undef MADRL_FS
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_frame_stack_f32(int T, int E, int A, int D, int B, const float* obs_dev,
+                                     const uint8_t* done_dev, float* carry_dev, float* out_dev,
+                                     void* stream) {
+  return frame_stack(T, E, A, D, B, obs_dev, done_dev, carry_dev, out_dev, stream);
+}
+
+extern "C" int madrl_frame_stack_bf16(int T, int E, int A, int D, int B, const void* obs_dev,
+                                      const uint8_t* done_dev, void* carry_dev, void* out_dev, void* stream) {
+  return frame_stack(T, E, A, D, B, (const uint16_t*)obs_dev, done_dev, (uint16_t*)carry_dev, (uint16_t*)out_dev, stream);
+}
+
+template <typename O>
+static int standardize(int T, size_t n, O* x_dev, double* mean_dev, double* var_dev, double alpha, double eps,
+                       int center, double scale, int enable, void* stream) {
+  MADRL_REQUIRE(T >= 1 && n >= 1, "bad sizes");
+  MADRL_REQUIRE(x_dev && mean_dev && var_dev, "NULL buffer");
+  MADRL_LAUNCH(standardize_kernel<O>, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream,
+      T, n, x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -409,13 +442,13 @@ extern "C" int madrl_frame_stack_f32(int T, int E, int A, int D, int B, const fl
 extern "C" int madrl_standardize_f32(int T, size_t n, float* x_dev, double* mean_dev, double* var_dev,
                                      double alpha, double eps, int center, double scale, int enable,
                                      void* stream) {
-  MADRL_REQUIRE(T >= 1 && n >= 1, "bad sizes");
-  MADRL_REQUIRE(x_dev && mean_dev && var_dev, "NULL buffer");
-  MADRL_LAUNCH(standardize_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, 
-      T, n, x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable);
-  g_launches.fetch_add(1);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
+  return standardize(T, n, x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable, stream);
+}
+
+extern "C" int madrl_standardize_bf16(int T, size_t n, void* x_dev, double* mean_dev, double* var_dev,
+                                      double alpha, double eps, int center, double scale, int enable,
+                                      void* stream) {
+  return standardize(T, n, (uint16_t*)x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable, stream);
 }
 
 static int run_moments(size_t n, const float* a, const float* b, double* stats, double* ws, cudaStream_t s) {
@@ -462,20 +495,45 @@ extern "C" int madrl_paths_plan(int T, int E, int A, const uint8_t* done_dev, in
   return MADRL_OK;
 }
 
-extern "C" int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
-                                    const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev,
-                                    void* stream) {
+template <typename W>
+static int paths_pack(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
+                      const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream) {
   MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && D >= 1, "bad shape");
   MADRL_REQUIRE(src_dev && seg_start_dev && seg_len_dev && dst_dev, "NULL pointer");
   const size_t rows = (size_t)T * E * A;
   const size_t blocks = D <= 4 ? (rows + 255) / 256 : (rows * 32 + 255) / 256;
   MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many rows for one launch");
   if (D <= 4)
-    MADRL_LAUNCH(paths_pack_narrow_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D,
-                 (const uint32_t*)src_dev, (const uint32_t*)first_dev, seg_start_dev, seg_len_dev, (uint32_t*)dst_dev);
+    MADRL_LAUNCH(paths_pack_narrow_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D,
+                 (const W*)src_dev, (const W*)first_dev, seg_start_dev, seg_len_dev, (W*)dst_dev);
   else
-    MADRL_LAUNCH(paths_pack_kernel, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D, (const uint32_t*)src_dev,
-                 (const uint32_t*)first_dev, seg_start_dev, seg_len_dev, (uint32_t*)dst_dev);
+    MADRL_LAUNCH(paths_pack_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D, (const W*)src_dev,
+                 (const W*)first_dev, seg_start_dev, seg_len_dev, (W*)dst_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
+                                    const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev,
+                                    void* stream) {
+  return paths_pack<uint32_t>(T, E, A, D, src_dev, first_dev, seg_start_dev, seg_len_dev, dst_dev, stream);
+}
+
+extern "C" int madrl_paths_pack_u16(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
+                                    const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev,
+                                    void* stream) {
+  return paths_pack<uint16_t>(T, E, A, D, src_dev, first_dev, seg_start_dev, seg_len_dev, dst_dev, stream);
+}
+
+template <typename O>
+static int standardize_obs_terminal(int T, int E, size_t per_env, O* x_dev, O* term_dev, const uint8_t* done_dev,
+                                    double* mean_dev, double* var_dev, double alpha, double eps, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && per_env >= 1, "bad sizes");
+  MADRL_REQUIRE(x_dev && term_dev && done_dev && mean_dev && var_dev, "NULL buffer");
+  const size_t n = (size_t)E * per_env;
+  MADRL_LAUNCH(standardize_terminal_kernel<O>, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, T, E, per_env,
+               x_dev, term_dev, done_dev, mean_dev, var_dev, alpha, eps);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -484,12 +542,12 @@ extern "C" int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_
 extern "C" int madrl_standardize_obs_terminal_f32(int T, int E, size_t per_env, float* x_dev, float* term_dev,
                                                   const uint8_t* done_dev, double* mean_dev, double* var_dev,
                                                   double alpha, double eps, void* stream) {
-  MADRL_REQUIRE(T >= 1 && E >= 1 && per_env >= 1, "bad sizes");
-  MADRL_REQUIRE(x_dev && term_dev && done_dev && mean_dev && var_dev, "NULL buffer");
-  const size_t n = (size_t)E * per_env;
-  MADRL_LAUNCH(standardize_terminal_kernel, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, T, E, per_env,
-               x_dev, term_dev, done_dev, mean_dev, var_dev, alpha, eps);
-  g_launches.fetch_add(1);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
+  return standardize_obs_terminal(T, E, per_env, x_dev, term_dev, done_dev, mean_dev, var_dev, alpha, eps, stream);
+}
+
+extern "C" int madrl_standardize_obs_terminal_bf16(int T, int E, size_t per_env, void* x_dev, void* term_dev,
+                                                   const uint8_t* done_dev, double* mean_dev, double* var_dev,
+                                                   double alpha, double eps, void* stream) {
+  return standardize_obs_terminal(T, E, per_env, (uint16_t*)x_dev, (uint16_t*)term_dev, done_dev, mean_dev, var_dev,
+                                  alpha, eps, stream);
 }

@@ -34,6 +34,7 @@
 
 namespace madrl {
 
+template <typename O>   // observation element type: float, or uint16_t = bfloat16 bits (see obs_cvt)
 struct PEParams {
   int E, env_id_base, Np, Ne, R, off, xs, ys, n_maps, D;
   int n_catch, surround, reward_global, include_id, sample_maps, max_path_length, flatten, max_opponents;
@@ -56,15 +57,15 @@ struct PEParams {
   uint16_t* stale;                // [E][Np][R*R]  pursuer count | evader count << 8
   // trajectory tensors
   const int32_t* actions;         // [T][E][Np]
-  float* obs;                     // [T][E][Np][D]
+  O* obs;                         // [T][E][Np][D]
   float* rew;                     // [T][E][Np]
   uint8_t* done;                  // [T][E]
   int32_t* info;                  // [T][E]  removed
   const uint8_t* mask;
-  float* term_obs;                // optional [T][E][Np][D]: terminal observations of done steps
+  O* term_obs;                    // optional [T][E][Np][D]: terminal observations of done steps
   // in-kernel action source (POLICY instantiation, madrl_pursuit_rollout_heuristic): the reference's
   // hand-written policy (heuristics/pursuit.py:18-50) closes the loop inside the launch
-  const float* policy_obs0;       // [E][Np][D] the observation the FIRST action is computed from
+  const O* policy_obs0;           // [E][Np][D] the observation the FIRST action is computed from
   int32_t* actions_out;           // [T][E][Np] the actions taken (NULL = not recorded)
   int policy_c2;                  // twice the policy's window centre: R (x = R/2) or 2*(R//2) (Python 2 `/`)
   uint8_t policy_lut[128];        // window cell of the nearest visible evader -> action (host-computed, see pe_policy_table)
@@ -102,8 +103,8 @@ __device__ __forceinline__ double numpy_mean(const double* a, int n) {
 // (a separate instantiation: the open-loop kernel carries none of its instructions).
 // FLAT = flatten=True layout (3R^2 [+1]); false = the (R, R, 4) conv layout: compile-time, so the window loop has no
 // layout branch.
-template <int EPL, int CPL, int RC, bool POLICY, bool FLAT>
-__global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEParams p) {
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
+__global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEParams<O> p) {
   extern __shared__ __align__(16) uint32_t smem_u32[];
   const int lane = threadIdx.x, wib = 0;
   const int warp_global = blockIdx.x;
@@ -172,7 +173,7 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
     bool rebuild = true;   // cell words must be (re)built from map + positions
     int coff = -1;   // word offset of draw `ctr` inside the warp's cache of 32 Philox blocks (warp-uniform); < 0 = cache empty
 
-    float* obs_t = p.obs + (size_t)e * Np * p.D;
+    O* obs_t = p.obs + (size_t)e * Np * p.D;
     float* rew_t = p.rew + (size_t)e * Np + lane;
     const int32_t* act_t = p.actions + (size_t)e * Np + lane;
     size_t te = (size_t)e;
@@ -180,13 +181,13 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
     // POLICY: pursuer `lane`'s action for the NEXT step, first from the caller's observation
     int next_act = 4;
     if constexpr (POLICY) {
-      const float* o0 = p.policy_obs0 + (size_t)e * Np * p.D;
+      const O* o0 = p.policy_obs0 + (size_t)e * Np * p.D;
       for (int i = 0; i < Np; ++i, o0 += p.D) {
         uint32_t key = 0xffffffffu;
 #pragma unroll
         for (int it = 0; it < CPL; ++it) {
           const int w = lane + 32 * it;
-          if (w < RR && (FLAT ? o0[2 * RR + w] : o0[4 * w + 2]) > 0.0f) key = min(key, pkey[it]);
+          if (w < RR && obs_widen<float>(FLAT ? o0[2 * RR + w] : o0[4 * w + 2]) > 0.0f) key = min(key, pkey[it]);
         }
         key = __reduce_min_sync(FULL_MASK, key);
         if (lane == i)
@@ -366,7 +367,7 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
         }
         // ---- collect_obs: pe:418-461 (flatten): channel-major, then x, then y, then id ----------
         {
-          float* row = obs_t;
+          O* row = obs_t;
           uint32_t st_row = stale_a + 2u * lane;
           for (int i = 0; i < Np; ++i, row += p.D, st_row += 2u * RR) {
             const int pxi = __shfl_sync(FULL_MASK, px, i), pyi = __shfl_sync(FULL_MASK, py, i);
@@ -408,14 +409,15 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
                 const int w = lane + 32 * it;
                 if (w < RR) {
                   const float v0 = inb[it] ? ((wv[it] & 0xff) ? p.one_val : 0.0f) : p.wall_val;   // pe:433,438
-                  store_stream(row + w, v0);
-                  store_stream(row + RR + w, v1[it]);
-                  store_stream(row + 2 * RR + w, v2[it]);
+                  store_stream(row + w, obs_cvt<O>(v0));
+                  store_stream(row + RR + w, obs_cvt<O>(v1[it]));
+                  store_stream(row + 2 * RR + w, obs_cvt<O>(v2[it]));
                 }
               }
             } else {
               // flatten=False: np.rollaxis(local_obs[i], 0, 3) -> [x][y][channel], channel 3 holds
-              // i/Np at the window centre and zeros elsewhere (pe:440-449): one 16-byte store per cell
+              // i/Np at the window centre and zeros elsewhere (pe:440-449): one 16-byte store per cell (8 bytes
+              // in bfloat16)
               const float idval = __shfl_sync(FULL_MASK, my_idv, i);
               const int centre = (R / 2) * R + (R / 2);
 #pragma unroll
@@ -423,12 +425,17 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
                 const int w = lane + 32 * it;
                 if (w < RR) {
                   const float v0 = inb[it] ? ((wv[it] & 0xff) ? p.one_val : 0.0f) : p.wall_val;
-                  __stcs(reinterpret_cast<float4*>(row) + w, make_float4(v0, v1[it], v2[it], w == centre ? idval : 0.0f));
+                  const float v3 = w == centre ? idval : 0.0f;
+                  if constexpr (sizeof(O) == 2)
+                    __stcs(reinterpret_cast<unsigned long long*>(row) + w,
+                           (unsigned long long)bf16x2_rn(v0, v1[it]) | ((unsigned long long)bf16x2_rn(v2[it], v3) << 32));
+                  else
+                    __stcs(reinterpret_cast<float4*>(row) + w, make_float4(v0, v1[it], v2[it], v3));
                 }
               }
             }
           }
-          if (FLAT && n_tail && lane < Np) store_stream(obs_t + (size_t)lane * p.D + 3 * RR, my_idv);   // pe:444-445
+          if (FLAT && n_tail && lane < Np) store_stream(obs_t + (size_t)lane * p.D + 3 * RR, obs_cvt<O>(my_idv));   // pe:444-445
         }
         need_reset = false;
         if (!pass) {
@@ -505,7 +512,7 @@ struct madrl_pursuit : EngineCore {
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Np = cfg.n_pursuers;
-    return {E * Np * 4, E * Np * lay.obs_dim * 4, E * Np * 4, E, E * 4};
+    return {E * Np * 4, E * Np * lay.obs_dim * obs_elem_bytes(4), E * Np * 4, E, E * 4};
   }
 };
 
@@ -618,6 +625,10 @@ extern "C" int madrl_pursuit_set_terminal_obs(madrl_pursuit* h, void* term_obs_d
   return engine_set_terminal_obs(h, term_obs_dev);
 }
 
+extern "C" int madrl_pursuit_set_obs_format(madrl_pursuit* h, int format) {
+  return engine_set_obs_format(h, format, false);
+}
+
 extern "C" int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
@@ -653,31 +664,32 @@ void pe_policy_table(int R, int c2, uint8_t* lut) {
   }
 }
 
-template <int EPL, int CPL, int RC, bool POLICY, bool FLAT>
-static int pe_launch_inst3(madrl_pursuit* h, PEParams& p, cudaStream_t stream) {
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
+static int pe_launch_inst3(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)p.smem_per_warp;   // block LUT + per-warp regions
   MADRL_REQUIRE(smem <= 200 * 1024, "map too large for shared memory (%zu B per block)", smem);
-  return engine_launch(h, pe_kernel<EPL, CPL, RC, POLICY, FLAT>, smem, p.E, stream, p);
+  return engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT>, smem, p.E, stream, p);
 }
 
-template <int EPL, int CPL, int RC, bool POLICY>
-static int pe_launch_inst2(madrl_pursuit* h, PEParams& p, cudaStream_t stream) {
-  return p.flatten ? pe_launch_inst3<EPL, CPL, RC, POLICY, true>(h, p, stream)
-                   : pe_launch_inst3<EPL, CPL, RC, POLICY, false>(h, p, stream);
+template <typename O, int EPL, int CPL, int RC, bool POLICY>
+static int pe_launch_inst2(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
+  return p.flatten ? pe_launch_inst3<O, EPL, CPL, RC, POLICY, true>(h, p, stream)
+                   : pe_launch_inst3<O, EPL, CPL, RC, POLICY, false>(h, p, stream);
 }
 
-template <int EPL, int CPL, int RC>
-static int pe_launch_inst(madrl_pursuit* h, PEParams& p, cudaStream_t stream) {
-  return p.policy_obs0 != nullptr ? pe_launch_inst2<EPL, CPL, RC, true>(h, p, stream)
-                                  : pe_launch_inst2<EPL, CPL, RC, false>(h, p, stream);
+template <typename O, int EPL, int CPL, int RC>
+static int pe_launch_inst(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
+  return p.policy_obs0 != nullptr ? pe_launch_inst2<O, EPL, CPL, RC, true>(h, p, stream)
+                                  : pe_launch_inst2<O, EPL, CPL, RC, false>(h, p, stream);
 }
 
-static int pe_launch(madrl_pursuit* h, int mode, int T, const int32_t* actions, float* obs, float* rew,
-                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream,
-                     const float* policy_obs0 = nullptr, int32_t* actions_out = nullptr, int policy_c2 = 0) {
+template <typename O>
+static int pe_launch_t(madrl_pursuit* h, int mode, int T, const int32_t* actions, void* obs, float* rew,
+                       uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream,
+                       const void* policy_obs0, int32_t* actions_out, int policy_c2) {
   const madrl_pursuit_config& c = h->cfg;
-  PEParams p;
-  p.policy_obs0 = policy_obs0; p.actions_out = actions_out; p.policy_c2 = policy_c2;
+  PEParams<O> p;
+  p.policy_obs0 = (const O*)policy_obs0; p.actions_out = actions_out; p.policy_c2 = policy_c2;
   memset(p.policy_lut, 4, sizeof(p.policy_lut));
   if (policy_obs0 != nullptr) pe_policy_table(c.obs_range, policy_c2, p.policy_lut);
   p.E = c.n_envs; p.env_id_base = c.env_id_base; p.Np = c.n_pursuers; p.Ne = c.n_evaders;
@@ -705,10 +717,10 @@ static int pe_launch(madrl_pursuit* h, int mode, int T, const int32_t* actions, 
   p.pos = (uint8_t*)(st + h->lay.pos); p.gone = (uint64_t*)(st + h->lay.gone);
   p.map_id = (int32_t*)(st + h->lay.map_id); p.path_len = (int32_t*)(st + h->lay.path_len);
   p.ctr = (uint64_t*)(st + h->lay.rng_counter); p.stale = (uint16_t*)(st + h->lay.stale);
-  p.actions = actions; p.obs = obs; p.rew = rew; p.done = done; p.info = info; p.mask = mask;
-  p.term_obs = (mode == 0) ? (float*)h->term_obs : nullptr;
+  p.actions = actions; p.obs = (O*)obs; p.rew = rew; p.done = done; p.info = info; p.mask = mask;
+  p.term_obs = (mode == 0) ? (O*)h->term_obs : nullptr;
   const int epl = (p.Ne + 31) / 32, cpl = (RR + 31) / 32;
-#define MADRL_PE_CASE(EP, CP, RC_) return pe_launch_inst<EP, CP, RC_>(h, p, stream)
+#define MADRL_PE_CASE(EP, CP, RC_) return pe_launch_inst<O, EP, CP, RC_>(h, p, stream)
   if (p.R == 7) { if (epl == 1) MADRL_PE_CASE(1, 2, 7); MADRL_PE_CASE(2, 2, 7); }
   if (cpl == 1) { if (epl == 1) MADRL_PE_CASE(1, 1, 0); MADRL_PE_CASE(2, 1, 0); }
   if (cpl == 2) { if (epl == 1) MADRL_PE_CASE(1, 2, 0); MADRL_PE_CASE(2, 2, 0); }
@@ -717,12 +729,20 @@ static int pe_launch(madrl_pursuit* h, int mode, int T, const int32_t* actions, 
 #undef MADRL_PE_CASE
 }
 
-extern "C" int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, float* obs_dev, void* stream) {
+static int pe_launch(madrl_pursuit* h, int mode, int T, const int32_t* actions, void* obs, float* rew,
+                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream,
+                     const void* policy_obs0 = nullptr, int32_t* actions_out = nullptr, int policy_c2 = 0) {
+  return h->obs_format == MADRL_OBS_BF16
+             ? pe_launch_t<uint16_t>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out, policy_c2)
+             : pe_launch_t<float>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out, policy_c2);
+}
+
+extern "C" int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, void* obs_dev, void* stream) {
   MADRL_REQUIRE(h != nullptr && obs_dev != nullptr, "handle/obs is NULL");
   return pe_launch(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
 }
 
-extern "C" int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, float* obs_dev,
+extern "C" int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, void* obs_dev,
                                      float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
                                      int auto_reset, void* stream) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
@@ -731,8 +751,8 @@ extern "C" int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* act
   return pe_launch(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
 }
 
-extern "C" int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const float* obs0_dev, int32_t* actions_out_dev,
-                                               float* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
+extern "C" int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const void* obs0_dev, int32_t* actions_out_dev,
+                                               void* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
                                                int auto_reset, int floor_centre, void* stream) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
   MADRL_REQUIRE(T >= 1, "T must be >= 1");
@@ -743,27 +763,27 @@ extern "C" int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const fl
                    obs0_dev, actions_out_dev, floor_centre ? 2 * (R / 2) : R);
 }
 
-extern "C" int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, float* obs_dev, float* rew_dev,
+extern "C" int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, void* obs_dev, float* rew_dev,
                                   uint8_t* done_dev, int32_t* info_dev, int auto_reset, void* stream) {
   return madrl_pursuit_rollout(h, 1, actions_dev, obs_dev, rew_dev, done_dev, info_dev, auto_reset, stream);
 }
 
-extern "C" int madrl_pursuit_reset_host(madrl_pursuit* h, const uint8_t* mask_host, float* obs_host) {
+extern "C" int madrl_pursuit_reset_host(madrl_pursuit* h, const uint8_t* mask_host, void* obs_host) {
   return engine_reset_host(h, mask_host, obs_host,
-                           [h](uint8_t* mask, char* obs) { return madrl_pursuit_reset(h, mask, (float*)obs, nullptr); });
+                           [h](uint8_t* mask, char* obs) { return madrl_pursuit_reset(h, mask, obs, nullptr); });
 }
 
-extern "C" int madrl_pursuit_rollout_host2(madrl_pursuit* h, int T, const int32_t* actions_host, float* obs_host,
+extern "C" int madrl_pursuit_rollout_host2(madrl_pursuit* h, int T, const int32_t* actions_host, void* obs_host,
                                            float* rew_host, uint8_t* done_host, int32_t* info_host, int auto_reset,
                                            int flags) {
   return engine_rollout_host(h, T, actions_host, obs_host, rew_host, done_host, info_host, flags,
                              [&](int Tc, char* a, char* o, char* r, char* d, char* i, cudaStream_t st) {
-                               return madrl_pursuit_rollout(h, Tc, (const int32_t*)a, (float*)o, (float*)r, (uint8_t*)d,
+                               return madrl_pursuit_rollout(h, Tc, (const int32_t*)a, o, (float*)r, (uint8_t*)d,
                                                             (int32_t*)i, auto_reset, st);
                              });
 }
 
-extern "C" int madrl_pursuit_rollout_host(madrl_pursuit* h, int T, const int32_t* actions_host, float* obs_host,
+extern "C" int madrl_pursuit_rollout_host(madrl_pursuit* h, int T, const int32_t* actions_host, void* obs_host,
                                           float* rew_host, uint8_t* done_host, int32_t* info_host, int auto_reset) {
   return madrl_pursuit_rollout_host2(h, T, actions_host, obs_host, rew_host, done_host, info_host, auto_reset, 0);
 }

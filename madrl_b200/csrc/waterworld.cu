@@ -29,7 +29,7 @@
 
 namespace madrl {
 
-template <typename real>
+template <typename real, typename O = real>   // O: observation element type (see obs_cvt)
 struct WWParams {
   int E, env_id_base, Np, Ne, Npo, K, n_coop, D, Nall;
   int reward_global, addid, speed_features, random_obstacle, timestep_limit, max_path_length;
@@ -54,15 +54,15 @@ struct WWParams {
   const real* sensors;  // [2][K]
   // trajectory tensors
   const real* actions;
-  real* obs;
+  O* obs;
   real* rew;
   uint8_t* done;
   int32_t* info;
   const uint8_t* mask;
-  real* term_obs;   // optional [T][E][A][D]: terminal observations of done steps (see keep_terminal_rows)
+  O* term_obs;      // optional [T][E][A][D]: terminal observations of done steps (see keep_terminal_rows)
   // in-kernel action source (POLICY instantiation, madrl_ww_rollout_heuristic): the reference's hand-written
   // policy (heuristics/waterworld.py:11-53) closes the loop inside the launch -- no action tensor is read
-  const real* policy_obs0;   // [E][Np][D] the observation the FIRST action is computed from
+  const O* policy_obs0;      // [E][Np][D] the observation the FIRST action is computed from
   real* actions_out;         // [T][E][Np][2] the actions taken (NULL = not recorded)
   // fused per-rollout exchange (multi-GPU): every rank also stores its reward / done / info rows
   // into slot `peer_rank` of each destination gather buffer through NVLink peer mappings (CUDA
@@ -129,15 +129,15 @@ constexpr size_t kStepStageMaxBytes = 6 * 1024;
 // Shared address of element 0 of `row` (a row of the env-step starting at `obs_t`), after waiting for
 // the bulk store that last read that memory: the previous step's (whole-step staging, first row of
 // the step) or the one two rows ago (ring slot `slot_off`).
-template <typename real>
+template <typename O>
 __device__ __forceinline__ uint32_t obs_row_stage(bool whole_step, uint32_t stage, uint32_t slot_off,
-                                                  const real* obs_t, const real* row, int lane) {
+                                                  const O* obs_t, const O* row, int lane) {
   if (whole_step) {
     if (row == obs_t) {
       if (lane == 0) bulk_wait_read_all();
       __syncwarp();
     }
-    return stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)((row - obs_t) * sizeof(real));
+    return stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)((row - obs_t) * sizeof(O));
   }
   if (lane == 0) bulk_wait_read_all_but_1();
   __syncwarp();
@@ -148,19 +148,19 @@ __device__ __forceinline__ uint32_t obs_row_stage(bool whole_step, uint32_t stag
 // (HBM then sees whole sectors from one writer), the <= 16 bytes outside it on either side by
 // direct stores of one lane per element.  Full writes, no read-back, so the rows are bit-identical
 // to per-lane stores.
-template <typename real>
-__device__ __forceinline__ void obs_row_store(uint32_t slot, real* row, int n, int lane) {
+template <typename O>
+__device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int lane) {
   fence_async_shared();   // this lane's shared stores -> visible to the async proxy ...
   __syncwarp();           // ... before lane 0 issues the copy; the edge lanes read other lanes' values
-  const uintptr_t g0 = (uintptr_t)row, g1 = g0 + (uintptr_t)n * sizeof(real);
+  const uintptr_t g0 = (uintptr_t)row, g1 = g0 + (uintptr_t)n * sizeof(O);
   const uintptr_t a0 = (g0 + 15u) & ~(uintptr_t)15u, a1 = g1 & ~(uintptr_t)15u;
   const bool bulk = a1 > a0;
   if (lane == 0 && bulk) bulk_store_stream((void*)a0, slot + (uint32_t)(a0 - (g0 & ~(uintptr_t)15u)), (uint32_t)(a1 - a0));
-  const int head = bulk ? (int)((a0 - g0) / sizeof(real)) : n;
-  const int tail = bulk ? (int)((g1 - a1) / sizeof(real)) : 0;
+  const int head = bulk ? (int)((a0 - g0) / sizeof(O)) : n;
+  const int tail = bulk ? (int)((g1 - a1) / sizeof(O)) : 0;
   if (lane < head + tail) {
     const int i = lane < head ? lane : n - tail + (lane - head);
-    store_stream(row + i, lds_real<real>(slot + ((uint32_t)g0 & 15u) + (uint32_t)(i * sizeof(real))));
+    store_stream(row + i, lds_obs<O>(slot + ((uint32_t)g0 & 15u) + (uint32_t)(i * sizeof(O))));
   }
 }
 
@@ -171,9 +171,9 @@ __device__ __forceinline__ void obs_row_store(uint32_t slot, real* row, int n, i
 // carries none of its registers).
 // POLICY = the actions come from the in-kernel heuristic policy instead of the action tensor (again a
 // separate instantiation: the open-loop kernel carries none of its instructions).
-template <typename real, int OPL, int KCH, int KC, bool PEER, bool POLICY = false>
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false>
 __global__ void __launch_bounds__(32, (OPL <= 4 ? 28 : 16))
-ww_kernel(const __grid_constant__ WWParams<real> p) {
+ww_kernel(const __grid_constant__ WWParams<real, O> p) {
   const real INF = real_inf<real>();
   const int K = KC > 0 ? KC : p.K;
   // 32-thread blocks: the env index derives from blockIdx alone, so ptxas can prove every loop and
@@ -215,7 +215,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
   const bool speed = KC > 0 ? true : (p.speed_features != 0);
   const int n_feat = speed ? 7 : 4;
   const uint32_t stage = slots + (SMEM ? (uint32_t)Nall * CandSlot<real>::kStride : 0u);
-  const uint32_t slot_bytes = obs_stage_bytes(n_feat * K, sizeof(real));
+  const uint32_t slot_bytes = obs_stage_bytes(n_feat * K, sizeof(O));
   uint32_t slot_off = 0u;   // row-by-row staging: ring slot of the next row, 0 or slot_bytes
   typedef typename Vec2<real>::type V2;
 
@@ -241,7 +241,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
     uint64_t ctr = p.ctr[e];
 
     // running output pointers: the env's first pursuer row at step t (warp-uniform), this lane's reward
-    real* obs_t = p.obs + (size_t)e * p.Np * p.D;
+    O* obs_t = p.obs + (size_t)e * p.Np * p.D;
     real* rew_t = p.rew + (size_t)e * p.Np + lane;
     size_t te = (size_t)e;   // index of (t, e) in the [T][E] done / info tensors
     int pass = (p.mode == 1) ? 1 : 0;  // pass 1 = reset pass: fresh draws, zero action, obs only
@@ -251,16 +251,18 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
     // first from the caller's observation, afterwards from the features this warp has just computed
     real pax = 0, pay = 0;
     if constexpr (POLICY) {
-      const real* o0 = p.policy_obs0 + (size_t)e * p.Np * p.D;
+      // (bf16 obs0: the widened values -- the first decision after a launch boundary sees rounded features)
+      const O* o0 = p.policy_obs0 + (size_t)e * p.Np * p.D;
       for (int pi = 0; pi < p.Np; ++pi, o0 += p.D) {
-        const real cE = o0[7 * K] > (real)0 ? (real)1.5 : (real)1;        // heuristics/waterworld.py:41
-        const real cP = o0[7 * K + 1] > (real)0 ? (real)1.5 : (real)1;    // :42
+        const real cE = obs_widen<real>(o0[7 * K]) > (real)0 ? (real)1.5 : (real)1;        // heuristics/waterworld.py:41
+        const real cP = obs_widen<real>(o0[7 * K + 1]) > (real)0 ? (real)1.5 : (real)1;    // :42
         real wx = 0, wy = 0;
 #pragma unroll
         for (int kc = 0; kc < KCH; ++kc) {
           const int k = lane + 32 * kc;
           if (k < K) {
-            const real w = (real)0.5 * o0[5 * K + k] + (cE * o0[K + k] - o0[k]) - cP * o0[3 * K + k];
+            const real w = (real)0.5 * obs_widen<real>(o0[5 * K + k]) +
+                           (cE * obs_widen<real>(o0[K + k]) - obs_widen<real>(o0[k])) - cP * obs_widen<real>(o0[3 * K + k]);
             wx += w * sx_l[kc]; wy += w * sy_l[kc];
           }
         }
@@ -355,7 +357,7 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
           if (dx * dx + dy * dy <= thr) { vx[c] = kf * vx[c]; vy[c] = kf * vy[c]; }
         }
         // ---- sense: one pursuer at a time -----------------------------------------------------
-        real* obs_row = obs_t;
+        O* obs_row = obs_t;
         for (int pi = 0; pi < p.Np; ++pi, obs_row += p.D) {
           const real mx = __shfl_sync(FULL_MASK, x[0], pi), my = __shfl_sync(FULL_MASK, y[0], pi);
           const real mvx = __shfl_sync(FULL_MASK, vx[0], pi), mvy = __shfl_sync(FULL_MASK, vy[0], pi);
@@ -425,8 +427,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
               const int k = lane + 32 * kc;
               const bool hO = bO[kc] < INF, hE = bE[kc] < up, hP = bP[kc] < up, hU = bU[kc] < up;
               const real z = (real)0;
-              const uint32_t o = srow + (uint32_t)(k * sizeof(real));   // this lane's column
-              constexpr uint32_t R = sizeof(real);
+              const uint32_t o = srow + (uint32_t)(k * sizeof(O));   // this lane's column
+              constexpr uint32_t R = sizeof(O);
               if constexpr (POLICY) {
                 if (k < K) {
                   const real w = (real)0.5 * (hU ? bU[kc] : z) + ((tE ? (real)1.5 : (real)1) * (hE ? bE[kc] : z) - (hO ? bO[kc] : z)) -
@@ -441,19 +443,19 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
                 CandSlot<real>::vel(aP[kc], oPx, oPy);
                 CandSlot<real>::vel(aU[kc], oUx, oUy);
                 if (k < K) {
-                  sts_real(o + 0 * K * R, hO ? bO[kc] : z);
-                  sts_real(o + 1 * K * R, hE ? bE[kc] : z);
-                  sts_real(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
-                  sts_real(o + 3 * K * R, hP ? bP[kc] : z);
-                  sts_real(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
-                  sts_real(o + 5 * K * R, hU ? bU[kc] : z);
-                  sts_real(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
+                  stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
+                  stage_obs<O>(o + 1 * K * R, hE ? bE[kc] : z);
+                  stage_obs<O>(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
+                  stage_obs<O>(o + 3 * K * R, hP ? bP[kc] : z);
+                  stage_obs<O>(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
+                  stage_obs<O>(o + 5 * K * R, hU ? bU[kc] : z);
+                  stage_obs<O>(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
                 }
               } else if (k < K) {
-                sts_real(o + 0 * K * R, hO ? bO[kc] : z);
-                sts_real(o + 1 * K * R, hE ? bE[kc] : z);
-                sts_real(o + 2 * K * R, hP ? bP[kc] : z);
-                sts_real(o + 3 * K * R, hU ? bU[kc] : z);
+                stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
+                stage_obs<O>(o + 1 * K * R, hE ? bE[kc] : z);
+                stage_obs<O>(o + 2 * K * R, hP ? bP[kc] : z);
+                stage_obs<O>(o + 3 * K * R, hU ? bU[kc] : z);
               }
             }
             __syncwarp();   // the next pursuer's staging overwrites the slots
@@ -495,8 +497,8 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
             const int k = lane + 32 * kc;
             const bool hO = bO[kc] < INF, hE = bE[kc] < INF, hP = bP[kc] < INF, hU = bU[kc] < INF;
             const real z = (real)0;
-            const uint32_t o = srow + (uint32_t)(k * sizeof(real));   // this lane's column
-            constexpr uint32_t R = sizeof(real);
+            const uint32_t o = srow + (uint32_t)(k * sizeof(O));   // this lane's column
+            constexpr uint32_t R = sizeof(O);
             if constexpr (POLICY) {
               if (k < K) {
                 const real w = (real)0.5 * (hU ? bU[kc] : z) + ((tE ? (real)1.5 : (real)1) * (hE ? bE[kc] : z) - (hO ? bO[kc] : z)) -
@@ -523,19 +525,19 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
                 }
               }
               if (k < K) {
-                sts_real(o + 0 * K * R, hO ? bO[kc] : z);
-                sts_real(o + 1 * K * R, hE ? bE[kc] : z);
-                sts_real(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
-                sts_real(o + 3 * K * R, hP ? bP[kc] : z);
-                sts_real(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
-                sts_real(o + 5 * K * R, hU ? bU[kc] : z);
-                sts_real(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
+                stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
+                stage_obs<O>(o + 1 * K * R, hE ? bE[kc] : z);
+                stage_obs<O>(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
+                stage_obs<O>(o + 3 * K * R, hP ? bP[kc] : z);
+                stage_obs<O>(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
+                stage_obs<O>(o + 5 * K * R, hU ? bU[kc] : z);
+                stage_obs<O>(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
               }
             } else if (k < K) {
-              sts_real(o + 0 * K * R, hO ? bO[kc] : z);
-              sts_real(o + 1 * K * R, hE ? bE[kc] : z);
-              sts_real(o + 2 * K * R, hP ? bP[kc] : z);
-              sts_real(o + 3 * K * R, hU ? bU[kc] : z);
+              stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
+              stage_obs<O>(o + 1 * K * R, hE ? bE[kc] : z);
+              stage_obs<O>(o + 2 * K * R, hP ? bP[kc] : z);
+              stage_obs<O>(o + 3 * K * R, hU ? bU[kc] : z);
             }
           }
           }
@@ -583,14 +585,14 @@ ww_kernel(const __grid_constant__ WWParams<real> p) {
           const real vE = (real)((whoEnc >> lane) & 1u), vP = (real)((whoP >> lane) & 1u), id = (real)(lane + 1);
           const int i = lane * p.D + n_feat * K;
           if (p.stage_step) {
-            const uint32_t a = stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)(i * sizeof(real));
-            sts_real(a, vE);
-            sts_real(a + (uint32_t)sizeof(real), vP);
-            if (p.addid) sts_real(a + 2 * (uint32_t)sizeof(real), id);
+            const uint32_t a = stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)(i * sizeof(O));
+            stage_obs<O>(a, vE);
+            stage_obs<O>(a + (uint32_t)sizeof(O), vP);
+            if (p.addid) stage_obs<O>(a + 2 * (uint32_t)sizeof(O), id);
           } else {
-            store_stream(obs_t + i, vE);
-            store_stream(obs_t + i + 1, vP);
-            if (p.addid) store_stream(obs_t + i + 2, id);
+            store_stream(obs_t + i, obs_cvt<O>(vE));
+            store_stream(obs_t + i + 1, obs_cvt<O>(vP));
+            if (p.addid) store_stream(obs_t + i + 2, obs_cvt<O>(id));
           }
         }
         if (p.stage_step) obs_row_store(stage, obs_t, p.Np * p.D, lane);
@@ -701,7 +703,7 @@ struct madrl_ww : EngineCore {
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Np = cfg.n_pursuers, rb = lay.real_bytes;
-    return {E * Np * 2 * rb, E * Np * lay.obs_dim * rb, E * Np * rb, E, E * 2 * 4};
+    return {E * Np * 2 * rb, E * Np * lay.obs_dim * obs_elem_bytes(rb), E * Np * rb, E, E * 2 * 4};
   }
 };
 
@@ -771,6 +773,10 @@ extern "C" int madrl_ww_set_terminal_obs(madrl_ww* h, void* term_obs_dev) {
   return engine_set_terminal_obs(h, term_obs_dev);
 }
 
+extern "C" int madrl_ww_set_obs_format(madrl_ww* h, int format) {
+  return engine_set_obs_format(h, format, h != nullptr && h->cfg.fp64);
+}
+
 extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
@@ -778,26 +784,29 @@ extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_
 template <typename real>
 static size_t ww_cand_bytes(int opl, int n_obj) { return opl >= 2 ? (size_t)n_obj * CandSlot<real>::kStride : 0; }
 
-template <typename real, int OPL, int KCH, int KC, bool PEER, bool POLICY>
-static int ww_launch_inst2(madrl_ww* h, const WWParams<real>& p, cudaStream_t stream) {
-  const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(real))
-                                                                        : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(real)));
-  return engine_launch(h, ww_kernel<real, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p);
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY>
+static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t stream) {
+  const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(O))
+                                                                        : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(O)));
+  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p);
 }
 
-template <typename real, int OPL, int KCH, int KC>
-static int ww_launch_inst(madrl_ww* h, const WWParams<real>& p, cudaStream_t stream) {
-  if (p.policy_obs0 != nullptr) return ww_launch_inst2<real, OPL, KCH, KC, false, true>(h, p, stream);
-  return p.n_peers > 0 ? ww_launch_inst2<real, OPL, KCH, KC, true, false>(h, p, stream)
-                       : ww_launch_inst2<real, OPL, KCH, KC, false, false>(h, p, stream);
+// The fused peer exchange is instantiated for native observations only (bf16 rollouts with peers are
+// rejected in ww_launch): it adds nothing to the observation path.
+template <typename real, typename O, int OPL, int KCH, int KC>
+static int ww_launch_inst(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t stream) {
+  if (p.policy_obs0 != nullptr) return ww_launch_inst2<real, O, OPL, KCH, KC, false, true>(h, p, stream);
+  if constexpr (sizeof(O) == sizeof(real))
+    if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, false>(h, p, stream);
+  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, stream);
 }
 
-template <typename real>
-static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* obs, void* rew,
-                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset,
-                     cudaStream_t stream, const void* policy_obs0 = nullptr, void* actions_out = nullptr) {
+template <typename real, typename O>
+static int ww_launch_t(madrl_ww* h, int mode, int T, const void* actions, void* obs, void* rew,
+                       uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset,
+                       cudaStream_t stream, const void* policy_obs0, void* actions_out) {
   const madrl_ww_config& c = h->cfg;
-  WWParams<real> p;
+  WWParams<real, O> p;
   p.E = c.n_envs; p.env_id_base = c.env_id_base;
   p.Np = c.n_pursuers; p.Ne = c.n_evaders; p.Npo = c.n_poison; p.K = c.n_sensors;
   p.n_coop = c.n_coop; p.D = h->lay.obs_dim; p.Nall = h->lay.n_obj;
@@ -833,13 +842,14 @@ static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* ob
   p.timestep = (int32_t*)(st + h->lay.timestep); p.path_len = (int32_t*)(st + h->lay.path_len);
   p.ctr = (uint64_t*)(st + h->lay.rng_counter);
   p.sensors = (const real*)(st + h->lay.sensors);
-  p.actions = (const real*)actions; p.obs = (real*)obs; p.rew = (real*)rew;
+  p.actions = (const real*)actions; p.obs = (O*)obs; p.rew = (real*)rew;
   p.done = done; p.info = info; p.mask = mask;
-  p.term_obs = (mode == 0) ? (real*)h->term_obs : nullptr;
-  p.policy_obs0 = (const real*)policy_obs0; p.actions_out = (real*)actions_out;
+  p.term_obs = (mode == 0) ? (O*)h->term_obs : nullptr;
+  p.policy_obs0 = (const O*)policy_obs0; p.actions_out = (real*)actions_out;
   // the policy instantiation is single-GPU: its rows go through the copy-engine exchange, not peer stores
   p.n_peers = (mode == 0 && policy_obs0 == nullptr) ? h->n_peers : 0;
   p.peer_rank = h->peer_rank;
+  MADRL_REQUIRE(p.n_peers == 0 || sizeof(O) == sizeof(real), "the fused peer exchange needs native observations (set_obs_format)");
   if (p.n_peers > 0) {
     MADRL_REQUIRE(T <= h->peer_tmax, "rollout of %d steps exceeds the peer buffers (t_max %d)", T, h->peer_tmax);
     p.peer_tmax = h->peer_tmax;
@@ -851,8 +861,8 @@ static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* ob
   }
 
   const int opl = (p.Nall + 31) / 32, kch = (p.K + 31) / 32;
-  p.stage_step = ww_cand_bytes<real>(opl, p.Nall) + obs_stage_bytes(p.Np * p.D, sizeof(real)) <= kStepStageMaxBytes;
-#define MADRL_WW_CASE(O, KH, KC_) return ww_launch_inst<real, O, KH, KC_>(h, p, stream)
+  p.stage_step = ww_cand_bytes<real>(opl, p.Nall) + obs_stage_bytes(p.Np * p.D, sizeof(O)) <= kStepStageMaxBytes;
+#define MADRL_WW_CASE(OP, KH, KC_) return ww_launch_inst<real, O, OP, KH, KC_>(h, p, stream)
   if (p.K == 30 && p.speed_features) {   // the reference's defaults (n_sensors = 30, speed features): compile-time K and layout
     if (opl == 1) MADRL_WW_CASE(1, 1, 30);
     if (opl == 2) MADRL_WW_CASE(2, 1, 30);
@@ -872,10 +882,20 @@ static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* ob
 #undef MADRL_WW_CASE
 }
 
+// fp64 verification build, fp32 with fp32 observations, or fp32 with bfloat16 observations
+static int ww_launch(madrl_ww* h, int mode, int T, const void* actions, void* obs, void* rew,
+                     uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset,
+                     cudaStream_t stream, const void* policy_obs0 = nullptr, void* actions_out = nullptr) {
+  if (h->cfg.fp64)
+    return ww_launch_t<double, double>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out);
+  if (h->obs_format == MADRL_OBS_BF16)
+    return ww_launch_t<float, uint16_t>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out);
+  return ww_launch_t<float, float>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out);
+}
+
 extern "C" int madrl_ww_reset(madrl_ww* h, const uint8_t* mask_dev, void* obs_dev, void* stream) {
   MADRL_REQUIRE(h != nullptr && obs_dev != nullptr, "handle/obs is NULL");
-  return h->cfg.fp64 ? ww_launch<double>(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream)
-                     : ww_launch<float>(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
+  return ww_launch(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_ww_rollout(madrl_ww* h, int T, const void* actions_dev, void* obs_dev,
@@ -885,8 +905,7 @@ extern "C" int madrl_ww_rollout(madrl_ww* h, int T, const void* actions_dev, voi
   MADRL_REQUIRE(T >= 1, "T must be >= 1");
   MADRL_REQUIRE(actions_dev && obs_dev && rew_dev && done_dev && info_dev, "NULL trajectory buffer");
   MADRL_REQUIRE(((uintptr_t)info_dev & 7) == 0, "info_dev must be 8-byte aligned (rows are stored as one 8-byte word)");
-  return h->cfg.fp64 ? ww_launch<double>(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream)
-                     : ww_launch<float>(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
+  return ww_launch(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_ww_rollout_heuristic(madrl_ww* h, int T, const void* obs0_dev, void* actions_out_dev,
@@ -899,8 +918,8 @@ extern "C" int madrl_ww_rollout_heuristic(madrl_ww* h, int T, const void* obs0_d
   MADRL_REQUIRE(((uintptr_t)actions_out_dev & (h->cfg.fp64 ? 15 : 7)) == 0, "actions_out_dev must be aligned to one (x, y) pair");
   MADRL_REQUIRE(h->cfg.speed_features, "the heuristic policy reads the 7K feature layout (speed_features=True; "
                                        "heuristics/waterworld.py:12-22)");
-  return h->cfg.fp64 ? ww_launch<double>(h, 0, T, nullptr, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream, obs0_dev, actions_out_dev)
-                     : ww_launch<float>(h, 0, T, nullptr, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream, obs0_dev, actions_out_dev);
+  return ww_launch(h, 0, T, nullptr, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream,
+                   obs0_dev, actions_out_dev);
 }
 
 extern "C" int madrl_ww_step(madrl_ww* h, const void* actions_dev, void* obs_dev, void* rew_dev,

@@ -91,17 +91,18 @@ class PackedTrajectory(object):
     tensor.  The env kernels write straight into the views.  Sections (each 16-byte aligned -- the
     kernels store info rows as 8-byte words): rew [T,E,A], info [T,E,w] int32, done [T,E] uint8 and,
     with ``obs_dim`` / ``act_shape`` given, obs [T,E,A,D] and actions [T,E,*act_shape] (the full
-    trajectory the reference's workers return, rllab/rllab/sampler/ma_sampler.py:88-100)."""
+    trajectory the reference's workers return, rllab/rllab/sampler/ma_sampler.py:88-100).  ``obs_dtype``:
+    the obs section's element type (default ``rew_dtype``; torch.bfloat16 for bfloat16-observation engines)."""
 
     def __init__(self, T, n_envs, n_agents, info_width, device, rew_dtype=torch.float32, obs_dim=0,
-                 act_shape=None, act_dtype=None):
+                 act_shape=None, act_dtype=None, obs_dtype=None):
         esz = torch.empty((), dtype=rew_dtype).element_size()
         self.shapes = dict(rew=(T, n_envs, n_agents), info=(T, n_envs, info_width) if info_width > 1 else (T, n_envs),
                            done=(T, n_envs))
         self.dtypes = dict(rew=rew_dtype, info=torch.int32, done=torch.uint8)
         if obs_dim:
             self.shapes['obs'] = (T, n_envs, n_agents, obs_dim)
-            self.dtypes['obs'] = rew_dtype
+            self.dtypes['obs'] = obs_dtype or rew_dtype
         if act_shape is not None:
             self.shapes['act'] = (T, n_envs) + tuple(act_shape)
             self.dtypes['act'] = act_dtype or rew_dtype
@@ -279,7 +280,7 @@ class AsyncRootGather(object):
     MBOX_WORDS = 64      # arrived[set][rank] at set * 8 + rank (W <= 8); released[set] at 32 + set
 
     def __init__(self, T, n_envs, n_agents, info_width, device, rew_dtype=torch.float32, root=0,
-                 n_sets=2, group=None, completion="auto", obs_dim=0, act_shape=None, act_dtype=None):
+                 n_sets=2, group=None, completion="auto", obs_dim=0, act_shape=None, act_dtype=None, obs_dtype=None):
         import ctypes as C
         from . import _lib
         assert dist.is_initialized()
@@ -290,7 +291,7 @@ class AsyncRootGather(object):
         _same_on_all_ranks((T, n_envs, n_agents, info_width, obs_dim), "(T, n_envs, n_agents, info_width, obs_dim)",
                            group)
         self.local = [PackedTrajectory(T, n_envs, n_agents, info_width, device, rew_dtype, obs_dim=obs_dim,
-                                       act_shape=act_shape, act_dtype=act_dtype) for _ in range(n_sets)]
+                                       act_shape=act_shape, act_dtype=act_dtype, obs_dtype=obs_dtype) for _ in range(n_sets)]
         nb = self.local[0].nbytes
         W, is_root = self.world, self.rank == root
         self._slots, self._own, self._opened, self.root_bufs = [], [], [], []

@@ -27,9 +27,13 @@ class BatchedEngine(object):
     _info_tail = ()   # info shape of one env
     _info_keys = ()   # step() info keys: one per info column, or a single key for the whole row
 
-    def __init__(self, cfg, n_acting, device, dtype, act_dtype, create_args=()):
-        """`n_acting`: agents that act and observe per env; `dtype`: observations and rewards;
-        `act_dtype`: actions; `create_args`: family arguments of madrl_<abi>_create before the blob."""
+    def __init__(self, cfg, n_acting, device, dtype, act_dtype, create_args=(), obs_dtype=None):
+        """`n_acting`: agents that act and observe per env; `dtype`: rewards (and state);
+        `act_dtype`: actions; `create_args`: family arguments of madrl_<abi>_create before the blob;
+        `obs_dtype`: observations, `dtype` (None) or torch.bfloat16 (fp32 engines only)."""
+        obs_dtype = dtype if obs_dtype is None else obs_dtype
+        if obs_dtype not in (dtype, torch.bfloat16) or (obs_dtype == torch.bfloat16 and dtype != torch.float32):
+            raise ValueError("obs_dtype must be %s or torch.bfloat16 (with float32 rewards), got %s" % (dtype, obs_dtype))
         if not torch.cuda.is_available():
             raise _lib.EngineError("madrl_b200 needs a CUDA device (there is no CPU fallback)")
         self._L = _lib.lib()
@@ -46,6 +50,9 @@ class BatchedEngine(object):
             h = C.c_void_p()
             _lib.check(self._fn("create")(C.byref(cfg), *create_args, _ptr(self._blob), C.byref(h)))
         self._h = h
+        self.obs_dtype = obs_dtype
+        if obs_dtype == torch.bfloat16:
+            _lib.check(self._fn("set_obs_format")(self._h, _lib.OBS_BF16))
 
     def _fn(self, name):
         return getattr(self._L, "madrl_%s_%s" % (self._abi, name))
@@ -63,12 +70,14 @@ class BatchedEngine(object):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
     def set_terminal_obs(self, term_obs):
-        """Keep the terminal observations of done steps: `term_obs` (same shape / dtype as the obs tensor
+        """Keep the terminal observations of done steps: `term_obs` (same shape / obs_dtype as the obs tensor
         of the following auto-reset rollouts) receives, at the [t, e] slots where `done` is set, the
         observation the env returned BEFORE it was reset in place (StandardizedEnv needs it,
         madrl_environments/__init__.py:283-291).  None switches it off."""
         if term_obs is not None:
             assert term_obs.is_contiguous() and term_obs.device == self.device, "term_obs must be a contiguous device tensor"
+            if term_obs.dtype != self.obs_dtype:
+                raise TypeError("term_obs must be %s, got %s" % (self.obs_dtype, term_obs.dtype))
         self._term_keepalive = term_obs
         _lib.check(self._fn("set_terminal_obs")(self._h, _ptr(term_obs)))
 
@@ -83,9 +92,9 @@ class BatchedEngine(object):
     def reset(self, mask=None, out=None):
         """reset() of the masked envs (all if None) -> obs [E, A, D]."""
         shape = (self.n_envs, self._n_acting, self.obs_dim)
-        obs = out if out is not None else torch.zeros(shape, dtype=self.dtype, device=self.device)
+        obs = out if out is not None else torch.zeros(shape, dtype=self.obs_dtype, device=self.device)
         if out is not None:
-            _lib.require_tensor(out, "out", self.dtype, shape, self.device)
+            _lib.require_tensor(out, "out", self.obs_dtype, shape, self.device)
         if mask is not None:
             mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
         with torch.cuda.device(self.device):
@@ -95,7 +104,7 @@ class BatchedEngine(object):
     def _trajectory_shapes(self, T):
         """(dtype, shape) of obs, rew, done and info of a T-step rollout."""
         E, A = self.n_envs, self._n_acting
-        return ((self.dtype, (T, E, A, self.obs_dim)), (self.dtype, (T, E, A)), (torch.uint8, (T, E)),
+        return ((self.obs_dtype, (T, E, A, self.obs_dim)), (self.dtype, (T, E, A)), (torch.uint8, (T, E)),
                 (torch.int32, (T, E) + self._info_tail))
 
     def _outputs(self, T, out):
@@ -103,7 +112,7 @@ class BatchedEngine(object):
         contiguity / placement, or new ones."""
         if out is None:   # spelled out: this is on the per-step path of the single-env drop-ins
             E, A, dev = self.n_envs, self._n_acting, self.device
-            return (torch.empty((T, E, A, self.obs_dim), dtype=self.dtype, device=dev),
+            return (torch.empty((T, E, A, self.obs_dim), dtype=self.obs_dtype, device=dev),
                     torch.empty((T, E, A), dtype=self.dtype, device=dev),
                     torch.empty((T, E), dtype=torch.uint8, device=dev),
                     torch.empty((T, E) + self._info_tail, dtype=torch.int32, device=dev))
@@ -127,7 +136,7 @@ class BatchedEngine(object):
     def _rollout_heuristic(self, T, obs0, auto_reset, out, record_actions, actions_out, *extra):
         """madrl_<abi>_rollout_heuristic; `extra`: the family's arguments before the stream."""
         E, A = self.n_envs, self._n_acting
-        _lib.require_tensor(obs0, "obs0", self.dtype, (E, A, self.obs_dim), self.device)
+        _lib.require_tensor(obs0, "obs0", self.obs_dtype, (E, A, self.obs_dim), self.device)
         obs, rew, done, info = self._outputs(T, out)
         act_shape = (T, E, A) + self._act_tail
         if actions_out is not None:   # caller-owned buffer for the actions taken (no allocation in a rollout loop)
@@ -158,7 +167,7 @@ class BatchedEngine(object):
         _lib.require_tensor(actions, "actions", self._act_dtype, (T, E, A) + self._act_tail, 'cpu')
         shapes = self._trajectory_shapes(T)
         if obs_last:
-            shapes = ((self.dtype, (E, A, self.obs_dim)),) + shapes[1:]
+            shapes = ((self.obs_dtype, (E, A, self.obs_dim)),) + shapes[1:]
         for t, n, (dt, s) in zip((obs, rew, done, info), ("obs", "rew", "done", "info"), shapes):
             _lib.require_tensor(t, n, dt, s, 'cpu')
         with torch.cuda.device(self.device):

@@ -50,7 +50,9 @@ def hw_config(n_envs, n_good, n_hostages, n_bad, n_coop_save, n_coop_avoid, radi
 
 
 class BatchedHostageWorld(BatchedEngine):
-    """E lockstep ContinuousHostageWorld instances resident in HBM (arguments: hostage.py:75-79)."""
+    """E lockstep ContinuousHostageWorld instances resident in HBM (arguments: hostage.py:75-79).
+    ``obs_dtype``: ``dtype`` (None) or torch.bfloat16 with float32 ``dtype`` -- observations stored as
+    bfloat16, bit-identical to the float32 ones rounded to nearest even (madrl_hostage_set_obs_format)."""
 
     timestep_limit = 1000
     _abi, _Layout, _act_tail, _info_tail, _info_keys = "hostage", _lib.HWLayout, (2,), (2,), ("ho_saved", "cr_encs")
@@ -60,7 +62,7 @@ class BatchedHostageWorld(BatchedEngine):
                  save_reward=5., hit_reward=-1., encounter_reward=0.01, not_saved_reward=-3,
                  bomb_reward=-5., bomb_radius=0.05, key_radius=0.0075, control_penalty=-.1,
                  reward_mech='global', addid=True, device=None, seed=0, env_id_base=0,
-                 max_path_length=0, dtype=torch.float32):
+                 max_path_length=0, dtype=torch.float32, obs_dtype=None):
         cfg = hw_config(n_envs, n_good, n_hostages, n_bad, n_coop_save, n_coop_avoid, radius=radius, key_loc=key_loc,
                         bad_speed=bad_speed, n_sensors=n_sensors, sensor_range=sensor_range,
                         action_scale=action_scale, save_reward=save_reward, hit_reward=hit_reward,
@@ -70,7 +72,7 @@ class BatchedHostageWorld(BatchedEngine):
                         env_id_base=env_id_base, max_path_length=max_path_length, fp64=dtype == torch.float64)
         self.n_envs, self.n_good, self.n_hostages, self.n_bad = n_envs, n_good, n_hostages, n_bad
         self.n_sensors, self.reward_mech = n_sensors, reward_mech
-        super().__init__(cfg, n_good, device, dtype, dtype)
+        super().__init__(cfg, n_good, device, dtype, dtype, obs_dtype=obs_dtype)
         self.n_obj = int(self.layout.n_obj)
 
     @property

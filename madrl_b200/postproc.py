@@ -24,11 +24,28 @@ def _stream(dev):
     return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
+def _require_dtype(t, name, dtypes=(torch.float32,)):
+    """The passes read and write raw buffers: a tensor of another dtype must not reach them."""
+    if t is not None and t.dtype not in dtypes:
+        raise TypeError("%s must be %s, got %s" % (name, " or ".join(str(d) for d in dtypes), t.dtype))
+
+
+def _obs_fn(name, dtype):
+    """The f32 or bf16 entry point of an observation pass."""
+    return getattr(_lib.lib(), "madrl_%s_%s" % (name, "bf16" if dtype == torch.bfloat16 else "f32"))
+
+
+_OBS_DTYPES = (torch.float32, torch.bfloat16)
+
+
 def gae(rew, values, done, discount, gae_lambda, last_value=None):
     """rew, values [T,E,A] float32 cuda; done [T,E] uint8 -> (advantages, returns) [T,E,A].
 
     Paths end where ``done`` is set (bootstrap 0, base.py:57) and at the end of the rollout
     (bootstrap ``last_value`` [E,A] if given, else 0)."""
+    for t, n in ((rew, "rew"), (values, "values"), (last_value, "last_value")):
+        _require_dtype(t, n)
+    _require_dtype(done, "done", (torch.uint8,))
     rew, values, done = rew.contiguous(), values.contiguous(), done.contiguous()
     T, E, A = rew.shape
     adv, ret = torch.empty_like(rew), torch.empty_like(rew)
@@ -52,6 +69,7 @@ def center_advantages(adv, center=True, positive=False, inplace=False):
     """``util.center_advantages`` / ``util.shift_advantages_to_positive`` over every sample of the
     batch (base.py:82-86 applies them to the concatenation of all paths): float64 mean / population
     std / min computed on the device, deterministic.  Returns the processed tensor (same shape)."""
+    _require_dtype(adv, "adv")
     out = adv.contiguous() if inplace else adv.contiguous().clone()
     stats, ws = _moments_buffers(out.device)
     with torch.cuda.device(out.device):
@@ -64,6 +82,8 @@ def center_advantages(adv, center=True, positive=False, inplace=False):
 def moments(a, b=None):
     """float64 [9] cuda tensor: means, population variances and minima of the series a, b, b - a
     taken over every element (NumPy's two-pass ``var``)."""
+    _require_dtype(a, "a")
+    _require_dtype(b, "b")
     a = a.contiguous()
     b = b.contiguous() if b is not None else None
     assert b is None or b.numel() == a.numel()
@@ -86,26 +106,33 @@ def explained_variance(ypred, y):
 
 class FrameStack(object):
     """ObservationBuffer for a whole env batch: the last ``buffer_size`` observations of every
-    agent stacked on a new minor axis; a reset fills every slot with the reset observation."""
+    agent stacked on a new minor axis; a reset fills every slot with the reset observation.
+    ``dtype``: the observations' (torch.float32, or torch.bfloat16 for an engine built with
+    ``obs_dtype=torch.bfloat16``); the stack keeps it (values are only moved)."""
 
-    def __init__(self, n_envs, n_agents, obs_dim, buffer_size, device):
-        self.shape = (n_envs, n_agents, obs_dim, buffer_size)
-        self.carry = torch.zeros(self.shape, dtype=torch.float32, device=device)   # __init__.py:150
+    def __init__(self, n_envs, n_agents, obs_dim, buffer_size, device, dtype=torch.float32):
+        _require_dtype(torch.empty(0, dtype=dtype), "dtype", _OBS_DTYPES)
+        self.shape, self.dtype = (n_envs, n_agents, obs_dim, buffer_size), dtype
+        self.carry = torch.zeros(self.shape, dtype=dtype, device=device)   # __init__.py:150
 
     def reset(self, obs0):
         """obs0 [E,A,D] from engine.reset() -> stacked [E,A,D,B] (__init__.py:186-196)."""
+        _require_dtype(obs0, "obs0", (self.dtype,))
         self.carry.copy_(obs0.unsqueeze(-1).expand(self.shape))
         return self.carry.clone()
 
     def rollout(self, obs, done):
         """obs [T,E,A,D], done [T,E] from engine.rollout(auto_reset=True) -> [T,E,A,D,B]."""
+        _require_dtype(obs, "obs", (self.dtype,))
+        _require_dtype(done, "done", (torch.uint8,))
         obs, done = obs.contiguous(), done.contiguous()
         T = obs.shape[0]
         E, A, D, B = self.shape
-        out = torch.empty((T, E, A, D, B), dtype=torch.float32, device=obs.device)
+        assert tuple(obs.shape) == (T, E, A, D) and tuple(done.shape) == (T, E), (obs.shape, done.shape)
+        out = torch.empty((T, E, A, D, B), dtype=self.dtype, device=obs.device)
         with torch.cuda.device(obs.device):
-            _lib.check(_lib.lib().madrl_frame_stack_f32(T, E, A, D, B, _ptr(obs), _ptr(done),
-                                                        _ptr(self.carry), _ptr(out), _stream(obs.device)))
+            _lib.check(_obs_fn("frame_stack", self.dtype)(T, E, A, D, B, _ptr(obs), _ptr(done),
+                                                          _ptr(self.carry), _ptr(out), _stream(obs.device)))
         return out
 
 
@@ -129,28 +156,34 @@ class Standardizer(object):
 
     def obs(self, obs, done=None, terminal_obs=None):
         """In place on obs [T,E,A,D] (or [E,A,D]); with `done` [T,E] and `terminal_obs` [T,E,A,D] the
-        terminal observations update the estimate first (and are standardised in place as well)."""
+        terminal observations update the estimate first (and are standardised in place as well).
+        float32 or bfloat16 observations; bfloat16 ones take the same float64 arithmetic on the widened
+        values and are rounded once, at the store."""
         if not self.enable_obsnorm:
             return obs
+        _require_dtype(obs, "obs", _OBS_DTYPES)
         x = obs if obs.dim() == 4 else obs.unsqueeze(0)
-        assert x.is_contiguous()
+        assert x.is_contiguous() and x[0].numel() == self.obs_mean.numel(), (x.shape, self.obs_mean.shape)
         if terminal_obs is not None:
+            _require_dtype(terminal_obs, "terminal_obs", (x.dtype,))
+            _require_dtype(done, "done", (torch.uint8,))
             assert done is not None and terminal_obs.shape == x.shape and terminal_obs.is_contiguous()
             E = x.shape[1]
             with torch.cuda.device(x.device):
-                _lib.check(_lib.lib().madrl_standardize_obs_terminal_f32(
+                _lib.check(_obs_fn("standardize_obs_terminal", x.dtype)(
                     x.shape[0], E, self.obs_mean.numel() // E, _ptr(x), _ptr(terminal_obs), _ptr(done.contiguous()),
                     _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha, self.eps, _stream(x.device)))
             return obs
         with torch.cuda.device(x.device):
-            _lib.check(_lib.lib().madrl_standardize_f32(x.shape[0], self.obs_mean.numel(), _ptr(x),
-                                                        _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha,
-                                                        self.eps, 1, 1.0, 1, _stream(x.device)))
+            _lib.check(_obs_fn("standardize", x.dtype)(x.shape[0], self.obs_mean.numel(), _ptr(x),
+                                                       _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha,
+                                                       self.eps, 1, 1.0, 1, _stream(x.device)))
         return obs
 
     def rew(self, rew):
         """In place on rew [T,E,A]: optional running-std division, then scale_reward."""
-        assert rew.is_contiguous()
+        _require_dtype(rew, "rew")
+        assert rew.is_contiguous() and rew[0].numel() == self.rew_mean.numel(), rew.shape
         with torch.cuda.device(rew.device):
             _lib.check(_lib.lib().madrl_standardize_f32(rew.shape[0], self.rew_mean.numel(), _ptr(rew),
                                                         _ptr(self.rew_mean), _ptr(self.rew_var), self.rew_alpha,
@@ -172,6 +205,8 @@ class EpisodeStats(object):
     def rollout(self, rew, done):
         """rew [T,E,A] float32, done [T,E] uint8 -> dict(end [T,E] bool, episode_reward [T,E,A],
         episode_avg_reward [T,E], episode_disc_return [T,E], episode_length [T,E])."""
+        _require_dtype(rew, "rew")
+        _require_dtype(done, "done", (torch.uint8,))
         rew, done = rew.contiguous(), done.contiguous()
         T, E, A = rew.shape
         dev = rew.device
@@ -251,7 +286,12 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
     step, the reset observation on a done step) and the packed ``observations`` are shifted so that row t
     is the observation action t was taken in -- what rllab stores (ma_sampler.py:71-77).  Without it,
     ``obs`` is used as is (the host ``to_paths`` contract).  Two kernels of csrc/postproc.cu: a plan pass
-    over ``done`` and one HBM-bound row permutation per tensor; no host loop."""
+    over ``done`` and one HBM-bound row permutation per tensor; no host loop.  Tensors of 4-byte elements,
+    and bfloat16 observations (2-byte rows, ``madrl_paths_pack_u16``)."""
+    for name, x in [("obs", obs), ("actions", actions), ("rew", rew)] + sorted((infos or {}).items()):
+        if x.element_size() not in (2, 4) or (x.element_size() == 2 and x.dtype != torch.bfloat16):
+            raise TypeError("pack_paths packs 4-byte elements and bfloat16; %s is %s" % (name, x.dtype))
+    _require_dtype(done, "done", (torch.uint8,))
     L = _lib.lib()
     T, E, A = rew.shape
     dev = rew.device
@@ -266,7 +306,7 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
 
         def pack(x, per_agent, first=None):
             x = x.contiguous()
-            assert x.element_size() == 4 and x.shape[0] == T and x.shape[1] == E, (x.dtype, x.shape)
+            assert x.shape[0] == T and x.shape[1] == E, (x.dtype, x.shape)
             assert not per_agent or x.shape[2] == A, x.shape
             n_agents = A if per_agent else 1
             tail = tuple(x.shape[3:] if per_agent else x.shape[2:])
@@ -276,8 +316,8 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
                 first = first.to(x.dtype).contiguous()
                 assert first.shape == x.shape[1:], (first.shape, x.shape)
             # per-env tensors (n_agents = 1): the row offset e*T + s + (t - s) = e*T + t for any (s, L)
-            _lib.check(L.madrl_paths_pack_u32(T, E, n_agents, D, _ptr(x), _ptr(first), _ptr(seg_s), _ptr(seg_l),
-                                              _ptr(out), st))
+            fn = L.madrl_paths_pack_u16 if x.element_size() == 2 else L.madrl_paths_pack_u32
+            _lib.check(fn(T, E, n_agents, D, _ptr(x), _ptr(first), _ptr(seg_s), _ptr(seg_l), _ptr(out), st))
             return out
 
         packed_obs = pack(obs, True, obs_before)

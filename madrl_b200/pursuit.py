@@ -64,6 +64,9 @@ class BatchedPursuitEvade(BatchedEngine):
     Keyword names follow pursuit_evade.py:49-148.  Evader motion uses the env's counter-based
     stream (the reference's default controller is an unseeded RandomState shared by every
     instance, utils/Controllers.py:11, so there is no reference stream to reproduce).
+    ``obs_dtype`` torch.float32 (None) or torch.bfloat16: observations stored as bfloat16, bit-identical to
+    the float32 ones rounded to nearest even.  The in-kernel heuristic policy only tests which cells
+    hold an evader, which rounding never changes, so chained bfloat16 launches equal one long launch.
     """
 
     _abi, _Layout, _act_tail, _info_tail, _info_keys = "pursuit", _lib.PELayout, (), (), ("removed",)
@@ -72,7 +75,7 @@ class BatchedPursuitEvade(BatchedEngine):
                  layer_norm=10, n_catch=2, catchr=0.01, term_pursuit=5.0, urgency_reward=0.0,
                  include_id=True, surround=True, constraint_window=1.0, sample_maps=False,
                  reward_mech='global', random_opponents=False, max_opponents=10, device=None, seed=0,
-                 env_id_base=0, max_path_length=0):
+                 env_id_base=0, max_path_length=0, obs_dtype=None):
         mp = map_pool_array(map_pool)
         cfg = pe_config(n_envs, mp, n_evaders=n_evaders, n_pursuers=n_pursuers, obs_range=obs_range,
                         flatten=flatten, layer_norm=layer_norm, n_catch=n_catch, catchr=catchr,
@@ -84,7 +87,7 @@ class BatchedPursuitEvade(BatchedEngine):
         self.n_envs, self.n_pursuers, self.n_evaders = n_envs, n_pursuers, n_evaders
         self.obs_range, self.reward_mech, self.flatten = obs_range, reward_mech, bool(flatten)
         super().__init__(cfg, n_pursuers, device, torch.float32, torch.int32,
-                         create_args=(C.c_void_p(mp.ctypes.data),))
+                         create_args=(C.c_void_p(mp.ctypes.data),), obs_dtype=obs_dtype)
         self.n_agents = int(self.layout.n_agents)   # pursuers + evaders (the state records), not the acting agents
 
     @property

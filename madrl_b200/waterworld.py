@@ -65,7 +65,11 @@ class BatchedMAWaterWorld(BatchedEngine):
     Parameters mirror waterworld.py:77-81 plus the batch/engine arguments:
     ``n_envs``; ``device``; ``seed`` and ``env_id_base`` (RNG key = (seed, env_id_base + e), so a
     sharded batch reproduces the unsharded one); ``max_path_length`` (VecEnvExecutor horizon);
-    ``dtype`` torch.float32 (production) or torch.float64 (verification build).
+    ``dtype`` torch.float32 (production) or torch.float64 (verification build); ``obs_dtype``
+    ``dtype`` (None) or torch.bfloat16 with float32 ``dtype``: observations stored as bfloat16,
+    bit-identical to the float32 ones rounded to nearest even (madrl_ww_set_obs_format).  The
+    in-kernel heuristic policy widens a bfloat16 ``obs0``, so its first decision after a launch
+    boundary sees rounded features: chained launches equal one long launch in float32 only.
     """
 
     timestep_limit = 1000
@@ -76,7 +80,7 @@ class BatchedMAWaterWorld(BatchedEngine):
                  poison_speed=0.01, n_sensors=30, sensor_range=0.2, action_scale=0.01,
                  poison_reward=-1., food_reward=1., encounter_reward=.05, control_penalty=-.5,
                  reward_mech='local', addid=True, speed_features=True, device=None, seed=0,
-                 env_id_base=0, max_path_length=0, dtype=torch.float32):
+                 env_id_base=0, max_path_length=0, dtype=torch.float32, obs_dtype=None):
         assert dtype in (torch.float32, torch.float64)
         cfg = ww_config(n_envs, n_pursuers, n_evaders, n_coop=n_coop, n_poison=n_poison, radius=radius,
                         obstacle_radius=obstacle_radius, obstacle_loc=obstacle_loc, ev_speed=ev_speed,
@@ -88,7 +92,7 @@ class BatchedMAWaterWorld(BatchedEngine):
         self.n_envs, self.n_pursuers, self.n_evaders, self.n_poison = n_envs, n_pursuers, n_evaders, n_poison
         self.n_sensors = n_sensors
         self.reward_mech = reward_mech
-        super().__init__(cfg, n_pursuers, device, dtype, dtype)
+        super().__init__(cfg, n_pursuers, device, dtype, dtype, obs_dtype=obs_dtype)
         self.n_obj = int(self.layout.n_obj)
 
     @property
