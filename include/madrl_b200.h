@@ -436,6 +436,32 @@ int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const 
 int madrl_paths_pack_u16(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
                          const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream);
 
+/* rllab's LinearFeatureBaseline (rllab/rllab/baselines/linear_feature_baseline.py), decentralized mode: one
+ * baseline over every (t, e, a) row of a rollout.  Row (t, e, a) uses the observation the action of step t was
+ * taken in (obs_before != NULL: obs_before [E][A][D] for t = 0, obs[t-1] afterwards; NULL: obs[t]) and the time
+ * index i = t - seg_start[t][e] (seg_start from madrl_paths_plan), plus t0[e] when seg_start[t][e] == 0
+ * (t0 int32 [E] or NULL).  Features, Df = 2D + 4: [clip(o,-10,10), clip(o,-10,10)^2, i/100, (i/100)^2,
+ * (i/100)^3, 1], in float64 (observations widened exactly, bfloat16 ones first to float32).
+ *   madrl_lfb_normal_eq_*  ret float32 [T][E][A] -> G float64 [Df+1][Df+1] = [F y]^T [F y]: F^T F, with F^T y as
+ *                          row / column Df and y^T y at [Df][Df]; exactly symmetric, deterministic (fixed row
+ *                          partition and combination order).  ws: madrl_lfb_workspace_size bytes of device scratch,
+ *                          which depends on D only:  48 * P * 32768 bytes, P = nb (nb + 1) / 2, nb = ceil((2D+5)/64).
+ *   madrl_lfb_predict_*    coef float64 [Df] -> values float32 [T][E][A] = features . coef, evaluated in float64.
+ * MADRL_EINVAL for D outside [1, 8192], T*E*A >= 2^31 or a NULL required buffer. */
+int madrl_lfb_workspace_size(int D, size_t* bytes);
+int madrl_lfb_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+                            const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev,
+                            double* ws_dev, void* stream);
+int madrl_lfb_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+                             const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev,
+                             double* ws_dev, void* stream);
+int madrl_lfb_predict_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+                          const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
+                          float* values_dev, void* stream);
+int madrl_lfb_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+                           const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
+                           float* values_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -159,6 +159,11 @@ def _declare(lib):
         lib.madrl_standardize_bf16.argtypes = lib.madrl_standardize_f32.argtypes
         lib.madrl_standardize_obs_terminal_bf16.argtypes = lib.madrl_standardize_obs_terminal_f32.argtypes
         lib.madrl_paths_pack_u16.argtypes = lib.madrl_paths_pack_u32.argtypes
+    if hasattr(lib, "madrl_lfb_normal_eq_f32"):  # linear feature baseline (absent from older builds)
+        lib.madrl_lfb_workspace_size.argtypes = [i32, C.POINTER(C.c_size_t)]
+        for dt in ("f32", "bf16"):
+            getattr(lib, "madrl_lfb_normal_eq_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
+            getattr(lib, "madrl_lfb_predict_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
 
 
 def lib():

@@ -277,4 +277,44 @@ __device__ __forceinline__ real clip01(real x) {
   return x < (real)0 ? (real)0 : (x > (real)1 ? (real)1 : x);
 }
 
+// FP64 tensor-core MMA (baseline.cu's Gram kernel) and the float64 shared-memory tile accesses around it.
+// mma.m16n8k16.f64: C[16x8] += A[16x16] B[16x8]; lane = 4 g + q (g = lane >> 2, q = lane & 3) holds
+//   a[i] = A[g + 8 (i & 1)][q + 4 (i >> 1)],  b[i] = B[q + 4 i][g],  c[i] = C[g + 8 (i >> 1)][2 q + (i & 1)].
+#ifndef MADRL_EMU_PTX_HELPERS
+__device__ __forceinline__ double lds_f64(const double* p) { return *p; }
+__device__ __forceinline__ void sts_f64(double* p, double v) { *p = v; }
+__device__ __forceinline__ void mma_f64_16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f64.f64.f64.f64 {%0, %1, %2, %3}, "
+               "{%4, %5, %6, %7, %8, %9, %10, %11}, {%12, %13, %14, %15}, {%0, %1, %2, %3};"
+               : "+d"(c[0]), "+d"(c[1]), "+d"(c[2]), "+d"(c[3])
+               : "d"(a[0]), "d"(a[1]), "d"(a[2]), "d"(a[3]), "d"(a[4]), "d"(a[5]), "d"(a[6]), "d"(a[7]),
+                 "d"(b[0]), "d"(b[1]), "d"(b[2]), "d"(b[3]));
+}
+#else   // MADRL_EMU_PTX_HELPERS
+// Host versions: the tile accesses are recorded by the race checker; the MMA gathers every lane's fragment
+// registers through the emulator's warp exchange (one rendezvous per register, as the hardware's operand
+// collection is warp-wide) and forms each of this lane's four outputs as c + sum_k A[m][k] B[k][n], k ascending.
+static inline double lds_f64(const double* p) { smem_access(smem_addr(p), 8, SMEM_READ); return *p; }
+static inline void sts_f64(double* p, double v) { smem_access(smem_addr(p), 8, SMEM_WRITE); *p = v; }
+static inline void mma_f64_16816(double (&c)[4], const double (&a)[8], const double (&b)[4]) {
+  double A[8][32], B[4][32];
+  for (int r = 0; r < 8; ++r) {
+    const uint64_t* s = madrl_emu::warp_exchange(madrl_emu::to_bits(a[r]));
+    for (int l = 0; l < 32; ++l) A[r][l] = madrl_emu::from_bits<double>(s[l]);
+  }
+  for (int r = 0; r < 4; ++r) {
+    const uint64_t* s = madrl_emu::warp_exchange(madrl_emu::to_bits(b[r]));
+    for (int l = 0; l < 32; ++l) B[r][l] = madrl_emu::from_bits<double>(s[l]);
+  }
+  const int lane = threadIdx.x & 31, g = lane >> 2, q = lane & 3;
+  for (int i = 0; i < 4; ++i) {
+    const int m = g + 8 * (i >> 1), n = 2 * q + (i & 1);
+    double acc = c[i];
+    for (int k = 0; k < 16; ++k)   // A[m][k]: lane 4 (m & 7) + (k & 3), register (m >> 3) + 2 (k >> 2);  B[k][n]: lane 4 n + (k & 3), register k >> 2
+      acc += A[(m >> 3) + 2 * (k >> 2)][4 * (m & 7) + (k & 3)] * B[k >> 2][4 * n + (k & 3)];
+    c[i] = acc;
+  }
+}
+#endif  // MADRL_EMU_PTX_HELPERS
+
 }  // namespace madrl

@@ -7,6 +7,8 @@ right after ``env.step`` in its sampler loop, as streaming passes over ``[T, E, 
 * ``center_advantages`` / ``explained_variance``  the whole-batch statistics of
                      ``process_samples`` (base.py:69-86; rllab/rllab/algos/util.py:7-12,
                      rllab/rllab/misc/special.py:51-59)
+* ``LinearFeatureBaseline``  rllab's default baseline (rllab/rllab/baselines/linear_feature_baseline.py):
+                     ``predict`` before ``gae``, ``fit`` after it (base.py:52-55, :163-168)
 * ``to_paths``       the per-agent ``paths`` dicts of ``dec_rollout``
                      (rllab/rllab/sampler/ma_sampler.py:52-100), built on the host from gathered
                      tensors for callers that still want rllab's list-of-paths format.
@@ -220,6 +222,144 @@ class EpisodeStats(object):
                                                           _ptr(ep_d), _ptr(ep_l), _ptr(ep_e), _stream(dev)))
         return dict(end=ep_e.bool(), episode_reward=ep_r, episode_avg_reward=ep_r.mean(dim=-1),
                     episode_disc_return=ep_d, episode_length=ep_l)
+
+
+def _require_shape(t, name, shape):
+    if tuple(t.shape) != tuple(shape):
+        raise ValueError("%s must have shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
+
+
+class LinearFeatureBaseline(object):
+    """rllab's ``LinearFeatureBaseline`` (rllab/rllab/baselines/linear_feature_baseline.py) over the rows of a
+    rollout, pooled over envs and agents (the decentralized mode: one baseline for every agent's paths).
+
+    Row (t, e, a) is the observation action t was taken in -- with ``obs_before`` [E,A,D] (what
+    ``engine.rollout(auto_reset=True)`` returns plus the observations before the launch) row t uses
+    ``obs[t-1]`` (``obs_before`` for t = 0), as ``pack_paths`` does; without it ``obs[t]`` as given.  Its time
+    index is its 0-based position in its path (paths cut at ``done``), plus ``t0[e]`` (int32 [E]) on env e's
+    first path: pass the engine's ``state['path_len']`` read before the launch so that a path begun in an
+    earlier launch continues its index.  Features ``[clip(o,±10), clip(o,±10)², i/100, (i/100)², (i/100)³, 1]``
+    (Df = 2D + 4) are built on the device from the observation rows, never stored: ``fit`` forms the float64
+    normal equations ``[F y]ᵀ[F y]`` on the FP64 tensor cores (``madrl_lfb_normal_eq_*``), optionally
+    all-reduces them over a ``torch.distributed`` group, and solves ``(FᵀF + reg·I) c = Fᵀy`` by Cholesky on
+    the device; only if that fails does it fall back to rllab's host ``lstsq`` with its retry loop.
+    Observations: float32 or bfloat16 (widened exactly: a bfloat16 call equals the call on ``obs.float()``).
+    Centralized control is the view ``obs.view(T, E, 1, A * D)``."""
+
+    def __init__(self, obs_dim, device, reg_coeff=1e-5):
+        device = torch.device(device)
+        if device.type == "cuda" and device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
+        self.obs_dim, self.device, self.reg_coeff = int(obs_dim), device, reg_coeff
+        self.n_features = 2 * self.obs_dim + 4
+        self._coeffs = None
+
+    def get_param_values(self):
+        """float64 coefficients [Df] (NumPy), or None before the first fit."""
+        return None if self._coeffs is None else self._coeffs.cpu().numpy()
+
+    def set_param_values(self, val):
+        if val is None:
+            self._coeffs = None
+            return
+        c = torch.as_tensor(np.asarray(val, dtype=np.float64) if not torch.is_tensor(val) else val)
+        _require_dtype(c, "coefficients", (torch.float64,))
+        _require_shape(c, "coefficients", (self.n_features,))
+        self._coeffs = c.to(self.device).contiguous().clone()
+
+    def _rows(self, obs, done, obs_before, t0, returns=None):
+        """Validates the rollout tensors (before any pointer reaches a kernel) and runs the path plan."""
+        for t, n in ((obs, "obs"), (done, "done"), (obs_before, "obs_before"), (t0, "t0"), (returns, "returns")):
+            if t is not None and not torch.is_tensor(t):
+                raise TypeError("%s must be a torch.Tensor, got %r" % (n, type(t)))
+        _require_dtype(obs, "obs", _OBS_DTYPES)
+        _require_dtype(obs_before, "obs_before", (obs.dtype,))
+        _require_dtype(done, "done", (torch.uint8,))
+        _require_dtype(t0, "t0", (torch.int32,))
+        _require_dtype(returns, "returns")
+        if obs.dim() != 4:
+            raise ValueError("obs must be [T, E, A, D], got shape %s" % (tuple(obs.shape),))
+        T, E, A, D = obs.shape
+        if D != self.obs_dim:
+            raise ValueError("obs has %d features per row, the baseline was built for %d" % (D, self.obs_dim))
+        _require_shape(done, "done", (T, E))
+        if obs_before is not None:
+            _require_shape(obs_before, "obs_before", (E, A, D))
+        if t0 is not None:
+            _require_shape(t0, "t0", (E,))
+        if returns is not None:
+            _require_shape(returns, "returns", (T, E, A))
+        for t, n in ((obs, "obs"), (done, "done"), (obs_before, "obs_before"), (t0, "t0"), (returns, "returns")):
+            if t is not None and t.device != self.device:
+                raise ValueError("%s must live on %s, got %s" % (n, self.device, t.device))
+        if T * E * A >= 2 ** 31:
+            raise ValueError("T*E*A must be < 2^31, got %d" % (T * E * A))
+        L = _lib.lib()
+        done = done.contiguous()
+        seg_s = torch.empty((T, E), dtype=torch.int32, device=self.device)
+        seg_l = torch.empty((T, E), dtype=torch.int32, device=self.device)
+        n_ep = torch.empty((E,), dtype=torch.int32, device=self.device)
+        ep_rec = torch.empty((E, T, 3), dtype=torch.int32, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(L.madrl_paths_plan(T, E, A, _ptr(done), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep), _ptr(ep_rec),
+                                          _stream(self.device)))
+        cont = lambda x: None if x is None else x.contiguous()          # noqa: E731
+        return (T, E, A, D), cont(obs), cont(obs_before), cont(t0), seg_s
+
+    def normal_equations(self, obs, done, returns, obs_before=None, t0=None):
+        """G = [F y]ᵀ[F y], float64 [Df+1, Df+1] on the device: FᵀF, with Fᵀy as row and column Df."""
+        (T, E, A, D), obs, obs_before, t0, seg_s = self._rows(obs, done, obs_before, t0, returns)
+        returns = returns.contiguous()
+        L = _lib.lib()
+        nbytes = C.c_size_t()
+        _lib.check(L.madrl_lfb_workspace_size(D, C.byref(nbytes)))
+        ws = torch.empty(nbytes.value // 8, dtype=torch.float64, device=self.device)
+        G = torch.empty((self.n_features + 1, self.n_features + 1), dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(_obs_fn("lfb_normal_eq", obs.dtype)(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s),
+                                                           _ptr(t0), _ptr(returns), _ptr(G), _ptr(ws),
+                                                           _stream(self.device)))
+        return G
+
+    def solve(self, G):
+        """Coefficients from normal equations G (as `normal_equations` returns them), rllab's regularisation."""
+        Df = self.n_features
+        M, b = G[:Df, :Df], G[:Df, Df]
+        Lc, info = torch.linalg.cholesky_ex(M + self.reg_coeff * torch.eye(Df, dtype=G.dtype, device=G.device))
+        if int(info) == 0:
+            c = torch.cholesky_solve(b.unsqueeze(1), Lc).squeeze(1)
+            if bool(torch.isfinite(c).all()):
+                return c
+        # the factorisation failed: rllab's loop (linear_feature_baseline.py:29-37) on the host
+        Mn, bn, reg = M.cpu().numpy(), b.cpu().numpy(), self.reg_coeff
+        for _ in range(5):
+            c = np.linalg.lstsq(Mn + reg * np.identity(Df), bn, rcond=None)[0]
+            if np.all(np.isfinite(c)):
+                break
+            reg *= 10
+        return torch.from_numpy(c).to(G.device)
+
+    def fit(self, obs, done, returns, obs_before=None, t0=None, group=None):
+        """Fit to ``returns`` [T,E,A] float32 (``gae``'s second output).  With a ``torch.distributed`` group the
+        normal equations are summed over its ranks before the solve (every rank gets the pooled coefficients;
+        no observation moves)."""
+        G = self.normal_equations(obs, done, returns, obs_before, t0)
+        if group is not None:
+            import torch.distributed as dist
+            dist.all_reduce(G, op=dist.ReduceOp.SUM, group=group)
+        self._coeffs = self.solve(G)
+
+    def predict(self, obs, done, obs_before=None, t0=None):
+        """values [T,E,A] float32 = features(row) . coefficients, evaluated in float64; zeros before the first fit."""
+        (T, E, A, D), obs, obs_before, t0, seg_s = self._rows(obs, done, obs_before, t0)
+        values = torch.empty((T, E, A), dtype=torch.float32, device=self.device)
+        if self._coeffs is None:
+            return values.zero_()
+        with torch.cuda.device(self.device):
+            _lib.check(_obs_fn("lfb_predict", obs.dtype)(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s),
+                                                         _ptr(t0), _ptr(self._coeffs), _ptr(values),
+                                                         _stream(self.device)))
+        return values
 
 
 def to_paths(obs, actions, rew, done, infos=None):
