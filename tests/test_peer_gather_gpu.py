@@ -18,8 +18,12 @@ def _worker(rank, world, port, q):
     dev = torch.device("cuda", rank)
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
     try:
-        E, T, Np = 96, 45, 5       # T not a multiple of the 6- and 32-step staging runs
+        # one block per SM and E > 2 SMs: the fused-exchange kernel's warps step several envs each
+        sms = torch.cuda.get_device_properties(dev).multi_processor_count
+        E, T, Np = 2 * sms + 7, 45, 5       # T not a multiple of the 6- and 32-step staging runs
+        assert E > 2 * sms
         eng = BatchedMAWaterWorld(E, Np, 5, device=dev, seed=9, env_id_base=rank * E, n_coop=1, radius=0.04)
+        eng.set_launch(blocks_per_sm=1)
         eng.reset()
         ok = True
         for mode in ("root", "all"):
