@@ -127,10 +127,15 @@ int madrl_ww_destroy(madrl_ww* h);
 void* madrl_ww_state_ptr(madrl_ww* h);
 /* seed(): new key, draw counters reset to 0 (waterworld.py:135-137 creates a fresh generator). */
 int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream);
-/* Launch geometry override (0 = library default): resident blocks per SM.  Blocks are one warp (= one
- * env); `warps_per_block` is range-checked ([0,4]) for ABI stability and otherwise ignored.  The same
- * holds for madrl_pursuit_set_launch and madrl_hostage_set_launch. */
+/* Launch geometry override (0 = library default, see below): resident blocks per SM.  Blocks are one warp
+ * (= one env); `warps_per_block` is range-checked ([0,4]) for ABI stability and otherwise ignored.  The same
+ * holds for madrl_pursuit_set_launch and madrl_hostage_set_launch, whose default is as many as fit. */
 int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm);
+/* The library default's cap on resident blocks per SM for an open-loop rollout of T steps of this handle
+ * (madrl_ww_rollout / _step / _rollout_host*): 16 for some float32-observation batches (DESIGN §4.3), else 0
+ * = as many as fit.  Resets, heuristic-policy and peer-exchange rollouts always use as many as fit.
+ * Negative on error. */
+int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
  * terminal one.  After this call every `*_rollout` (device pointers) with auto_reset first copies the rows

@@ -118,6 +118,8 @@ def _declare_engines(lib):
         # absent from libraries built before the bfloat16 observation format (timed side by side by scripts/)
         if hasattr(lib, "madrl_%s_set_obs_format" % fam):
             f("set_obs_format").argtypes = [vp, i32]
+    if hasattr(lib, "madrl_ww_default_blocks_per_sm"):   # absent from older builds timed by scripts/
+        lib.madrl_ww_default_blocks_per_sm.argtypes = [vp, i32]
     lib.madrl_ww_set_peers.argtypes = [vp, i32, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
     lib.madrl_ww_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
     lib.madrl_pursuit_set_params.argtypes = [vp, C.c_double, C.c_double]

@@ -18,7 +18,7 @@ struct EngineCore {
   char* state = nullptr;     // state blob (state_layout's total_bytes)
   bool owns_state = false;   // cudaMalloc'ed by create (not the caller's)
   int device = 0, sms = 0;
-  int blocks_per_sm = 0;     // set_launch override of resident blocks per SM (0 = as many as fit)
+  int blocks_per_sm = 0;     // set_launch override of resident blocks per SM (0 = the family's default)
   HostPipe pipe;             // staging + streams of the host-buffer entry points (lazily created)
   void* term_obs = nullptr;  // set_terminal_obs (NULL = off)
   int obs_format = MADRL_OBS_NATIVE;   // set_obs_format: element type of every observation buffer
@@ -110,15 +110,18 @@ inline int engine_set_launch(EngineCore* h, int warps_per_block, int blocks_per_
 }
 
 // One launch of a warp-per-env kernel over E envs: one 32-thread block per env, or a single
-// persistent wave (SMs x resident blocks per SM, capped by set_launch) whose warps loop over the envs.
+// persistent wave (SMs x resident blocks per SM, capped by set_launch, else by the family's
+// `default_blocks_per_sm` when that is not 0) whose warps loop over the envs.
 template <class Kernel, class Params>
-int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStream_t stream, const Params& p) {
+int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStream_t stream, const Params& p,
+                  int default_blocks_per_sm = 0) {
   if (smem > 48 * 1024)
     MADRL_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int resident = 0;
   MADRL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kfn, 32, smem));
   if (resident < 1) resident = 1;
-  if (h->blocks_per_sm > 0 && h->blocks_per_sm < resident) resident = h->blocks_per_sm;
+  const int cap = h->blocks_per_sm > 0 ? h->blocks_per_sm : default_blocks_per_sm;
+  if (cap > 0 && cap < resident) resident = cap;
   int grid = E;
   if (grid > h->sms * resident) grid = h->sms * resident;
   MADRL_LAUNCH(kfn, grid, 32, smem, stream, p);

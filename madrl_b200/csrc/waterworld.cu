@@ -784,21 +784,49 @@ extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_
 template <typename real>
 static size_t ww_cand_bytes(int opl, int n_obj) { return opl >= 2 ? (size_t)n_obj * CandSlot<real>::kStride : 0; }
 
+// The library's default cap on resident one-warp blocks per SM for an open-loop rollout of T steps with
+// float32 observations (0 = as many as fit; set_launch overrides it).  See DESIGN §4.3 for the numbers
+// behind each condition, measured on C2 (5 pursuers, 4096 envs: 2.17 -> 2.02 ms per 256-step launch):
+//   * whole-step staging only: the C2 kernel computes about as fast with 16 warps per SM, each stepping two
+//     envs in turn, as with 31, but its observation stores overlap the sensing better.  The ring staging of
+//     larger env-steps (C4) and bfloat16 observations gain nothing or lose at 16;
+//   * T >= 16: a launch of a step or a few has no later steps for the stores to overlap with;
+//   * 16 x SMs warps split the envs into at least two rounds and the last is at least 4/5 full: a mostly
+//     empty last round (e.g. 3000 envs on 132 SMs: 2112 + 888) costs more than the overlap saves.
+static int ww_default_blocks_per_sm(const madrl_ww* h, int T) {
+  const madrl_ww_config& c = h->cfg;
+  if (c.fp64 || h->obs_format != MADRL_OBS_NATIVE || T < 16) return 0;
+  const int opl = (h->lay.n_obj + 31) / 32;
+  if (ww_cand_bytes<float>(opl, h->lay.n_obj) + obs_stage_bytes(c.n_pursuers * h->lay.obs_dim, sizeof(float)) >
+      kStepStageMaxBytes)
+    return 0;
+  const long g = 16L * h->sms, E = c.n_envs, rounds = (E + g - 1) / g;
+  return rounds >= 2 && 5 * (E - (rounds - 1) * g) >= 4 * g ? 16 : 0;
+}
+
+extern "C" int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(T >= 1, "T must be >= 1");
+  return ww_default_blocks_per_sm(h, T);
+}
+
 template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY>
-static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t stream) {
+static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, int cap, cudaStream_t stream) {
   const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(O))
                                                                         : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(O)));
-  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p);
+  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p, cap);
 }
 
 // The fused peer exchange is instantiated for native observations only (bf16 rollouts with peers are
 // rejected in ww_launch): it adds nothing to the observation path.
 template <typename real, typename O, int OPL, int KCH, int KC>
 static int ww_launch_inst(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t stream) {
-  if (p.policy_obs0 != nullptr) return ww_launch_inst2<real, O, OPL, KCH, KC, false, true>(h, p, stream);
+  if (p.policy_obs0 != nullptr) return ww_launch_inst2<real, O, OPL, KCH, KC, false, true>(h, p, 0, stream);
   if constexpr (sizeof(O) == sizeof(real))
-    if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, false>(h, p, stream);
-  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, stream);
+    if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, false>(h, p, 0, stream);
+  // only the plain open-loop rollout was measured with the default cap
+  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, p.mode == 0 ? ww_default_blocks_per_sm(h, p.T) : 0,
+                                                               stream);
 }
 
 template <typename real, typename O>

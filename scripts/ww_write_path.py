@@ -1,6 +1,6 @@
 """Waterworld observation write path against the card's streaming-write rate (one GPU command).
 
-    python scripts/ww_write_path.py [--lib NAME=PATH ...] [--rounds R]
+    python scripts/ww_write_path.py [--lib NAME=PATH ...] [--rounds R] [--blocks-per-sm N ...]
 
 Prints the card (name, power limit, SM clock), then times with CUDA events
   * `fill_` of a float32 tensor the size of one headline launch's observations ([256, 4096, 5, 213]):
@@ -10,7 +10,9 @@ Prints the card (name, power limit, SM clock), then times with CUDA events
 Every `--lib` build (default: the library MADRL_B200_LIB names, else the in-tree one; a PATH is loaded
 through MADRL_B200_LIB, e.g. one made by scripts/build_variant.py from another checkout) is timed in a
 child process of its own, the builds alternating for R rounds, and the median and min-max spread over
-the rounds are printed per build.
+the rounds are printed per build.  Each `--blocks-per-sm N` times every build once more with the
+persistent wave capped at N one-warp blocks per SM (engine.set_launch): at N = 16 each warp steps about
+two envs in turn, which shows how much of a warp's time the other resident warps can absorb.
 """
 import argparse
 import json
@@ -59,13 +61,14 @@ def fill_rate(reps):
     return {"bytes": nbytes, "ms": ms, "gbs": nbytes / (ms * 1e-3) / 1e9}
 
 
-def rollout_rate(name, reps):
+def rollout_rate(name, reps, bps):
     import torch
     sys.path.insert(0, ROOT)
     from madrl_b200 import BatchedMAWaterWorld
     s = SHAPES[name]
     E, T, Np = s["E"], s["T"], s["cfg"]["n_pursuers"]
     eng = BatchedMAWaterWorld(E, device="cuda", seed=0, **s["cfg"])
+    eng.set_launch(blocks_per_sm=bps)
     eng.reset()
     g = torch.Generator(device="cuda")
     g.manual_seed(1234)
@@ -78,8 +81,8 @@ def rollout_rate(name, reps):
             "agent_steps_per_sec": E * Np * T / (ms * 1e-3)}
 
 
-def child(reps):
-    print(json.dumps({n: rollout_rate(n, reps) for n in SHAPES}), flush=True)
+def child(reps, bps):
+    print(json.dumps({n: rollout_rate(n, reps, bps) for n in SHAPES}), flush=True)
 
 
 def main():
@@ -88,25 +91,31 @@ def main():
                     help="a build to time (PATH is loaded through MADRL_B200_LIB; 'NAME=' = the in-tree library)")
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--reps", type=int, default=10, help="timed launches per shape and round")
+    ap.add_argument("--blocks-per-sm", type=int, action="append", default=[], metavar="N",
+                    help="also time with at most N resident blocks per SM (0 = the library default)")
     ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
+    ap.add_argument("--bps", type=int, default=0, help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.child:
-        return child(a.reps)
+        return child(a.reps, a.bps)
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("ww_write_path.py needs a CUDA device")
     libs = [tuple(s.split("=", 1)) for s in a.lib] or [("default", os.environ.get("MADRL_B200_LIB", ""))]
+    # one timed build per (library, blocks per SM); bps 0 = the default launch, named by the library alone
+    libs = [(n if b == 0 else "%s@%d" % (n, b), path, b) for b in [0] + a.blocks_per_sm for n, path in libs]
     print("card:", json.dumps(card()))
     fill = fill_rate(20)
     print("fill_ float32 %.2f GB: %.3f ms, %.1f GB/s (streaming-write rate)" % (fill["bytes"] / 1e9, fill["ms"], fill["gbs"]))
-    res = {n: {s: [] for s in SHAPES} for n, _ in libs}
+    res = {n: {s: [] for s in SHAPES} for n, _, _ in libs}
     for r in range(a.rounds):
-        for n, path in libs:
+        for n, path, bps in libs:
             env = dict(os.environ)
             env.pop("MADRL_B200_LIB", None)
             if path:
                 env["MADRL_B200_LIB"] = os.path.abspath(path)
-            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--reps", str(a.reps)],
+            p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--reps", str(a.reps),
+                                "--bps", str(bps)],
                                env=env, cwd=ROOT, capture_output=True, text=True)
             if p.returncode:
                 sys.stderr.write(p.stdout + p.stderr)
@@ -114,16 +123,16 @@ def main():
             rec = json.loads(p.stdout.strip().splitlines()[-1])
             for s in SHAPES:
                 res[n][s].append(rec[s])
-                print("round %d %-8s %s: %.3f ms/launch, obs %.1f GB/s (%.1f%% of fill), %.3g agent-steps/s"
+                print("round %d %-11s %s: %.3f ms/launch, obs %.1f GB/s (%.1f%% of fill), %.3g agent-steps/s"
                       % (r, n, s, rec[s]["ms"], rec[s]["obs_gbs"], 100 * rec[s]["obs_gbs"] / fill["gbs"],
                          rec[s]["agent_steps_per_sec"]), flush=True)
     print("summary (median over %d rounds; spread = (max - min) / median of the launch time):" % a.rounds)
-    for n, _ in libs:
+    for n, _, _ in libs:
         for s in SHAPES:
             ms = sorted(x["ms"] for x in res[n][s])
             med = ms[len(ms) // 2]
             gbs = res[n][s][0]["obs_bytes"] / (med * 1e-3) / 1e9
-            print("  %-8s %s: %.3f ms (spread %.1f%%), obs %.1f GB/s = %.1f%% of the fill rate"
+            print("  %-11s %s: %.3f ms (spread %.1f%%), obs %.1f GB/s = %.1f%% of the fill rate"
                   % (n, s, med, 100 * (ms[-1] - ms[0]) / med, gbs, 100 * gbs / fill["gbs"]))
 
 
