@@ -420,6 +420,16 @@ int madrl_moments_f32(size_t n, const float* a_dev, const float* b_dev, double* 
  * stats_dev receives the moments of the INPUT as in madrl_moments_f32 (series 0). */
 int madrl_center_advantages_f32(size_t n, float* adv_dev, int center, int positive, double* stats_dev,
                                 double* workspace_dev, void* stream);
+/* Per-agent (column) versions for concurrent mode: a, b, adv are [rows][A] (A = the innermost axis, e.g. a
+ * [T][E][A] tensor with rows = T*E) and every statistic is taken over one column, i.e. one agent's samples:
+ * stats [A][MADRL_MOMENTS_STATS] (agent a's block laid out as above), workspace MADRL_MOMENTS_WS * A doubles.
+ * Centring / shifting applies agent a's statistics to column a.  Same arithmetic and combination order per
+ * column as the whole-batch passes, so A = 1 gives their bits.  MADRL_EINVAL for A outside
+ * [1, MADRL_AGENTS_MAX] (declared below), rows == 0 or a NULL required buffer. */
+int madrl_moments_agents_f32(size_t rows, int A, const float* a_dev, const float* b_dev, double* stats_dev,
+                             double* workspace_dev, void* stream);
+int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
+                                       double* stats_dev, double* workspace_dev, void* stream);
 
 /* Path packing: time-major rollout tensors -> rllab's per-(env, episode, agent) paths
  * (rllab/rllab/sampler/ma_sampler.py:52-100 `dec_rollout`, episodes cut at `done` as
@@ -466,6 +476,30 @@ int madrl_lfb_predict_f32(int T, int E, int A, int D, const float* obs_dev, cons
 int madrl_lfb_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
                            const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
                            float* values_dev, void* stream);
+
+/* Concurrent mode: one LinearFeatureBaseline per agent (rllab/sandbox/rocky/tf/samplers/batch_ma_sampler.py:64-188).
+ * Agent a's rows are (t, e, a) for every t, e; rows, features and time indices as above.
+ *   madrl_lfb_normal_eq_agents_*  G float64 [A][Df+1][Df+1]: agent a's [F y]^T [F y] over its own rows only, each
+ *                                 exactly symmetric and deterministic, all A from one launch.  Agent a's rows are
+ *                                 cut into S = ceil(48 / A) fixed slices.  ws: madrl_lfb_agents_workspace_size bytes,
+ *                                 A * S * P * 32768 (D = 213: 45.9 MB at A = 5, 55.1 MB at A = 20).  With A = 1 the
+ *                                 result equals madrl_lfb_normal_eq_* bit for bit.
+ *   madrl_lfb_predict_agents_*    coef float64 [A][Df]: row (t, e, a) is evaluated with coef[a].
+ * MADRL_EINVAL as above, and for A outside [1, MADRL_AGENTS_MAX]. */
+#define MADRL_AGENTS_MAX 1024
+int madrl_lfb_agents_workspace_size(int D, int A, size_t* bytes);
+int madrl_lfb_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+                                   const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
+                                   double* G_dev, double* ws_dev, void* stream);
+int madrl_lfb_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+                                    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
+                                    double* G_dev, double* ws_dev, void* stream);
+int madrl_lfb_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+                                 const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
+                                 float* values_dev, void* stream);
+int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+                                  const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
+                                  float* values_dev, void* stream);
 
 #ifdef __cplusplus
 }

@@ -166,6 +166,13 @@ def _declare(lib):
         for dt in ("f32", "bf16"):
             getattr(lib, "madrl_lfb_normal_eq_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
             getattr(lib, "madrl_lfb_predict_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
+    if hasattr(lib, "madrl_lfb_normal_eq_agents_f32"):  # per-agent baselines (absent from older builds)
+        lib.madrl_lfb_agents_workspace_size.argtypes = [i32, i32, C.POINTER(C.c_size_t)]
+        for dt in ("f32", "bf16"):
+            getattr(lib, "madrl_lfb_normal_eq_agents_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
+            getattr(lib, "madrl_lfb_predict_agents_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
+        lib.madrl_moments_agents_f32.argtypes = [C.c_size_t, i32, vp, vp, vp, vp, vp]
+        lib.madrl_center_advantages_agents_f32.argtypes = [C.c_size_t, i32, vp, i32, i32, vp, vp, vp]
 
 
 def lib():

@@ -12,6 +12,11 @@
 //                          column Df) on the FP64 tensor cores, features generated per chunk of rows in shared
 //                          memory: no [N][Df] matrix exists and the workspace does not depend on N.
 //   madrl_lfb_predict_*    values[r] = features(r) . c in float64, stored as float32 (predict, :39-43).
+//
+// Concurrent mode (one baseline per agent, rllab/sandbox/rocky/tf/samplers/batch_ma_sampler.py:64-188): the
+// *_agents entry points run the same kernels over A row groups, group a = the rows r = k A + a of agent a.  Each
+// group's normal equations read that agent's rows only, so all A systems come from one launch with the same rows,
+// tile pairs and MMAs as the pooled one; predict reads coefficient row a for agent a's rows.
 #include "common.cuh"
 
 namespace madrl {
@@ -21,6 +26,9 @@ namespace madrl {
 // N = columns of tile J, K = rows).  kLfbSlices fixed row slices, independent of the SM count; the CTAs of one
 // slice are adjacent in the grid, so they read the same rows while they sit in L2.  Partial tiles go to the
 // workspace and lfb_reduce_kernel sums them over the slices in ascending order: same inputs, same bits.
+// Per agent (kAgents): group g = rows k A + g, k in [0, T E), cut into lfb_agent_slices(A) slices; the grid is
+// (group, slice, pair) with the pair fastest, so the CTAs of one (group, slice) stay adjacent.  The pooled
+// launch is the one-group case with kLfbSlices slices.
 constexpr int kLfbTile = 64;
 constexpr int kLfbRows = 32;             // rows per shared-memory chunk: 2 MMA k-steps
 constexpr int kLfbLd = kLfbTile + 4;     // row pitch (doubles): a half-warp's fragment loads hit 16 distinct bank pairs
@@ -35,6 +43,7 @@ constexpr int kLfbFlush = 64;
 
 static inline int lfb_cols(int D) { return 2 * D + 5; }
 static inline int lfb_tiles(int D) { return (lfb_cols(D) + kLfbTile - 1) / kLfbTile; }
+__host__ __device__ __forceinline__ int lfb_agent_slices(int A) { return (kLfbSlices + A - 1) / A; }
 
 // Source row and time index of row r.
 template <typename O>
@@ -103,19 +112,25 @@ __device__ __forceinline__ double lfb_value(int kind, uint32_t v) {
   return kind == kLfbA1 ? a1 : (kind == kLfbA2 ? a2 : a3);
 }
 
-template <typename O>
+// kAgents = false: one group (every row), kLfbSlices slices.  kAgents = true: A groups of T E rows each (row
+// k A + g of group g), lfb_agent_slices(A) slices per group.  The loop runs over the group's row counter k.
+template <typename O, bool kAgents>
 __global__ void __launch_bounds__(kLfbThreads, 2)
 lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* __restrict__ obs_before,
                 const int32_t* __restrict__ seg_start, const int32_t* __restrict__ t0, const float* __restrict__ ret,
                 double* __restrict__ ws) {
   __shared__ __align__(16) double sF[2][kLfbRows][kLfbLd];   // features of tiles I and J (J only if J != I)
   const int nb = (2 * D + 5 + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
-  const int pair = blockIdx.x % P, slice = blockIdx.x / P;
+  const int pair = blockIdx.x % P, gs = blockIdx.x / P;      // gs = group * S + slice
+  const int S = kAgents ? lfb_agent_slices(A) : kLfbSlices;
+  const int group = kAgents ? gs / S : 0, slice = kAgents ? gs - group * S : gs;
   int I, J;
   lfb_pair(pair, nb, I, J);
-  const uint32_t N = (uint32_t)T * E * A;
-  const uint32_t r_begin = (uint32_t)((uint64_t)N * slice / kLfbSlices);
-  const uint32_t r_end = (uint32_t)((uint64_t)N * (slice + 1) / kLfbSlices);
+  const uint32_t N = kAgents ? (uint32_t)T * E : (uint32_t)T * E * A;   // rows of the group
+  const uint32_t r_begin = (uint32_t)((uint64_t)N * slice / S);
+  const uint32_t r_end = (uint32_t)((uint64_t)N * (slice + 1) / S);
+  // rollout row of the group's k-th row
+  auto row_of = [&](uint32_t k) -> uint32_t { return kAgents ? k * (uint32_t)A + (uint32_t)group : k; };
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5, g = lane >> 2, q = lane & 3;
   const int wm = (w & 1) * 32, wn = (w >> 1) * 32;
   const int j = tid & (kLfbTile - 1), k0 = tid >> 6;     // feature fill: column j, rows k0, k0 + 2, ...
@@ -141,7 +156,7 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
       for (int i = 0; i < 4; ++i) acc[mt][nt][i] = 0.0;
 
   // every thread owns its 32 elements of the tile: the first flush stores, later ones add (fixed order)
-  double* out = ws + ((size_t)slice * P + pair) * (kLfbTile * kLfbTile);
+  double* out = ws + ((size_t)gs * P + pair) * (kLfbTile * kLfbTile);
   bool first = true;
   int pending = 0;
   auto flush = [&]() {
@@ -168,16 +183,16 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
       if (obs_only[b]) {
 #pragma unroll
         for (int i = 0; i < kLfbRows / 2; ++i) {
-          const uint32_t r = r0 + k0 + 2 * i;
+          const uint32_t k = r0 + k0 + 2 * i, r = row_of(k);
           const O* src = obs_before ? (r < EA ? obs_before + (size_t)r * D : obs + (size_t)(r - EA) * D)
                                     : obs + (size_t)r * D;
-          nxt[b][i] = r < r_end ? __float_as_uint(obs_widen<float>(src[d[b]])) : 0u;
+          nxt[b][i] = k < r_end ? __float_as_uint(obs_widen<float>(src[d[b]])) : 0u;
         }
       } else {
 #pragma unroll
         for (int i = 0; i < kLfbRows / 2; ++i) {
-          const uint32_t r = r0 + k0 + 2 * i;
-          nxt[b][i] = lfb_fetch(kind[b], d[b], r, r < r_end, E, A, D, obs, obs_before, seg_start, t0, ret);
+          const uint32_t k = r0 + k0 + 2 * i;
+          nxt[b][i] = lfb_fetch(kind[b], d[b], row_of(k), k < r_end, E, A, D, obs, obs_before, seg_start, t0, ret);
         }
       }
     }
@@ -225,24 +240,28 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
 }
 
 // G[i][j] = G[j][i] = sum over the slices (ascending) of the partial tiles; the upper triangle of a diagonal tile
-// is mirrored, so G is exactly symmetric.  G: [Df+1][Df+1].
-__global__ void lfb_reduce_kernel(int D, const double* __restrict__ ws, double* __restrict__ G) {
+// is mirrored, so G is exactly symmetric.  One CTA per (group, tile pair), S slices per group;
+// G: [groups][Df+1][Df+1].
+__global__ void lfb_reduce_kernel(int D, int S, const double* __restrict__ ws, double* __restrict__ G) {
   const int Dc = 2 * D + 5, nb = (Dc + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
-  const int pair = blockIdx.x;
+  const int pair = blockIdx.x % P, group = blockIdx.x / P;
   int I, J;
   lfb_pair(pair, nb, I, J);
+  ws += (size_t)group * S * P * (kLfbTile * kLfbTile);
+  G += (size_t)group * Dc * Dc;
   for (int x = threadIdx.x; x < kLfbTile * kLfbTile; x += blockDim.x) {
     const int m = x / kLfbTile, n = x % kLfbTile, i = I * kLfbTile + m, j = J * kLfbTile + n;
     if (i >= Dc || j >= Dc || (I == J && m > n)) continue;
     double s = 0.0;
-    for (int sl = 0; sl < kLfbSlices; ++sl) s += ws[((size_t)sl * P + pair) * (kLfbTile * kLfbTile) + x];
+    for (int sl = 0; sl < S; ++sl) s += ws[((size_t)sl * P + pair) * (kLfbTile * kLfbTile) + x];
     G[(size_t)i * Dc + j] = s;
     G[(size_t)j * Dc + i] = s;
   }
 }
 
 // One warp per row: lanes stride over the D observation values (coalesced), float64 FMAs, butterfly sum.
-template <typename O>
+// kAgents: coef is [A][Df] and row (t, e, a) uses row a.
+template <typename O, bool kAgents>
 __global__ void lfb_predict_kernel(int T, int E, int A, int D, const O* __restrict__ obs,
                                    const O* __restrict__ obs_before, const int32_t* __restrict__ seg_start,
                                    const int32_t* __restrict__ t0, const double* __restrict__ coef,
@@ -250,6 +269,7 @@ __global__ void lfb_predict_kernel(int T, int E, int A, int D, const O* __restri
   const size_t r = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (r >= (size_t)T * E * A) return;                  // warp-uniform
+  if (kAgents) coef += (size_t)(r % (size_t)A) * (2 * D + 4);
   int idx;
   const O* src = lfb_row(r, E, A, D, obs, obs_before, seg_start, t0, idx);
   double acc = 0.0;
@@ -276,11 +296,24 @@ using namespace madrl;
 
 static const int kLfbMaxD = 8192;
 
+// Bytes of scratch for `groups` row groups of S slices each.
+static size_t lfb_ws_bytes(int D, int groups, int S) {
+  const size_t nb = (size_t)lfb_tiles(D);
+  return (size_t)groups * S * (nb * (nb + 1) / 2) * kLfbTile * kLfbTile * sizeof(double);
+}
+
 extern "C" int madrl_lfb_workspace_size(int D, size_t* bytes) {
   MADRL_REQUIRE(D >= 1 && D <= kLfbMaxD, "obs_dim must be in [1, %d], got %d", kLfbMaxD, D);
   MADRL_REQUIRE(bytes, "NULL pointer");
-  const size_t nb = (size_t)lfb_tiles(D);
-  *bytes = (size_t)kLfbSlices * (nb * (nb + 1) / 2) * kLfbTile * kLfbTile * sizeof(double);
+  *bytes = lfb_ws_bytes(D, 1, kLfbSlices);
+  return MADRL_OK;
+}
+
+extern "C" int madrl_lfb_agents_workspace_size(int D, int A, size_t* bytes) {
+  MADRL_REQUIRE(D >= 1 && D <= kLfbMaxD, "obs_dim must be in [1, %d], got %d", kLfbMaxD, D);
+  MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
+  MADRL_REQUIRE(bytes, "NULL pointer");
+  *bytes = lfb_ws_bytes(D, A, lfb_agent_slices(A));
   return MADRL_OK;
 }
 
@@ -291,18 +324,21 @@ static int lfb_check(int T, int E, int A, int D) {
   return MADRL_OK;
 }
 
-template <typename O>
+template <typename O, bool kAgents>
 static int lfb_normal_eq(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
                          const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev,
                          double* ws_dev, void* stream) {
   const int rc = lfb_check(T, E, A, D);
   if (rc) return rc;
+  if (kAgents)
+    MADRL_REQUIRE(A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
   MADRL_REQUIRE(obs_dev && seg_start_dev && ret_dev && G_dev && ws_dev, "NULL buffer");
   const int nb = lfb_tiles(D), P = nb * (nb + 1) / 2;
+  const int groups = kAgents ? A : 1, S = kAgents ? lfb_agent_slices(A) : kLfbSlices;
   cudaStream_t s = (cudaStream_t)stream;
-  MADRL_LAUNCH(lfb_gram_kernel<O>, (unsigned)(P * kLfbSlices), kLfbThreads, 0, s, T, E, A, D, (const O*)obs_dev,
-               (const O*)obs_before_dev, seg_start_dev, t0_dev, ret_dev, ws_dev);
-  MADRL_LAUNCH(lfb_reduce_kernel, (unsigned)P, 128, 0, s, D, ws_dev, G_dev);
+  MADRL_LAUNCH((lfb_gram_kernel<O, kAgents>), (unsigned)(P * S * groups), kLfbThreads, 0, s, T, E, A, D,
+               (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, ret_dev, ws_dev);
+  MADRL_LAUNCH(lfb_reduce_kernel, (unsigned)(P * groups), 128, 0, s, D, S, ws_dev, G_dev);
   g_launches.fetch_add(2);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -311,27 +347,45 @@ static int lfb_normal_eq(int T, int E, int A, int D, const void* obs_dev, const 
 extern "C" int madrl_lfb_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
                                        const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
                                        double* G_dev, double* ws_dev, void* stream) {
-  return lfb_normal_eq<float>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev, ws_dev,
-                              stream);
+  return lfb_normal_eq<float, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
+                                     ws_dev, stream);
 }
 
 extern "C" int madrl_lfb_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
                                         const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
                                         double* G_dev, double* ws_dev, void* stream) {
-  return lfb_normal_eq<uint16_t>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev, ws_dev,
-                                 stream);
+  return lfb_normal_eq<uint16_t, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
+                                        ws_dev, stream);
 }
 
-template <typename O>
+extern "C" int madrl_lfb_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev,
+                                              const float* obs_before_dev, const int32_t* seg_start_dev,
+                                              const int32_t* t0_dev, const float* ret_dev, double* G_dev,
+                                              double* ws_dev, void* stream) {
+  return lfb_normal_eq<float, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
+                                    ws_dev, stream);
+}
+
+extern "C" int madrl_lfb_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev,
+                                               const void* obs_before_dev, const int32_t* seg_start_dev,
+                                               const int32_t* t0_dev, const float* ret_dev, double* G_dev,
+                                               double* ws_dev, void* stream) {
+  return lfb_normal_eq<uint16_t, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
+                                       ws_dev, stream);
+}
+
+template <typename O, bool kAgents>
 static int lfb_predict(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
                        const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev,
                        void* stream) {
   const int rc = lfb_check(T, E, A, D);
   if (rc) return rc;
+  if (kAgents)
+    MADRL_REQUIRE(A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
   MADRL_REQUIRE(obs_dev && seg_start_dev && coef_dev && values_dev, "NULL buffer");
   const size_t rows = (size_t)T * E * A;
-  MADRL_LAUNCH(lfb_predict_kernel<O>, (unsigned)((rows * 32 + 255) / 256), 256, 0, (cudaStream_t)stream, T, E, A,
-               D, (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev);
+  MADRL_LAUNCH((lfb_predict_kernel<O, kAgents>), (unsigned)((rows * 32 + 255) / 256), 256, 0, (cudaStream_t)stream,
+               T, E, A, D, (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -340,12 +394,29 @@ static int lfb_predict(int T, int E, int A, int D, const void* obs_dev, const vo
 extern "C" int madrl_lfb_predict_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
                                      const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
                                      float* values_dev, void* stream) {
-  return lfb_predict<float>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev, stream);
+  return lfb_predict<float, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev,
+                                   stream);
 }
 
 extern "C" int madrl_lfb_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
                                       const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
                                       float* values_dev, void* stream) {
-  return lfb_predict<uint16_t>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev,
-                               stream);
+  return lfb_predict<uint16_t, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev,
+                                      values_dev, stream);
+}
+
+extern "C" int madrl_lfb_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev,
+                                            const float* obs_before_dev, const int32_t* seg_start_dev,
+                                            const int32_t* t0_dev, const double* coef_dev, float* values_dev,
+                                            void* stream) {
+  return lfb_predict<float, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev,
+                                  stream);
+}
+
+extern "C" int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev,
+                                             const void* obs_before_dev, const int32_t* seg_start_dev,
+                                             const int32_t* t0_dev, const double* coef_dev, float* values_dev,
+                                             void* stream) {
+  return lfb_predict<uint16_t, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev,
+                                     values_dev, stream);
 }

@@ -194,6 +194,8 @@ __global__ void episode_stats_kernel(int T, int E, int A, const float* __restric
 // order by one warp (no atomics), so a given input always yields the same bits.
 //
 // Three series are derived per element from (a, b):  s0 = a,  s1 = b,  s2 = b - a  (b optional).
+// The *_agents passes take the same statistics per column of a [rows][A] tensor (one agent's samples,
+// concurrent mode), one group of kMomBlocks CTAs per column.
 #ifndef MADRL_MOM_BLOCKS
 #define MADRL_MOM_BLOCKS 528           // 4 CTAs x 132 SMs (H100 SXM) (the CPU emulator of tests/emu builds with fewer)
 #endif
@@ -214,11 +216,23 @@ __device__ __forceinline__ double warp_min(double v) {
 }
 
 // pass 0 (means == nullptr): partial sums and minima; pass 1: partial sums of squared deviations.
-// part [kMomBlocks][2*kMomSeries].
-__global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, const float* __restrict__ a,
+// part [kMomBlocks][2*kMomSeries].  kAgents: a, b are [n][A] and CTA blockIdx.x covers column
+// blockIdx.x / kMomBlocks (an agent) as block blockIdx.x % kMomBlocks of a whole-batch pass over that column;
+// means and part then point at that column's [MADRL_MOMENTS_STATS] and [MADRL_MOMENTS_WS] blocks.
+template <bool kAgents>
+__global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, int A, const float* __restrict__ a,
                                                                       const float* __restrict__ b,
                                                                       const double* __restrict__ means,
                                                                       double* __restrict__ part) {
+  const int col = kAgents ? (int)(blockIdx.x / kMomBlocks) : 0;
+  const unsigned blk = kAgents ? blockIdx.x - col * kMomBlocks : blockIdx.x;
+  if (kAgents) {
+    a += col;
+    if (b) b += col;
+    if (means) means += (size_t)col * MADRL_MOMENTS_STATS;
+    part += (size_t)col * MADRL_MOMENTS_WS;
+  }
+  const size_t lda = kAgents ? (size_t)A : 1;
   double acc[kMomSeries] = {0.0, 0.0, 0.0};
   double mn[kMomSeries] = {INFINITY, INFINITY, INFINITY};
   double mu[kMomSeries] = {0.0, 0.0, 0.0};
@@ -226,10 +240,10 @@ __global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, 
 #pragma unroll
     for (int s = 0; s < kMomSeries; ++s) mu[s] = means[s];
   }
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const double va = (double)__ldcs(a + i);
-    const double vb = b ? (double)__ldcs(b + i) : 0.0;
+  const size_t stride = (size_t)kMomBlocks * blockDim.x;
+  for (size_t i = (size_t)blk * blockDim.x + threadIdx.x; i < n; i += stride) {
+    const double va = (double)__ldcs(a + i * lda);
+    const double vb = b ? (double)__ldcs(b + i * lda) : 0.0;
     const double v[kMomSeries] = {va, vb, vb - va};
 #pragma unroll
     for (int s = 0; s < kMomSeries; ++s) {
@@ -255,15 +269,18 @@ __global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, 
     double r = sh[0][threadIdx.x];
     for (int k = 1; k < kMomThreads / 32; ++k)
       r = (threadIdx.x & 1) ? fmin(r, sh[k][threadIdx.x]) : r + sh[k][threadIdx.x];
-    part[(size_t)blockIdx.x * 2 * kMomSeries + threadIdx.x] = r;
+    part[(size_t)blk * 2 * kMomSeries + threadIdx.x] = r;
   }
 }
 
 // One warp folds the block partials in a fixed order.  pass 0: stats[s] = mean_s, stats[6+s] = min_s;
 // pass 1: stats[3+s] = var_s (population).
+// One warp per column (agent): CTA c folds the partials at part + c * MADRL_MOMENTS_WS into stats + c * 9.
 __global__ void moments_finalize_kernel(size_t n, const double* __restrict__ part, int pass,
                                         double* __restrict__ stats) {
   const int lane = threadIdx.x;
+  part += (size_t)blockIdx.x * MADRL_MOMENTS_WS;
+  stats += (size_t)blockIdx.x * MADRL_MOMENTS_STATS;
 #pragma unroll
   for (int s = 0; s < kMomSeries; ++s) {
     double t = 0.0, m = INFINITY;
@@ -291,6 +308,29 @@ __global__ void center_apply_kernel(size_t n, float* __restrict__ x, const doubl
     double v = (double)x[i];
     if (center) v = (v - mean) / sd;
     if (positive) v = (v - cmin) + 1e-8;
+    __stcs(x + i, (float)v);
+  }
+}
+
+// The same per column of x [n][A], with column a's statistics (stats [A][MADRL_MOMENTS_STATS]); the per-agent
+// constants are formed once per CTA by the expressions above.
+__global__ void center_apply_agents_kernel(size_t n, int A, float* __restrict__ x, const double* __restrict__ stats,
+                                           int center, int positive) {
+  __shared__ double sc[MADRL_AGENTS_MAX][3];
+  for (int c = threadIdx.x; c < A; c += blockDim.x) {
+    const double* st = stats + (size_t)c * MADRL_MOMENTS_STATS;
+    const double mean = st[0], sd = sqrt(st[3]) + 1e-8, mn = st[6];
+    sc[c][0] = mean;
+    sc[c][1] = sd;
+    sc[c][2] = center ? (mn - mean) / sd : mn;
+  }
+  __syncthreads();
+  const size_t total = n * (size_t)A, stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) {
+    const int c = (int)(i % (size_t)A);
+    double v = (double)x[i];
+    if (center) v = (v - sc[c][0]) / sc[c][1];
+    if (positive) v = (v - sc[c][2]) + 1e-8;
     __stcs(x + i, (float)v);
   }
 }
@@ -451,11 +491,20 @@ extern "C" int madrl_standardize_bf16(int T, size_t n, void* x_dev, double* mean
   return standardize(T, n, (uint16_t*)x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable, stream);
 }
 
-static int run_moments(size_t n, const float* a, const float* b, double* stats, double* ws, cudaStream_t s) {
-  MADRL_LAUNCH(moments_partial_kernel, kMomBlocks, kMomThreads, 0, s, n, a, b, nullptr, ws);
-  MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 0, stats);
-  MADRL_LAUNCH(moments_partial_kernel, kMomBlocks, kMomThreads, 0, s, n, a, b, stats, ws);
-  MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 1, stats);
+// A == 0: the whole batch of n elements; A >= 1: the A columns of [n][A].
+static int run_moments(size_t n, int A, const float* a, const float* b, double* stats, double* ws, cudaStream_t s) {
+  if (A == 0) {
+    MADRL_LAUNCH(moments_partial_kernel<false>, kMomBlocks, kMomThreads, 0, s, n, 1, a, b, nullptr, ws);
+    MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 0, stats);
+    MADRL_LAUNCH(moments_partial_kernel<false>, kMomBlocks, kMomThreads, 0, s, n, 1, a, b, stats, ws);
+    MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 1, stats);
+  } else {
+    const unsigned grid = (unsigned)(kMomBlocks * A);
+    MADRL_LAUNCH(moments_partial_kernel<true>, grid, kMomThreads, 0, s, n, A, a, b, nullptr, ws);
+    MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 0, stats);
+    MADRL_LAUNCH(moments_partial_kernel<true>, grid, kMomThreads, 0, s, n, A, a, b, stats, ws);
+    MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 1, stats);
+  }
   g_launches.fetch_add(4);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -466,7 +515,7 @@ extern "C" int madrl_center_advantages_f32(size_t n, float* adv_dev, int center,
   MADRL_REQUIRE(n >= 1, "bad sizes");
   MADRL_REQUIRE(adv_dev && stats_dev && workspace_dev, "NULL buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  const int rc = run_moments(n, adv_dev, nullptr, stats_dev, workspace_dev, s);
+  const int rc = run_moments(n, 0, adv_dev, nullptr, stats_dev, workspace_dev, s);
   if (rc) return rc;
   if (center || positive) {
     MADRL_LAUNCH(center_apply_kernel, kMomBlocks, kMomThreads, 0, s, n, adv_dev, stats_dev, center, positive);
@@ -480,7 +529,32 @@ extern "C" int madrl_moments_f32(size_t n, const float* a_dev, const float* b_de
                                  double* workspace_dev, void* stream) {
   MADRL_REQUIRE(n >= 1, "bad sizes");
   MADRL_REQUIRE(a_dev && stats_dev && workspace_dev, "NULL buffer");
-  return run_moments(n, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
+  return run_moments(n, 0, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
+}
+
+extern "C" int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
+                                                  double* stats_dev, double* workspace_dev, void* stream) {
+  MADRL_REQUIRE(rows >= 1, "bad sizes");
+  MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
+  MADRL_REQUIRE(adv_dev && stats_dev && workspace_dev, "NULL buffer");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int rc = run_moments(rows, A, adv_dev, nullptr, stats_dev, workspace_dev, s);
+  if (rc) return rc;
+  if (center || positive) {
+    MADRL_LAUNCH(center_apply_agents_kernel, kMomBlocks, kMomThreads, 0, s, rows, A, adv_dev, stats_dev, center,
+                 positive);
+    g_launches.fetch_add(1);
+    MADRL_CUDA_CHECK(cudaGetLastError());
+  }
+  return MADRL_OK;
+}
+
+extern "C" int madrl_moments_agents_f32(size_t rows, int A, const float* a_dev, const float* b_dev,
+                                        double* stats_dev, double* workspace_dev, void* stream) {
+  MADRL_REQUIRE(rows >= 1, "bad sizes");
+  MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
+  MADRL_REQUIRE(a_dev && stats_dev && workspace_dev, "NULL buffer");
+  return run_moments(rows, A, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_paths_plan(int T, int E, int A, const uint8_t* done_dev, int32_t* seg_start_dev,

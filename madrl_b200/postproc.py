@@ -8,7 +8,10 @@ right after ``env.step`` in its sampler loop, as streaming passes over ``[T, E, 
                      ``process_samples`` (base.py:69-86; rllab/rllab/algos/util.py:7-12,
                      rllab/rllab/misc/special.py:51-59)
 * ``LinearFeatureBaseline``  rllab's default baseline (rllab/rllab/baselines/linear_feature_baseline.py):
-                     ``predict`` before ``gae``, ``fit`` after it (base.py:52-55, :163-168)
+                     ``predict`` before ``gae``, ``fit`` after it (base.py:52-55, :163-168); one per agent
+                     with ``n_agents`` (concurrent control)
+* ``process_samples_concurrent``  the concurrent branch of ``BatchMASampler.process_samples``
+                     (rllab/sandbox/rocky/tf/samplers/batch_ma_sampler.py:64-123, :184-188)
 * ``to_paths``       the per-agent ``paths`` dicts of ``dec_rollout``
                      (rllab/rllab/sampler/ma_sampler.py:52-100), built on the host from gathered
                      tensors for callers that still want rllab's list-of-paths format.
@@ -67,12 +70,38 @@ def _moments_buffers(dev):
             torch.empty(MOMENTS_WS, dtype=torch.float64, device=dev))
 
 
-def center_advantages(adv, center=True, positive=False, inplace=False):
+AGENTS_MAX = 1024                               # include/madrl_b200.h MADRL_AGENTS_MAX
+
+
+def _agent_columns(t, name):
+    """(rows, A) of a tensor whose last axis is the agent; raises before any library call."""
+    if t.dim() < 1 or t.shape[-1] < 1 or t.numel() == 0:
+        raise ValueError("%s must have a non-empty last (agent) axis, got shape %s" % (name, tuple(t.shape)))
+    A = int(t.shape[-1])
+    if A > AGENTS_MAX:
+        raise ValueError("%s has %d agents, at most %d are supported" % (name, A, AGENTS_MAX))
+    return t.numel() // A, A
+
+
+def center_advantages(adv, center=True, positive=False, inplace=False, per_agent=False):
     """``util.center_advantages`` / ``util.shift_advantages_to_positive`` over every sample of the
     batch (base.py:82-86 applies them to the concatenation of all paths): float64 mean / population
-    std / min computed on the device, deterministic.  Returns the processed tensor (same shape)."""
+    std / min computed on the device, deterministic.  Returns the processed tensor (same shape).
+    ``per_agent=True``: the last axis of ``adv`` (e.g. [T,E,A]) is the agent, and each agent's samples are
+    centred with their own statistics, as the concurrent sampler does per agent
+    (batch_ma_sampler.py:102-106)."""
     _require_dtype(adv, "adv")
+    if per_agent:
+        rows, A = _agent_columns(adv, "adv")
     out = adv.contiguous() if inplace else adv.contiguous().clone()
+    if per_agent:
+        stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=out.device)
+        ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=out.device)
+        with torch.cuda.device(out.device):
+            _lib.check(_lib.lib().madrl_center_advantages_agents_f32(rows, A, _ptr(out), int(bool(center)),
+                                                                     int(bool(positive)), _ptr(stats), _ptr(ws),
+                                                                     _stream(out.device)))
+        return out
     stats, ws = _moments_buffers(out.device)
     with torch.cuda.device(out.device):
         _lib.check(_lib.lib().madrl_center_advantages_f32(out.numel(), _ptr(out), int(bool(center)),
@@ -96,14 +125,38 @@ def moments(a, b=None):
     return stats
 
 
-def explained_variance(ypred, y):
-    """``special.explained_variance_1d`` (special.py:51-59) of baseline predictions against returns,
-    over every sample of the batch; one 72-byte device->host read."""
-    st = moments(ypred, y).cpu().numpy()
+def moments_agents(a, b=None):
+    """float64 [A, 9] cuda tensor: ``moments`` of each agent's samples, the agent being the last axis of
+    a (and b), e.g. [T,E,A]."""
+    _require_dtype(a, "a")
+    _require_dtype(b, "b")
+    rows, A = _agent_columns(a, "a")
+    if b is not None and tuple(b.shape) != tuple(a.shape):
+        raise ValueError("b must have shape %s, got %s" % (tuple(a.shape), tuple(b.shape)))
+    a = a.contiguous()
+    b = b.contiguous() if b is not None else None
+    stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=a.device)
+    ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=a.device)
+    with torch.cuda.device(a.device):
+        _lib.check(_lib.lib().madrl_moments_agents_f32(rows, A, _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
+                                                       _stream(a.device)))
+    return stats
+
+
+def _explained_variance_1d(st):
     var_pred, vary, var_res = float(st[3]), float(st[4]), float(st[5])
     if np.isclose(vary, 0):
         return 0 if var_pred > 0 else 1
     return 1 - var_res / (vary + 1e-8)
+
+
+def explained_variance(ypred, y, per_agent=False):
+    """``special.explained_variance_1d`` (special.py:51-59) of baseline predictions against returns,
+    over every sample of the batch; one 72-byte device->host read.  ``per_agent=True``: one value per
+    agent (the last axis), over that agent's samples -- a list of A floats."""
+    if per_agent:
+        return [_explained_variance_1d(st) for st in moments_agents(ypred, y).cpu().numpy()]
+    return _explained_variance_1d(moments(ypred, y).cpu().numpy())
 
 
 class FrameStack(object):
@@ -244,28 +297,70 @@ class LinearFeatureBaseline(object):
     all-reduces them over a ``torch.distributed`` group, and solves ``(FᵀF + reg·I) c = Fᵀy`` by Cholesky on
     the device; only if that fails does it fall back to rllab's host ``lstsq`` with its retry loop.
     Observations: float32 or bfloat16 (widened exactly: a bfloat16 call equals the call on ``obs.float()``).
-    Centralized control is the view ``obs.view(T, E, 1, A * D)``."""
+    Centralized control is the view ``obs.view(T, E, 1, A * D)``.
 
-    def __init__(self, obs_dim, device, reg_coeff=1e-5):
+    Concurrent control (``n_agents=A``): one baseline per agent, as rllab's concurrent sampler keeps
+    (batch_ma_sampler.py:64-188).  Agent a is fitted on its own rows (t, e, a) only; ``fit`` forms all A
+    systems in one launch (``madrl_lfb_normal_eq_agents_*``) and solves them with one batched Cholesky, and
+    ``predict`` evaluates agent a with coefficient row a.  The coefficients are [A, Df].
+
+    ``shared=True`` reproduces the reference runner instead, which lists ONE baseline object A times
+    (runners/rurllab.py:275-276): within one ``process_samples`` call agent a >= 1 is predicted with the
+    coefficients just fitted on agent a-1's paths, agent 0 with the previous call's fit on agent A-1's paths
+    (zeros before the first fit), and the object ends holding agent A-1's fit.  After ``fit`` the rows held
+    are therefore ``[previous fit's row A-1 (zeros before any fit), this fit's rows 0..A-2]``; ``carry``
+    is this fit's row A-1, the object's own coefficients, which the next fit gives agent 0.  Because a
+    rollout's returns do not depend on the values, ``process_samples_concurrent`` fits a shared baseline
+    before it predicts and still gives the reference's numbers."""
+
+    def __init__(self, obs_dim, device, reg_coeff=1e-5, n_agents=None, shared=False):
+        if shared and n_agents is None:
+            raise ValueError("shared=True models one baseline object listed once per agent: it needs n_agents")
+        if n_agents is not None and not (1 <= int(n_agents) <= AGENTS_MAX):
+            raise ValueError("n_agents must be in [1, %d], got %r" % (AGENTS_MAX, n_agents))
         device = torch.device(device)
         if device.type == "cuda" and device.index is None:
             device = torch.device("cuda", torch.cuda.current_device() if torch.cuda.is_available() else 0)
         self.obs_dim, self.device, self.reg_coeff = int(obs_dim), device, reg_coeff
+        self.n_agents = None if n_agents is None else int(n_agents)
+        self.shared = bool(shared)
         self.n_features = 2 * self.obs_dim + 4
         self._coeffs = None
+        self._carry = None
+
+    def _coef_shape(self):
+        return (self.n_features,) if self.n_agents is None else (self.n_agents, self.n_features)
+
+    def _as_coeffs(self, val, name):
+        c = torch.as_tensor(np.asarray(val, dtype=np.float64) if not torch.is_tensor(val) else val)
+        _require_dtype(c, name, (torch.float64,))
+        return c
 
     def get_param_values(self):
-        """float64 coefficients [Df] (NumPy), or None before the first fit."""
+        """float64 coefficients [Df] ([A, Df] per agent) (NumPy), or None before the first fit."""
         return None if self._coeffs is None else self._coeffs.cpu().numpy()
 
-    def set_param_values(self, val):
+    def set_param_values(self, val, carry=None):
+        """``carry`` [Df] (shared flavour only): the coefficients the next fit gives agent 0; None = zeros, as
+        before any fit."""
+        if carry is not None and not self.shared:
+            raise ValueError("carry only exists for shared=True")
+        if carry is not None:
+            cc = self._as_coeffs(carry, "carry")
+            _require_shape(cc, "carry", (self.n_features,))
         if val is None:
             self._coeffs = None
-            return
-        c = torch.as_tensor(np.asarray(val, dtype=np.float64) if not torch.is_tensor(val) else val)
-        _require_dtype(c, "coefficients", (torch.float64,))
-        _require_shape(c, "coefficients", (self.n_features,))
-        self._coeffs = c.to(self.device).contiguous().clone()
+        else:
+            c = self._as_coeffs(val, "coefficients")
+            _require_shape(c, "coefficients", self._coef_shape())
+            self._coeffs = c.to(self.device).contiguous().clone()
+        if self.shared:
+            self._carry = None if carry is None else cc.to(self.device).contiguous().clone()
+
+    @property
+    def carry(self):
+        """Shared flavour: the last fit's agent A-1 coefficients [Df] (NumPy), None before any fit."""
+        return None if self._carry is None else self._carry.cpu().numpy()
 
     def _rows(self, obs, done, obs_before, t0, returns=None):
         """Validates the rollout tensors (before any pointer reaches a kernel) and runs the path plan."""
@@ -282,6 +377,8 @@ class LinearFeatureBaseline(object):
         T, E, A, D = obs.shape
         if D != self.obs_dim:
             raise ValueError("obs has %d features per row, the baseline was built for %d" % (D, self.obs_dim))
+        if self.n_agents is not None and A != self.n_agents:
+            raise ValueError("obs has %d agents, the baseline was built for %d" % (A, self.n_agents))
         _require_shape(done, "done", (T, E))
         if obs_before is not None:
             _require_shape(obs_before, "obs_before", (E, A, D))
@@ -307,23 +404,51 @@ class LinearFeatureBaseline(object):
         return (T, E, A, D), cont(obs), cont(obs_before), cont(t0), seg_s
 
     def normal_equations(self, obs, done, returns, obs_before=None, t0=None):
-        """G = [F y]ᵀ[F y], float64 [Df+1, Df+1] on the device: FᵀF, with Fᵀy as row and column Df."""
+        """G = [F y]ᵀ[F y], float64 [Df+1, Df+1] on the device: FᵀF, with Fᵀy as row and column Df.
+        Per agent: [A, Df+1, Df+1], agent a's system from its rows only."""
         (T, E, A, D), obs, obs_before, t0, seg_s = self._rows(obs, done, obs_before, t0, returns)
         returns = returns.contiguous()
         L = _lib.lib()
         nbytes = C.c_size_t()
-        _lib.check(L.madrl_lfb_workspace_size(D, C.byref(nbytes)))
+        per_agent = self.n_agents is not None
+        if per_agent:
+            _lib.check(L.madrl_lfb_agents_workspace_size(D, A, C.byref(nbytes)))
+        else:
+            _lib.check(L.madrl_lfb_workspace_size(D, C.byref(nbytes)))
         ws = torch.empty(nbytes.value // 8, dtype=torch.float64, device=self.device)
-        G = torch.empty((self.n_features + 1, self.n_features + 1), dtype=torch.float64, device=self.device)
+        Dc = self.n_features + 1
+        G = torch.empty(((A,) if per_agent else ()) + (Dc, Dc), dtype=torch.float64, device=self.device)
+        fn = _obs_fn("lfb_normal_eq_agents" if per_agent else "lfb_normal_eq", obs.dtype)
         with torch.cuda.device(self.device):
-            _lib.check(_obs_fn("lfb_normal_eq", obs.dtype)(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s),
-                                                           _ptr(t0), _ptr(returns), _ptr(G), _ptr(ws),
-                                                           _stream(self.device)))
+            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(returns), _ptr(G),
+                          _ptr(ws), _stream(self.device)))
         return G
 
-    def solve(self, G):
-        """Coefficients from normal equations G (as `normal_equations` returns them), rllab's regularisation."""
+    def _host_lstsq(self, M, b):
+        """rllab's loop (linear_feature_baseline.py:29-37) on the host."""
         Df = self.n_features
+        Mn, bn, reg = M.cpu().numpy(), b.cpu().numpy(), self.reg_coeff
+        for _ in range(5):
+            c = np.linalg.lstsq(Mn + reg * np.identity(Df), bn, rcond=None)[0]
+            if np.all(np.isfinite(c)):
+                break
+            reg *= 10
+        return torch.from_numpy(c).to(M.device)
+
+    def solve(self, G):
+        """Coefficients from normal equations G (as `normal_equations` returns them), rllab's regularisation.
+        A stack [A, Df+1, Df+1] is solved by one batched Cholesky; only the agents whose factorisation fails
+        take the host loop, the others keep their Cholesky solution."""
+        Df = self.n_features
+        if G.dim() == 3:
+            M, b = G[:, :Df, :Df], G[:, :Df, Df]
+            eye = torch.eye(Df, dtype=G.dtype, device=G.device)
+            Lc, info = torch.linalg.cholesky_ex(M + self.reg_coeff * eye)
+            c = torch.cholesky_solve(b.unsqueeze(-1), Lc).squeeze(-1)
+            ok = ((info == 0) & torch.isfinite(c).all(dim=1)).cpu()
+            for a in torch.nonzero(~ok).flatten().tolist():
+                c[a] = self._host_lstsq(M[a], b[a])
+            return c
         M, b = G[:Df, :Df], G[:Df, Df]
         Lc, info = torch.linalg.cholesky_ex(M + self.reg_coeff * torch.eye(Df, dtype=G.dtype, device=G.device))
         if int(info) == 0:
@@ -331,35 +456,77 @@ class LinearFeatureBaseline(object):
             if bool(torch.isfinite(c).all()):
                 return c
         # the factorisation failed: rllab's loop (linear_feature_baseline.py:29-37) on the host
-        Mn, bn, reg = M.cpu().numpy(), b.cpu().numpy(), self.reg_coeff
-        for _ in range(5):
-            c = np.linalg.lstsq(Mn + reg * np.identity(Df), bn, rcond=None)[0]
-            if np.all(np.isfinite(c)):
-                break
-            reg *= 10
-        return torch.from_numpy(c).to(G.device)
+        return self._host_lstsq(M, b)
 
     def fit(self, obs, done, returns, obs_before=None, t0=None, group=None):
         """Fit to ``returns`` [T,E,A] float32 (``gae``'s second output).  With a ``torch.distributed`` group the
-        normal equations are summed over its ranks before the solve (every rank gets the pooled coefficients;
-        no observation moves)."""
+        normal equations (the per-agent stack) are summed over its ranks before the solve (every rank gets the
+        pooled coefficients; no observation moves)."""
         G = self.normal_equations(obs, done, returns, obs_before, t0)
         if group is not None:
             import torch.distributed as dist
             dist.all_reduce(G, op=dist.ReduceOp.SUM, group=group)
-        self._coeffs = self.solve(G)
+        c = self.solve(G)
+        if self.shared:
+            prev = self._carry if self._carry is not None else torch.zeros_like(c[0])
+            self._coeffs = torch.cat([prev.unsqueeze(0), c[:-1]]).contiguous()
+            self._carry = c[-1].clone()
+        else:
+            self._coeffs = c.contiguous()
 
     def predict(self, obs, done, obs_before=None, t0=None):
-        """values [T,E,A] float32 = features(row) . coefficients, evaluated in float64; zeros before the first fit."""
+        """values [T,E,A] float32 = features(row) . coefficients, evaluated in float64; zeros before the first fit.
+        Per agent: row (t, e, a) with coefficient row a."""
         (T, E, A, D), obs, obs_before, t0, seg_s = self._rows(obs, done, obs_before, t0)
         values = torch.empty((T, E, A), dtype=torch.float32, device=self.device)
         if self._coeffs is None:
             return values.zero_()
+        fn = _obs_fn("lfb_predict" if self.n_agents is None else "lfb_predict_agents", obs.dtype)
         with torch.cuda.device(self.device):
-            _lib.check(_obs_fn("lfb_predict", obs.dtype)(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s),
-                                                         _ptr(t0), _ptr(self._coeffs), _ptr(values),
-                                                         _stream(self.device)))
+            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(self._coeffs),
+                          _ptr(values), _stream(self.device)))
         return values
+
+
+def process_samples_concurrent(baseline, obs, done, rew, discount, gae_lambda, obs_before=None, t0=None,
+                               center_adv=True, positive_adv=False, group=None):
+    """The non-recurrent concurrent branch of rllab's ``BatchMASampler.process_samples``
+    (batch_ma_sampler.py:64-123) and its baseline fit (:184-188) over one rollout, for every agent at once.
+
+    Per agent, in the reference's order: predict with the agent's baseline, GAE advantages and discounted
+    returns per path (``gae``: paths end at ``done`` and at the end of the rollout, bootstrap 0), the explained
+    variance of the predictions over the agent's samples, ``center_advantages`` / ``shift_advantages_to_positive``
+    over the agent's samples, then the fit to the agent's returns.  ``baseline``: a ``LinearFeatureBaseline``
+    with ``n_agents``; with ``shared=True`` the runner's single object (see the class), which is fitted first
+    -- the returns do not depend on the values -- and then predicts.
+
+    obs [T,E,A,D], done [T,E] uint8, rew [T,E,A] float32 (cuda) -> (values, advantages, returns) [T,E,A] and the
+    A explained variances (a list of floats)."""
+    if not isinstance(baseline, LinearFeatureBaseline) or baseline.n_agents is None:
+        raise ValueError("process_samples_concurrent needs a LinearFeatureBaseline built with n_agents")
+    for t, n in ((obs, "obs"), (rew, "rew")):
+        if not torch.is_tensor(t):
+            raise TypeError("%s must be a torch.Tensor, got %r" % (n, type(t)))
+    _require_dtype(rew, "rew")
+    if obs.dim() != 4:
+        raise ValueError("obs must be [T, E, A, D], got shape %s" % (tuple(obs.shape),))
+    if obs.shape[2] != baseline.n_agents:
+        raise ValueError("obs has %d agents, the baseline was built for %d" % (obs.shape[2], baseline.n_agents))
+    _require_shape(rew, "rew", tuple(obs.shape[:3]))
+    if baseline.shared:
+        _, ret = gae(rew, torch.zeros_like(rew), done, discount, gae_lambda)
+        baseline.fit(obs, done, ret, obs_before, t0, group)
+        values = baseline.predict(obs, done, obs_before, t0)
+        adv, _ = gae(rew, values, done, discount, gae_lambda)
+    else:
+        values = baseline.predict(obs, done, obs_before, t0)
+        adv, ret = gae(rew, values, done, discount, gae_lambda)
+    ev = explained_variance(values, ret, per_agent=True)
+    if center_adv or positive_adv:
+        adv = center_advantages(adv, center_adv, positive_adv, inplace=True, per_agent=True)
+    if not baseline.shared:
+        baseline.fit(obs, done, ret, obs_before, t0, group)
+    return values, adv, ret, ev
 
 
 def to_paths(obs, actions, rew, done, infos=None):
