@@ -6,6 +6,8 @@ engine class raises.  PyTorch is used only to own device memory and streams.
 import ctypes as C
 import os
 
+import torch
+
 from . import build as _build
 
 _lib = None
@@ -202,25 +204,43 @@ def lib():
     return _lib
 
 
-def require_tensor(t, name, dtype, shape, device):
-    """Validate a caller-supplied tensor before its data_ptr() crosses the C ABI (a wrong dtype,
-    a non-contiguous view or a short buffer would otherwise be silent garbage or an out-of-bounds
-    device write).  `device`: a torch.device for device buffers, 'cpu' for host buffers."""
-    import torch
+def require_tensor(t, name, dtype, shape, device, contiguous=True, optional=False):
+    """Validate a caller-supplied tensor before its data_ptr() crosses the C ABI.  The kernels trust the
+    sizes they are given: a wrong dtype, a short buffer, a host or foreign-device pointer or a strided view
+    would otherwise be silent garbage or an out-of-bounds device access.
+
+    `dtype`: a dtype or a tuple of them.  `shape`: a tuple of sizes; None matches any size, and a trailing
+    ``...`` any number of further dimensions (``(...,)``: any shape).  `device`: a torch.device; 'cuda' for
+    any CUDA device; 'cpu' for host buffers; None to leave it to a later call, once the shapes of every
+    tensor of the call are checked.  `contiguous=False`: a read-only input the caller copies with
+    .contiguous().  `optional=True`: None passes through.  Raises TypeError (not a tensor, wrong dtype),
+    then ValueError (shape, device, contiguity), naming `name`; returns `t`."""
+    if t is None and optional:
+        return None
     if not isinstance(t, torch.Tensor):
         raise TypeError("%s must be a torch.Tensor, got %r" % (name, type(t)))
-    if t.dtype != dtype:
-        raise TypeError("%s must be %s, got %s" % (name, dtype, t.dtype))
-    if tuple(t.shape) != tuple(shape):
-        raise ValueError("%s must have shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
-    if not t.is_contiguous():
-        raise ValueError("%s must be contiguous" % name)
-    if device == 'cpu':
-        if t.device.type != 'cpu':
-            raise ValueError("%s must be a host tensor, got %s" % (name, t.device))
-    elif t.device != device:
+    dtypes = dtype if isinstance(dtype, tuple) else (dtype,)
+    if t.dtype not in dtypes:
+        raise TypeError("%s must be %s, got %s" % (name, " or ".join(map(str, dtypes)), t.dtype))
+    got = tuple(t.shape)
+    if got != shape:
+        tail = shape[-1:] == (...,)
+        fixed = shape[:-1] if tail else shape
+        if (len(got) < len(fixed) if tail else len(got) != len(fixed)) or \
+                any(s is not None and s != n for s, n in zip(fixed, got)):
+            raise ValueError("%s must have shape [%s], got [%s]" % (
+                name, ", ".join("*" if s is None else "..." if s is ... else str(s) for s in shape),
+                ", ".join(map(str, got))))
+    if device is not None and (t.device.type != device if isinstance(device, str) else t.device != device):
         raise ValueError("%s must live on %s, got %s" % (name, device, t.device))
+    if contiguous and not t.is_contiguous():
+        raise ValueError("%s must be contiguous" % name)
     return t
+
+
+def stream(device):
+    """The current torch stream of `device`, as the cudaStream_t argument of the C ABI."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def check(rc):

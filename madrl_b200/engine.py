@@ -51,6 +51,7 @@ class BatchedEngine(object):
             _lib.check(self._fn("create")(C.byref(cfg), *create_args, _ptr(self._blob), C.byref(h)))
         self._h = h
         self.obs_dtype = obs_dtype
+        self._term_obs = None   # set_terminal_obs
         if obs_dtype == torch.bfloat16:
             _lib.check(self._fn("set_obs_format")(self._h, _lib.OBS_BF16))
 
@@ -66,19 +67,14 @@ class BatchedEngine(object):
         n = int(np.prod(shape)) * torch.empty((), dtype=dtype).element_size()
         return self._blob[off:off + n].view(dtype).view(*shape)
 
-    def _stream(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def set_terminal_obs(self, term_obs):
         """Keep the terminal observations of done steps: `term_obs` (same shape / obs_dtype as the obs tensor
-        of the following auto-reset rollouts) receives, at the [t, e] slots where `done` is set, the
-        observation the env returned BEFORE it was reset in place (StandardizedEnv needs it,
+        of the following auto-reset rollouts, which check it) receives, at the [t, e] slots where `done` is set,
+        the observation the env returned BEFORE it was reset in place (StandardizedEnv needs it,
         madrl_environments/__init__.py:283-291).  None switches it off."""
-        if term_obs is not None:
-            assert term_obs.is_contiguous() and term_obs.device == self.device, "term_obs must be a contiguous device tensor"
-            if term_obs.dtype != self.obs_dtype:
-                raise TypeError("term_obs must be %s, got %s" % (self.obs_dtype, term_obs.dtype))
-        self._term_keepalive = term_obs
+        _lib.require_tensor(term_obs, "term_obs", self.obs_dtype, (None, self.n_envs, self._n_acting, self.obs_dim),
+                            self.device, optional=True)
+        self._term_obs = term_obs
         _lib.check(self._fn("set_terminal_obs")(self._h, _ptr(term_obs)))
 
     def set_launch(self, warps_per_block=0, blocks_per_sm=0):
@@ -86,7 +82,7 @@ class BatchedEngine(object):
 
     def seed(self, seed=None):
         with torch.cuda.device(self.device):
-            _lib.check(self._fn("seed")(self._h, 0 if seed is None else int(seed), self._stream()))
+            _lib.check(self._fn("seed")(self._h, 0 if seed is None else int(seed), _lib.stream(self.device)))
         return [seed]
 
     def reset(self, mask=None, out=None):
@@ -96,9 +92,10 @@ class BatchedEngine(object):
         if out is not None:
             _lib.require_tensor(out, "out", self.obs_dtype, shape, self.device)
         if mask is not None:
-            mask = mask.to(device=self.device, dtype=torch.uint8).contiguous()
+            mask = _lib.require_tensor(mask.to(device=self.device, dtype=torch.uint8).contiguous(), "mask", torch.uint8,
+                                       (self.n_envs,), self.device)
         with torch.cuda.device(self.device):
-            _lib.check(self._fn("reset")(self._h, _ptr(mask), _ptr(obs), self._stream()))
+            _lib.check(self._fn("reset")(self._h, _ptr(mask), _ptr(obs), _lib.stream(self.device)))
         return obs
 
     def _trajectory_shapes(self, T):
@@ -107,9 +104,13 @@ class BatchedEngine(object):
         return ((self.obs_dtype, (T, E, A, self.obs_dim)), (self.dtype, (T, E, A)), (torch.uint8, (T, E)),
                 (torch.int32, (T, E) + self._info_tail))
 
-    def _outputs(self, T, out):
+    def _outputs(self, T, out, auto_reset):
         """The trajectory buffers of a T-step device rollout: `out` after checking dtype / shape /
-        contiguity / placement, or new ones."""
+        contiguity / placement, or new ones.  An auto-reset rollout also writes the set_terminal_obs
+        tensor, which must then have the shape of its obs tensor."""
+        if auto_reset and self._term_obs is not None:
+            _lib.require_tensor(self._term_obs, "the set_terminal_obs tensor", self.obs_dtype,
+                                (T, self.n_envs, self._n_acting, self.obs_dim), self.device)
         if out is None:   # spelled out: this is on the per-step path of the single-env drop-ins
             E, A, dev = self.n_envs, self._n_acting, self.device
             return (torch.empty((T, E, A, self.obs_dim), dtype=self.obs_dtype, device=dev),
@@ -125,19 +126,19 @@ class BatchedEngine(object):
         """T lockstep steps in one kernel launch.  actions [T, E, A, *act_tail] ->
         (obs [T,E,A,D], rew [T,E,A], done [T,E] uint8, info [T,E,*info_tail] int32)."""
         actions = actions.to(device=self.device, dtype=self._act_dtype).contiguous()
-        T = actions.shape[0]
-        assert actions.shape == (T, self.n_envs, self._n_acting) + self._act_tail, actions.shape
-        obs, rew, done, info = self._outputs(T, out)
+        T = _lib.require_tensor(actions, "actions", self._act_dtype,
+                                (None, self.n_envs, self._n_acting) + self._act_tail, self.device).shape[0]
+        obs, rew, done, info = self._outputs(T, out, auto_reset)
         with torch.cuda.device(self.device):
             _lib.check(self._fn("rollout")(self._h, T, _ptr(actions), _ptr(obs), _ptr(rew),
-                                           _ptr(done), _ptr(info), int(auto_reset), self._stream()))
+                                           _ptr(done), _ptr(info), int(auto_reset), _lib.stream(self.device)))
         return obs, rew, done, info
 
     def _rollout_heuristic(self, T, obs0, auto_reset, out, record_actions, actions_out, *extra):
         """madrl_<abi>_rollout_heuristic; `extra`: the family's arguments before the stream."""
         E, A = self.n_envs, self._n_acting
         _lib.require_tensor(obs0, "obs0", self.obs_dtype, (E, A, self.obs_dim), self.device)
-        obs, rew, done, info = self._outputs(T, out)
+        obs, rew, done, info = self._outputs(T, out, auto_reset)
         act_shape = (T, E, A) + self._act_tail
         if actions_out is not None:   # caller-owned buffer for the actions taken (no allocation in a rollout loop)
             act = _lib.require_tensor(actions_out, "actions_out", self._act_dtype, act_shape, self.device)
@@ -146,7 +147,7 @@ class BatchedEngine(object):
         with torch.cuda.device(self.device):
             _lib.check(self._fn("rollout_heuristic")(self._h, T, _ptr(obs0), _ptr(act), _ptr(obs), _ptr(rew),
                                                      _ptr(done), _ptr(info), int(auto_reset), *extra,
-                                                     self._stream()))
+                                                     _lib.stream(self.device)))
         return act, obs, rew, done, info
 
     def step(self, actions, auto_reset=False):

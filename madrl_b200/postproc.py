@@ -24,15 +24,9 @@ import torch
 from . import _lib
 from ._lib import _ptr
 
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
-def _require_dtype(t, name, dtypes=(torch.float32,)):
-    """The passes read and write raw buffers: a tensor of another dtype must not reach them."""
-    if t is not None and t.dtype not in dtypes:
-        raise TypeError("%s must be %s, got %s" % (name, " or ".join(str(d) for d in dtypes), t.dtype))
+# Argument checks (_lib.require_tensor): every tensor of a call is checked against the shape derived from its
+# first tensor and must sit on that tensor's device.  That device is checked last (it must be CUDA, and where an
+# object owns state, the state's device), so that a call on host tensors reports a wrong dtype or shape first.
 
 
 def _obs_fn(name, dtype):
@@ -41,6 +35,7 @@ def _obs_fn(name, dtype):
 
 
 _OBS_DTYPES = (torch.float32, torch.bfloat16)
+_PACKED_DTYPES = (torch.float32, torch.int32, torch.uint32, torch.bfloat16)   # pack_paths moves 4- and 2-byte words
 
 
 def gae(rew, values, done, discount, gae_lambda, last_value=None):
@@ -48,17 +43,19 @@ def gae(rew, values, done, discount, gae_lambda, last_value=None):
 
     Paths end where ``done`` is set (bootstrap 0, base.py:57) and at the end of the rollout
     (bootstrap ``last_value`` [E,A] if given, else 0)."""
-    for t, n in ((rew, "rew"), (values, "values"), (last_value, "last_value")):
-        _require_dtype(t, n)
-    _require_dtype(done, "done", (torch.uint8,))
+    T, E, A = _lib.require_tensor(rew, "rew", torch.float32, (None, None, None), None, contiguous=False).shape
+    dev = rew.device
+    _lib.require_tensor(values, "values", torch.float32, (T, E, A), dev, contiguous=False)
+    _lib.require_tensor(done, "done", torch.uint8, (T, E), dev, contiguous=False)
+    _lib.require_tensor(last_value, "last_value", torch.float32, (E, A), dev, contiguous=False, optional=True)
+    _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), "cuda", contiguous=False)
     rew, values, done = rew.contiguous(), values.contiguous(), done.contiguous()
-    T, E, A = rew.shape
     adv, ret = torch.empty_like(rew), torch.empty_like(rew)
     lv = last_value.contiguous() if last_value is not None else None
-    with torch.cuda.device(rew.device):
+    with torch.cuda.device(dev):
         _lib.check(_lib.lib().madrl_gae_f32(T, E, A, _ptr(rew), _ptr(values), _ptr(done), _ptr(lv),
                                             float(discount), float(gae_lambda), _ptr(adv), _ptr(ret),
-                                            _stream(rew.device)))
+                                            _lib.stream(dev)))
     return adv, ret
 
 
@@ -74,7 +71,9 @@ AGENTS_MAX = 1024                               # include/madrl_b200.h MADRL_AGE
 
 
 def _agent_columns(t, name):
-    """(rows, A) of a tensor whose last axis is the agent; raises before any library call."""
+    """(rows, A) of a float32 tensor whose last axis is the agent; raises before any library call.  Its
+    device is left to the caller."""
+    _lib.require_tensor(t, name, torch.float32, (...,), None, contiguous=False)
     if t.dim() < 1 or t.shape[-1] < 1 or t.numel() == 0:
         raise ValueError("%s must have a non-empty last (agent) axis, got shape %s" % (name, tuple(t.shape)))
     A = int(t.shape[-1])
@@ -90,9 +89,9 @@ def center_advantages(adv, center=True, positive=False, inplace=False, per_agent
     ``per_agent=True``: the last axis of ``adv`` (e.g. [T,E,A]) is the agent, and each agent's samples are
     centred with their own statistics, as the concurrent sampler does per agent
     (batch_ma_sampler.py:102-106)."""
-    _require_dtype(adv, "adv")
     if per_agent:
         rows, A = _agent_columns(adv, "adv")
+    _lib.require_tensor(adv, "adv", torch.float32, (...,), "cuda", contiguous=False)
     out = adv.contiguous() if inplace else adv.contiguous().clone()
     if per_agent:
         stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=out.device)
@@ -100,46 +99,44 @@ def center_advantages(adv, center=True, positive=False, inplace=False, per_agent
         with torch.cuda.device(out.device):
             _lib.check(_lib.lib().madrl_center_advantages_agents_f32(rows, A, _ptr(out), int(bool(center)),
                                                                      int(bool(positive)), _ptr(stats), _ptr(ws),
-                                                                     _stream(out.device)))
+                                                                     _lib.stream(out.device)))
         return out
     stats, ws = _moments_buffers(out.device)
     with torch.cuda.device(out.device):
         _lib.check(_lib.lib().madrl_center_advantages_f32(out.numel(), _ptr(out), int(bool(center)),
                                                           int(bool(positive)), _ptr(stats), _ptr(ws),
-                                                          _stream(out.device)))
+                                                          _lib.stream(out.device)))
     return out
 
 
 def moments(a, b=None):
     """float64 [9] cuda tensor: means, population variances and minima of the series a, b, b - a
-    taken over every element (NumPy's two-pass ``var``)."""
-    _require_dtype(a, "a")
-    _require_dtype(b, "b")
+    (b of a's shape) taken over every element (NumPy's two-pass ``var``)."""
+    _lib.require_tensor(a, "a", torch.float32, (...,), None, contiguous=False)
+    _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
+    _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
     a = a.contiguous()
     b = b.contiguous() if b is not None else None
-    assert b is None or b.numel() == a.numel()
     stats, ws = _moments_buffers(a.device)
     with torch.cuda.device(a.device):
         _lib.check(_lib.lib().madrl_moments_f32(a.numel(), _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
-                                                _stream(a.device)))
+                                                _lib.stream(a.device)))
     return stats
 
 
 def moments_agents(a, b=None):
     """float64 [A, 9] cuda tensor: ``moments`` of each agent's samples, the agent being the last axis of
     a (and b), e.g. [T,E,A]."""
-    _require_dtype(a, "a")
-    _require_dtype(b, "b")
     rows, A = _agent_columns(a, "a")
-    if b is not None and tuple(b.shape) != tuple(a.shape):
-        raise ValueError("b must have shape %s, got %s" % (tuple(a.shape), tuple(b.shape)))
+    _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
+    _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
     a = a.contiguous()
     b = b.contiguous() if b is not None else None
     stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=a.device)
     ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=a.device)
     with torch.cuda.device(a.device):
         _lib.check(_lib.lib().madrl_moments_agents_f32(rows, A, _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
-                                                       _stream(a.device)))
+                                                       _lib.stream(a.device)))
     return stats
 
 
@@ -166,28 +163,29 @@ class FrameStack(object):
     ``obs_dtype=torch.bfloat16``); the stack keeps it (values are only moved)."""
 
     def __init__(self, n_envs, n_agents, obs_dim, buffer_size, device, dtype=torch.float32):
-        _require_dtype(torch.empty(0, dtype=dtype), "dtype", _OBS_DTYPES)
+        if dtype not in _OBS_DTYPES:
+            raise TypeError("dtype must be torch.float32 or torch.bfloat16, got %s" % dtype)
         self.shape, self.dtype = (n_envs, n_agents, obs_dim, buffer_size), dtype
         self.carry = torch.zeros(self.shape, dtype=dtype, device=device)   # __init__.py:150
 
     def reset(self, obs0):
         """obs0 [E,A,D] from engine.reset() -> stacked [E,A,D,B] (__init__.py:186-196)."""
-        _require_dtype(obs0, "obs0", (self.dtype,))
+        _lib.require_tensor(obs0, "obs0", self.dtype, (...,), None, contiguous=False)   # copied by torch, not the ABI
         self.carry.copy_(obs0.unsqueeze(-1).expand(self.shape))
         return self.carry.clone()
 
     def rollout(self, obs, done):
         """obs [T,E,A,D], done [T,E] from engine.rollout(auto_reset=True) -> [T,E,A,D,B]."""
-        _require_dtype(obs, "obs", (self.dtype,))
-        _require_dtype(done, "done", (torch.uint8,))
-        obs, done = obs.contiguous(), done.contiguous()
-        T = obs.shape[0]
         E, A, D, B = self.shape
-        assert tuple(obs.shape) == (T, E, A, D) and tuple(done.shape) == (T, E), (obs.shape, done.shape)
+        T = _lib.require_tensor(obs, "obs", self.dtype, (None, E, A, D), None, contiguous=False).shape[0]
+        _lib.require_tensor(done, "done", torch.uint8, (T, E), obs.device, contiguous=False)
+        _lib.require_tensor(self.carry, "FrameStack.carry", self.dtype, self.shape, "cuda")
+        _lib.require_tensor(obs, "obs", self.dtype, (T, E, A, D), self.carry.device, contiguous=False)
+        obs, done = obs.contiguous(), done.contiguous()
         out = torch.empty((T, E, A, D, B), dtype=self.dtype, device=obs.device)
         with torch.cuda.device(obs.device):
             _lib.check(_obs_fn("frame_stack", self.dtype)(T, E, A, D, B, _ptr(obs), _ptr(done),
-                                                          _ptr(self.carry), _ptr(out), _stream(obs.device)))
+                                                          _ptr(self.carry), _ptr(out), _lib.stream(obs.device)))
         return out
 
 
@@ -216,34 +214,37 @@ class Standardizer(object):
         values and are rounded once, at the store."""
         if not self.enable_obsnorm:
             return obs
-        _require_dtype(obs, "obs", _OBS_DTYPES)
-        x = obs if obs.dim() == 4 else obs.unsqueeze(0)
-        assert x.is_contiguous() and x[0].numel() == self.obs_mean.numel(), (x.shape, self.obs_mean.shape)
+        E, A, D = self.obs_mean.shape
+        x = obs.unsqueeze(0) if torch.is_tensor(obs) and obs.dim() == 3 else obs
+        T = _lib.require_tensor(x, "obs", _OBS_DTYPES, (None, E, A, D), None).shape[0]
         if terminal_obs is not None:
-            _require_dtype(terminal_obs, "terminal_obs", (x.dtype,))
-            _require_dtype(done, "done", (torch.uint8,))
-            assert done is not None and terminal_obs.shape == x.shape and terminal_obs.is_contiguous()
-            E = x.shape[1]
+            _lib.require_tensor(terminal_obs, "terminal_obs", x.dtype, (T, E, A, D), x.device)
+            _lib.require_tensor(done, "done", torch.uint8, (T, E), x.device, contiguous=False)
+        _lib.require_tensor(self.obs_mean, "Standardizer.obs_mean", torch.float64, (E, A, D), "cuda")
+        _lib.require_tensor(x, "obs", x.dtype, (T, E, A, D), self.obs_mean.device)
+        if terminal_obs is not None:
             with torch.cuda.device(x.device):
                 _lib.check(_obs_fn("standardize_obs_terminal", x.dtype)(
-                    x.shape[0], E, self.obs_mean.numel() // E, _ptr(x), _ptr(terminal_obs), _ptr(done.contiguous()),
-                    _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha, self.eps, _stream(x.device)))
+                    T, E, A * D, _ptr(x), _ptr(terminal_obs), _ptr(done.contiguous()),
+                    _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha, self.eps, _lib.stream(x.device)))
             return obs
         with torch.cuda.device(x.device):
-            _lib.check(_obs_fn("standardize", x.dtype)(x.shape[0], self.obs_mean.numel(), _ptr(x),
+            _lib.check(_obs_fn("standardize", x.dtype)(T, self.obs_mean.numel(), _ptr(x),
                                                        _ptr(self.obs_mean), _ptr(self.obs_var), self.obs_alpha,
-                                                       self.eps, 1, 1.0, 1, _stream(x.device)))
+                                                       self.eps, 1, 1.0, 1, _lib.stream(x.device)))
         return obs
 
     def rew(self, rew):
         """In place on rew [T,E,A]: optional running-std division, then scale_reward."""
-        _require_dtype(rew, "rew")
-        assert rew.is_contiguous() and rew[0].numel() == self.rew_mean.numel(), rew.shape
+        E, A = self.rew_mean.shape
+        T = _lib.require_tensor(rew, "rew", torch.float32, (None, E, A), None).shape[0]
+        _lib.require_tensor(self.rew_mean, "Standardizer.rew_mean", torch.float64, (E, A), "cuda")
+        _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), self.rew_mean.device)
         with torch.cuda.device(rew.device):
-            _lib.check(_lib.lib().madrl_standardize_f32(rew.shape[0], self.rew_mean.numel(), _ptr(rew),
+            _lib.check(_lib.lib().madrl_standardize_f32(T, self.rew_mean.numel(), _ptr(rew),
                                                         _ptr(self.rew_mean), _ptr(self.rew_var), self.rew_alpha,
                                                         self.eps, 0, float(self.scale_reward),
-                                                        int(self.enable_rewnorm), _stream(rew.device)))
+                                                        int(self.enable_rewnorm), _lib.stream(rew.device)))
         return rew
 
 
@@ -260,11 +261,12 @@ class EpisodeStats(object):
     def rollout(self, rew, done):
         """rew [T,E,A] float32, done [T,E] uint8 -> dict(end [T,E] bool, episode_reward [T,E,A],
         episode_avg_reward [T,E], episode_disc_return [T,E], episode_length [T,E])."""
-        _require_dtype(rew, "rew")
-        _require_dtype(done, "done", (torch.uint8,))
-        rew, done = rew.contiguous(), done.contiguous()
-        T, E, A = rew.shape
-        dev = rew.device
+        E, A = self.n_envs, self.n_agents
+        T = _lib.require_tensor(rew, "rew", torch.float32, (None, E, A), None, contiguous=False).shape[0]
+        _lib.require_tensor(done, "done", torch.uint8, (T, E), rew.device, contiguous=False)
+        _lib.require_tensor(self.carry, "EpisodeStats.carry", torch.float64, (E, A + 3), "cuda")
+        _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), self.carry.device, contiguous=False)
+        rew, done, dev = rew.contiguous(), done.contiguous(), rew.device
         ep_r = torch.empty((T, E, A), dtype=torch.float32, device=dev)
         ep_d = torch.empty((T, E), dtype=torch.float32, device=dev)
         ep_l = torch.empty((T, E), dtype=torch.int32, device=dev)
@@ -272,14 +274,9 @@ class EpisodeStats(object):
         with torch.cuda.device(dev):
             _lib.check(_lib.lib().madrl_episode_stats_f32(T, E, A, _ptr(rew), _ptr(done), float(self.discount),
                                                           int(self.max_traj_len), _ptr(self.carry), _ptr(ep_r),
-                                                          _ptr(ep_d), _ptr(ep_l), _ptr(ep_e), _stream(dev)))
+                                                          _ptr(ep_d), _ptr(ep_l), _ptr(ep_e), _lib.stream(dev)))
         return dict(end=ep_e.bool(), episode_reward=ep_r, episode_avg_reward=ep_r.mean(dim=-1),
                     episode_disc_return=ep_d, episode_length=ep_l)
-
-
-def _require_shape(t, name, shape):
-    if tuple(t.shape) != tuple(shape):
-        raise ValueError("%s must have shape %s, got %s" % (name, tuple(shape), tuple(t.shape)))
 
 
 class LinearFeatureBaseline(object):
@@ -331,10 +328,9 @@ class LinearFeatureBaseline(object):
     def _coef_shape(self):
         return (self.n_features,) if self.n_agents is None else (self.n_agents, self.n_features)
 
-    def _as_coeffs(self, val, name):
+    def _as_coeffs(self, val, name, shape):
         c = torch.as_tensor(np.asarray(val, dtype=np.float64) if not torch.is_tensor(val) else val)
-        _require_dtype(c, name, (torch.float64,))
-        return c
+        return _lib.require_tensor(c, name, torch.float64, shape, None, contiguous=False)
 
     def get_param_values(self):
         """float64 coefficients [Df] ([A, Df] per agent) (NumPy), or None before the first fit."""
@@ -346,13 +342,11 @@ class LinearFeatureBaseline(object):
         if carry is not None and not self.shared:
             raise ValueError("carry only exists for shared=True")
         if carry is not None:
-            cc = self._as_coeffs(carry, "carry")
-            _require_shape(cc, "carry", (self.n_features,))
+            cc = self._as_coeffs(carry, "carry", (self.n_features,))
         if val is None:
             self._coeffs = None
         else:
-            c = self._as_coeffs(val, "coefficients")
-            _require_shape(c, "coefficients", self._coef_shape())
+            c = self._as_coeffs(val, "coefficients", self._coef_shape())
             self._coeffs = c.to(self.device).contiguous().clone()
         if self.shared:
             self._carry = None if carry is None else cc.to(self.device).contiguous().clone()
@@ -364,31 +358,17 @@ class LinearFeatureBaseline(object):
 
     def _rows(self, obs, done, obs_before, t0, returns=None):
         """Validates the rollout tensors (before any pointer reaches a kernel) and runs the path plan."""
-        for t, n in ((obs, "obs"), (done, "done"), (obs_before, "obs_before"), (t0, "t0"), (returns, "returns")):
-            if t is not None and not torch.is_tensor(t):
-                raise TypeError("%s must be a torch.Tensor, got %r" % (n, type(t)))
-        _require_dtype(obs, "obs", _OBS_DTYPES)
-        _require_dtype(obs_before, "obs_before", (obs.dtype,))
-        _require_dtype(done, "done", (torch.uint8,))
-        _require_dtype(t0, "t0", (torch.int32,))
-        _require_dtype(returns, "returns")
-        if obs.dim() != 4:
-            raise ValueError("obs must be [T, E, A, D], got shape %s" % (tuple(obs.shape),))
-        T, E, A, D = obs.shape
-        if D != self.obs_dim:
-            raise ValueError("obs has %d features per row, the baseline was built for %d" % (D, self.obs_dim))
-        if self.n_agents is not None and A != self.n_agents:
-            raise ValueError("obs has %d agents, the baseline was built for %d" % (A, self.n_agents))
-        _require_shape(done, "done", (T, E))
-        if obs_before is not None:
-            _require_shape(obs_before, "obs_before", (E, A, D))
-        if t0 is not None:
-            _require_shape(t0, "t0", (E,))
-        if returns is not None:
-            _require_shape(returns, "returns", (T, E, A))
-        for t, n in ((obs, "obs"), (done, "done"), (obs_before, "obs_before"), (t0, "t0"), (returns, "returns")):
-            if t is not None and t.device != self.device:
-                raise ValueError("%s must live on %s, got %s" % (n, self.device, t.device))
+        T, E, A, D = _lib.require_tensor(obs, "obs", _OBS_DTYPES, (None, None, self.n_agents, self.obs_dim), None,
+                                         contiguous=False).shape
+        dev = obs.device
+        _lib.require_tensor(done, "done", torch.uint8, (T, E), dev, contiguous=False)
+        _lib.require_tensor(obs_before, "obs_before", obs.dtype, (E, A, D), dev, contiguous=False, optional=True)
+        _lib.require_tensor(t0, "t0", torch.int32, (E,), dev, contiguous=False, optional=True)
+        _lib.require_tensor(returns, "returns", torch.float32, (T, E, A), dev, contiguous=False, optional=True)
+        if self.device.type != "cuda":
+            raise ValueError("this baseline lives on %s: its normal equations and predictions need a CUDA device"
+                             % self.device)
+        _lib.require_tensor(obs, "obs", obs.dtype, (T, E, A, D), self.device, contiguous=False)
         if T * E * A >= 2 ** 31:
             raise ValueError("T*E*A must be < 2^31, got %d" % (T * E * A))
         L = _lib.lib()
@@ -399,7 +379,7 @@ class LinearFeatureBaseline(object):
         ep_rec = torch.empty((E, T, 3), dtype=torch.int32, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(L.madrl_paths_plan(T, E, A, _ptr(done), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep), _ptr(ep_rec),
-                                          _stream(self.device)))
+                                          _lib.stream(self.device)))
         cont = lambda x: None if x is None else x.contiguous()          # noqa: E731
         return (T, E, A, D), cont(obs), cont(obs_before), cont(t0), seg_s
 
@@ -421,7 +401,7 @@ class LinearFeatureBaseline(object):
         fn = _obs_fn("lfb_normal_eq_agents" if per_agent else "lfb_normal_eq", obs.dtype)
         with torch.cuda.device(self.device):
             _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(returns), _ptr(G),
-                          _ptr(ws), _stream(self.device)))
+                          _ptr(ws), _lib.stream(self.device)))
         return G
 
     def _host_lstsq(self, M, b):
@@ -484,7 +464,7 @@ class LinearFeatureBaseline(object):
         fn = _obs_fn("lfb_predict" if self.n_agents is None else "lfb_predict_agents", obs.dtype)
         with torch.cuda.device(self.device):
             _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(self._coeffs),
-                          _ptr(values), _stream(self.device)))
+                          _ptr(values), _lib.stream(self.device)))
         return values
 
 
@@ -504,15 +484,9 @@ def process_samples_concurrent(baseline, obs, done, rew, discount, gae_lambda, o
     A explained variances (a list of floats)."""
     if not isinstance(baseline, LinearFeatureBaseline) or baseline.n_agents is None:
         raise ValueError("process_samples_concurrent needs a LinearFeatureBaseline built with n_agents")
-    for t, n in ((obs, "obs"), (rew, "rew")):
-        if not torch.is_tensor(t):
-            raise TypeError("%s must be a torch.Tensor, got %r" % (n, type(t)))
-    _require_dtype(rew, "rew")
-    if obs.dim() != 4:
-        raise ValueError("obs must be [T, E, A, D], got shape %s" % (tuple(obs.shape),))
-    if obs.shape[2] != baseline.n_agents:
-        raise ValueError("obs has %d agents, the baseline was built for %d" % (obs.shape[2], baseline.n_agents))
-    _require_shape(rew, "rew", tuple(obs.shape[:3]))
+    T, E, A, _ = _lib.require_tensor(obs, "obs", _OBS_DTYPES, (None, None, baseline.n_agents, baseline.obs_dim),
+                                     None, contiguous=False).shape
+    _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), obs.device, contiguous=False)
     if baseline.shared:
         _, ret = gae(rew, torch.zeros_like(rew), done, discount, gae_lambda)
         baseline.fit(obs, done, ret, obs_before, t0, group)
@@ -595,33 +569,34 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
     ``obs`` is used as is (the host ``to_paths`` contract).  Two kernels of csrc/postproc.cu: a plan pass
     over ``done`` and one HBM-bound row permutation per tensor; no host loop.  Tensors of 4-byte elements,
     and bfloat16 observations (2-byte rows, ``madrl_paths_pack_u16``)."""
-    for name, x in [("obs", obs), ("actions", actions), ("rew", rew)] + sorted((infos or {}).items()):
-        if x.element_size() not in (2, 4) or (x.element_size() == 2 and x.dtype != torch.bfloat16):
-            raise TypeError("pack_paths packs 4-byte elements and bfloat16; %s is %s" % (name, x.dtype))
-    _require_dtype(done, "done", (torch.uint8,))
+    T, E, A = _lib.require_tensor(obs, "obs", _PACKED_DTYPES, (None, None, None, ...), None,
+                                  contiguous=False).shape[:3]
+    dev = obs.device
+    _lib.require_tensor(actions, "actions", _PACKED_DTYPES, (T, E, A, ...), dev, contiguous=False)
+    _lib.require_tensor(rew, "rew", _PACKED_DTYPES, (T, E, A), dev, contiguous=False)
+    _lib.require_tensor(done, "done", torch.uint8, (T, E), dev, contiguous=False)
+    for k, v in (infos or {}).items():
+        _lib.require_tensor(v, "infos[%r]" % (k,), _PACKED_DTYPES, (T, E, ...), dev, contiguous=False)
+    if obs_before is not None:   # taken in the observations' dtype
+        obs_before = _lib.require_tensor(obs_before.to(obs.dtype).contiguous(), "obs_before", obs.dtype,
+                                         tuple(obs.shape[1:]), dev)
+    _lib.require_tensor(obs, "obs", obs.dtype, (T, E, A, ...), "cuda", contiguous=False)
     L = _lib.lib()
-    T, E, A = rew.shape
-    dev = rew.device
     done = done.contiguous()
     seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
     seg_l = torch.empty((T, E), dtype=torch.int32, device=dev)
     n_ep = torch.empty((E,), dtype=torch.int32, device=dev)
     ep_rec = torch.zeros((E, T, 3), dtype=torch.int32, device=dev)
     with torch.cuda.device(dev):
-        st = _stream(dev)
+        st = _lib.stream(dev)
         _lib.check(L.madrl_paths_plan(T, E, A, _ptr(done), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep), _ptr(ep_rec), st))
 
         def pack(x, per_agent, first=None):
             x = x.contiguous()
-            assert x.shape[0] == T and x.shape[1] == E, (x.dtype, x.shape)
-            assert not per_agent or x.shape[2] == A, x.shape
             n_agents = A if per_agent else 1
             tail = tuple(x.shape[3:] if per_agent else x.shape[2:])
             D = max(1, int(np.prod(tail)))
             out = torch.empty((T * E * n_agents,) + tail, dtype=x.dtype, device=dev)
-            if first is not None:
-                first = first.to(x.dtype).contiguous()
-                assert first.shape == x.shape[1:], (first.shape, x.shape)
             # per-env tensors (n_agents = 1): the row offset e*T + s + (t - s) = e*T + t for any (s, L)
             fn = L.madrl_paths_pack_u16 if x.element_size() == 2 else L.madrl_paths_pack_u32
             _lib.check(fn(T, E, n_agents, D, _ptr(x), _ptr(first), _ptr(seg_s), _ptr(seg_l), _ptr(out), st))

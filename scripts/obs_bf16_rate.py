@@ -74,7 +74,7 @@ def kernel_rates(wl, fmts, reps):
     g.manual_seed(1234)
     act = bench.make_actions(wl, T, E, "cuda", g)
     engs = {f: engine(wl, dt) for f, dt in fmts.items()}
-    outs = {f: e._outputs(T, None) for f, e in engs.items()}
+    outs = {f: e._outputs(T, None, True) for f, e in engs.items()}
     for e in engs.values():
         e.reset()
     for _ in range(3):
