@@ -58,7 +58,10 @@ __device__ __forceinline__ const O* lfb_row(size_t r, int E, int A, int D, const
 }
 
 // a = i / 100 (correctly rounded, as NumPy's arange(l) / 100.0), a^2 = a * a, a^3 = (a^2 + its rounding error) * a
-// rounded once: NumPy evaluates al ** 3 with pow().
+// rounded once: the correctly rounded cube of a (checked against exact rational arithmetic for every i < 200 000),
+// the same on every device and host.  NumPy's al ** 3 (the reference's _features, and oracle/baseline_oracle.py)
+// goes through a pow() that is within 1 ulp of it; which indices differ depends on the host's NumPy build and SIMD
+// path.
 __device__ __forceinline__ void lfb_time(int idx, double& a1, double& a2, double& a3) {
   a1 = (double)idx / 100.0;
   a2 = a1 * a1;

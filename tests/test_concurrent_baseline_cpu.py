@@ -206,6 +206,8 @@ EMU_SHAPES = [  # T, E, A, D, p_done, obs_before, t0
     (11, 2, 5, 5, 0.3, False, False),
     (5, 2, 3, 70, 0.2, True, True),        # 145 columns: three tiles, pairs off the diagonal
     (13, 2, 20, 3, 0.15, True, False),     # 20 agents: 3 slices per agent (1 in this 3-slice build)
+    (6, 2, 3, 30, 0.2, True, True),        # 65 columns: y alone in the second tile
+    (5, 3, 4, 31, 0.25, False, True),      # 67 columns: the time, constant and return columns cross the tile edge
 ]
 
 

@@ -9,6 +9,9 @@ import shutil
 import numpy as np
 import pytest
 
+import postproc_edges as pe
+from emu import build_emu
+from emu.driver import Guarded
 from oracle import postproc_oracle as po
 
 pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
@@ -29,6 +32,13 @@ def lib():
     L.madrl_episode_stats_f32.argtypes = [i32, i32, i32, vp, vp, dbl, i32, vp, vp, vp, vp, vp, vp]
     L.madrl_moments_f32.argtypes = [C.c_size_t, vp, vp, vp, vp, vp]
     L.madrl_center_advantages_f32.argtypes = [C.c_size_t, vp, i32, i32, vp, vp, vp]
+    L.madrl_moments_agents_f32.argtypes = [C.c_size_t, i32, vp, vp, vp, vp, vp]
+    L.madrl_center_advantages_agents_f32.argtypes = [C.c_size_t, i32, vp, i32, i32, vp, vp, vp]
+    L.madrl_frame_stack_bf16.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
+    L.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.madrl_paths_pack_u32.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.madrl_paths_pack_u16.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
+    L.madrl_standardize_obs_terminal_f32.argtypes = [i32, i32, C.c_size_t] + [vp] * 5 + [dbl, dbl, vp]
     return L
 
 
@@ -207,3 +217,153 @@ def test_standardizer_with_terminal_observations_follows_the_reference_order(lib
                 assert np.array_equal(tm[t, e], term[t, e])          # untouched
             assert np.abs(np.array(mine.obs(d['obs'][t, e].astype(np.float64))) - x[t, e]).max() < 1e-5, (t, e)
         assert np.abs(np.array(mine.obs_mean) - mean[e]).max() < 1e-12
+
+
+# ---------------------------------------------------------------- the edges of tests/test_postproc_edges_gpu.py
+# The same cases and checks (tests/postproc_edges.py), with the size edges of this build: its moments grid is
+# MADRL_MOM_BLOCKS CTAs of 256 threads (build_emu.PER_FILE_FLAGS), so its stride edge is that times 256.
+
+EMU_MOM_BLOCKS = int(next(f.split("=")[1] for f in build_emu.PER_FILE_FLAGS["postproc.cu"]
+                          if f.startswith("-DMADRL_MOM_BLOCKS=")))
+
+
+def test_moments_at_the_grid_stride_edges(lib):
+    """n at the block edge and at one and three grid strides, data offset by 1e4 (a one-pass variance fails)."""
+    for n in pe.stride_sizes(EMU_MOM_BLOCKS):
+        a, b = pe.offset_series(n, n)
+        stats, ws = np.full(9, np.nan), np.empty(4096)
+        assert lib.madrl_moments_f32(n, _p(a), _p(b), _p(stats), _p(ws), None) == 0
+        assert np.allclose(stats, pe.moments_want(a, b), rtol=1e-10, atol=1e-12), n
+
+
+@pytest.mark.parametrize("A", [1, 2, 3, 257])
+def test_agent_moments_and_centring_equal_pooled_bitwise(lib, A):
+    """Agent a's statistics and centred column are the pooled call's on that column alone, bit for bit (same block
+    loop, fold order and constant expressions).  A = 257: the per-agent constants of the centring kernel take a
+    second pass of its strided loop; a launch then has 6 x 257 CTAs of fibers, so that case runs one centring
+    mode and compares the agents on either side of 256 (the GPU test covers every agent and mode)."""
+    rows = 2 * EMU_MOM_BLOCKS * 256 + 7 if A <= 3 else 45
+    x, y = pe.agent_columns(rows, A, A)
+    agents, modes = (range(A), pe.CENTRE_MODES) if A <= 3 else ((0, 255, 256), ((1, 1),))
+    stats, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
+    st1, ws1 = np.empty(9), np.empty(4096)
+    if A <= 3:
+        assert lib.madrl_moments_agents_f32(rows, A, _p(x), _p(y), _p(stats), _p(ws), None) == 0
+        for a in agents:
+            xa, ya = np.ascontiguousarray(x[:, a]), np.ascontiguousarray(y[:, a])
+            assert lib.madrl_moments_f32(rows, _p(xa), _p(ya), _p(st1), _p(ws1), None) == 0
+            assert np.array_equal(stats[a], st1), a
+    for center, positive in modes:
+        xs = Guarded(x.shape, np.float32, x)
+        assert lib.madrl_center_advantages_agents_f32(rows, A, _p(xs.arr), center, positive, _p(stats), _p(ws),
+                                                      None) == 0
+        got = xs.check("adv")
+        for a in agents:
+            xa = x[:, a].copy()
+            assert lib.madrl_center_advantages_f32(rows, _p(xa), center, positive, _p(st1), _p(ws1), None) == 0
+            assert np.array_equal(stats[a], st1) and np.array_equal(got[:, a], xa), (center, positive, a)
+
+
+def test_frame_stack_every_buffer_size(lib):
+    """B = 1..8, float32 and bfloat16, n = E*A*D over several blocks with a tail; three chained calls (done on a
+    call's first step, on every step, never) bit for bit ObservationBuffer's; outputs and carry canary-guarded."""
+    E, A, D = 37, 3, 29
+    for bf16 in (False, True):
+        obs0, calls = pe.frame_stack_calls(E, A, D, 5, bf16)
+        dt = np.uint16 if bf16 else np.float32
+        enc = (lambda v: pe.bf16_bits(v)[0]) if bf16 else (lambda v: v)                      # noqa: E731
+        dec = (lambda v: (v.astype(np.uint32) << 16).view(np.float32)) if bf16 else np.copy   # noqa: E731
+        fn = lib.madrl_frame_stack_bf16 if bf16 else lib.madrl_frame_stack_f32
+        for B in range(1, 9):
+            carry = Guarded((E, A, D, B), dt, enc(obs0)[..., None])
+            outs = []
+            for obs, done in calls:
+                T = obs.shape[0]
+                res = Guarded((T, E, A, D, B), dt, 0)
+                src = np.ascontiguousarray(enc(obs))     # bound: _p keeps only the address of the array
+                assert fn(T, E, A, D, B, _p(src), _p(done), _p(carry.arr), _p(res.arr), None) == 0
+                carry.check("carry")
+                outs.append(dec(res.check("out")))
+            pe.check_frame_stack(obs0, calls, outs, B)
+
+
+def test_standardizer_across_both_inv_std_paths(lib):
+    """Running estimates set so that the updated variance v' lands on 0, subnormals, 1e-300, float32 1e-30 and its
+    neighbours, 1, float32 1e30 and its neighbours and 1e300; one step, within a float32 ulp of the float64
+    (x - m') / (sqrt(v') + eps); then pure scaling and the terminal-observation pass."""
+    eps, alpha = pe.STD_EPS, pe.STD_ALPHA
+    x, m, v, vt = pe.std_reward_case()
+    n = x.size
+    xr, mean, var = x.copy(), m.copy(), v.copy()
+    assert lib.madrl_standardize_f32(1, n, _p(xr), _p(mean), _p(var), alpha, eps, 0, 0.5, 1, None) == 0
+    assert np.array_equal(mean, m) and np.array_equal(var, vt)
+    off = pe.check_standardized(xr, 0.5 * x.astype(np.float64) / (np.sqrt(vt) + eps))
+    xs, mean, var = x.copy(), m.copy(), v.copy()
+    assert lib.madrl_standardize_f32(1, n, _p(xs), _p(mean), _p(var), alpha, eps, 0, 0.5, 0, None) == 0
+    assert np.array_equal(xs, (0.5 * x.astype(np.float64)).astype(np.float32))              # pure scaling
+    assert np.array_equal(mean, m) and np.array_equal(var, v)
+    x, m, v, m1, v1 = pe.std_obs_case()
+    assert all(pe.std_target_classes(v1).values())
+    xo, mean, var = x.copy(), m.copy(), v.copy()
+    assert lib.madrl_standardize_f32(1, x.size, _p(xo), _p(mean), _p(var), alpha, eps, 1, 1.0, 1, None) == 0
+    assert np.array_equal(mean, m1) and np.array_equal(var, v1)
+    off += pe.check_standardized(xo, (x.astype(np.float64) - m1) / (np.sqrt(v1) + eps))
+    assert off <= 2, off
+    obs, term, done = pe.terminal_case(4, 7, 40, 3)
+    T, E, P = obs.shape
+    xt, tm, mean, var = obs.copy(), term.copy(), np.zeros((E, P)), np.ones((E, P))
+    assert lib.madrl_standardize_obs_terminal_f32(T, E, P, _p(xt), _p(tm), _p(done), _p(mean), _p(var), 0.05, eps,
+                                                  None) == 0
+    pe.check_terminal(xt, tm, obs, term, done, 0.05, mean)
+
+
+def test_gae_edges(lib):
+    """E*A over several blocks with a tail; T = 1 and 17; done at t = 0, at T-1, on every step, never; with and
+    without last_value; (gamma, lambda) in {(0.99, 0.95), (1, 1), (0, 0.5)}."""
+    E, A = 301, 3
+    for T in (1, 17):
+        rew, val, last, done = pe.gae_case(T, E, A, T)
+        for discount, lam in pe.GAE_PARAMS:
+            for lv in (None, last):
+                adv, ret = np.full_like(rew, np.nan), np.full_like(rew, np.nan)
+                assert lib.madrl_gae_f32(T, E, A, _p(rew), _p(val), _p(done), _p(lv), discount, lam, _p(adv), _p(ret),
+                                         None) == 0
+                pe.check_gae(adv, ret, rew, val, done, discount, lam, lv)
+
+
+@pytest.mark.parametrize("E,A,kind", [(131, 32, "len1"), (131, 3, "boundary"), (140, 5, "span3")])
+def test_episode_stats_edges(lib, E, A, kind):
+    mtl, calls = pe.episode_stats_calls(E, A, kind, 1)
+    carry, outs = np.zeros((E, A + 3)), []
+    for rew, done in calls:
+        T = rew.shape[0]
+        part = [np.empty((T, E, A), np.float32), np.empty((T, E), np.float32), np.empty((T, E), np.int32),
+                np.empty((T, E), np.uint8)]
+        assert lib.madrl_episode_stats_f32(T, E, A, _p(rew), _p(done), 0.9, mtl, _p(carry), *[_p(p) for p in part],
+                                           None) == 0
+        outs.append(part)
+    assert pe.check_episode_stats(outs, calls, 0.9, mtl) > 0
+
+
+@pytest.mark.parametrize("itemsize", [4, 2], ids=["u32", "u16"])
+def test_path_packing_word_counts(lib, itemsize):
+    """D in {1..5, 31, 32, 33} words (one thread per row up to 4, one warp beyond), with and without the
+    obs_before shift; T = 1, episodes of one step, E > 128; bit for bit the host to_paths."""
+    pack = lib.madrl_paths_pack_u32 if itemsize == 4 else lib.madrl_paths_pack_u16
+    for k, D in enumerate(pe.PACK_WORDS):
+        for shifted in (False, True):
+            T, E, A, p_done = pe.PACK_SHAPES[(k + shifted) % len(pe.PACK_SHAPES)]
+            c = pe.pack_case(T, E, A, D, p_done, itemsize, 10 * D + shifted)
+            seg_s, seg_l = np.full((T, E), -1, np.int32), np.full((T, E), -1, np.int32)
+            n_ep, ep_rec = np.zeros(E, np.int32), np.zeros((E, T, 3), np.int32)
+            assert lib.madrl_paths_plan(T, E, A, _p(c["done"]), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
+            p_obs = Guarded((T * E * A, D), c["obs"].dtype, 0)
+            assert pack(T, E, A, D, _p(c["obs"]), _p(c["obs_before"] if shifted else None), _p(seg_s), _p(seg_l),
+                        _p(p_obs.arr), None) == 0
+            words = []
+            for x, n_agents in ((c["act"], A), (c["rew"], A), (c["info"], 1)):
+                out = Guarded((T * E * n_agents,), x.dtype, 0)
+                assert lib.madrl_paths_pack_u32(T, E, n_agents, 1, _p(x), None, _p(seg_s), _p(seg_l), _p(out.arr),
+                                                None) == 0
+                words.append(out.check("packed"))
+            pe.check_packed(c, shifted, pe.plan_paths(n_ep, ep_rec, T, A), p_obs.check("packed obs"), *words)

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 import torch
 
+import postproc_edges as pe
 from oracle import baseline_oracle as bo
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "linear_baseline_ref.npz")
@@ -162,6 +163,8 @@ EMU_SHAPES = [  # T, E, A, D, p_done, obs_before, t0
     (11, 2, 3, 5, 0.3, False, False),
     (6, 2, 3, 213, 0.2, True, True),
     (40, 3, 1, 1, 0.15, False, True),
+    (7, 3, 2, 30, 0.25, True, True),       # 65 columns: y alone in the second tile
+    (5, 2, 3, 31, 0.3, False, True),       # 67 columns: the time, constant and return columns cross the tile edge
 ]
 
 
@@ -201,6 +204,32 @@ def test_emulated_kernels_match_oracle(lib, shape):
         assert np.all(np.abs(vals.reshape(-1).astype(np.float64) - want) <= tol)
     for a, b in zip(results["bf16"], results["f32_widened"]):                 # bf16 == the call on obs.float()
         assert np.array_equal(a, b)
+    assert _races(lib) == 0
+
+
+@have_cxx
+@pytest.mark.parametrize("bf16", [False, True], ids=["f32", "bf16"])
+def test_emulated_single_row_reads_out_the_exact_features(lib, bf16):
+    """One row: G = outer(f, f) bit for bit, f = [clip(o), clip(o)^2, a, a^2, a^3, 1, y] with the correctly rounded
+    a^3 (not NumPy's al ** 3, which is an ulp off at some of these indices), at the obs_dims whose time columns sit
+    at a tile edge; predict with a unit coefficient on a time column returns that feature rounded to float32
+    (tests/test_postproc_edges_gpu.py sweeps more obs_dims and indices on the device)."""
+    rs = np.random.RandomState(3 + bf16)
+    done = np.zeros((1, 1), np.uint8)
+    _races(lib)
+    for D in (30, 31, 32):
+        for before in (False, True):
+            for k, t0 in enumerate((1, 99, 767, 50004)):
+                o = pe.single_row_obs(D, k, bf16, rs)
+                y = np.float32(rs.randn())
+                f = pe.single_row_features(o, y, t0)
+                row = (pe.bf16_bits(o)[0] if bf16 else o).reshape(1, 1, 1, D)
+                obs, ob = (np.full_like(row, 0x7FC0 if bf16 else np.nan), row.reshape(1, 1, D)) if before else (row, None)
+                for j in (2 * D, 2 * D + 1, 2 * D + 2):
+                    G, vals = _run(lib, obs, ob, done, np.array([[[y]]], np.float32), np.array([t0], np.int32),
+                                   np.eye(2 * D + 4)[j], bf16)
+                    assert np.array_equal(G, np.outer(f, f)), (D, before, t0)
+                    assert vals.item() == np.float32(f[j]), (D, before, t0, j)
     assert _races(lib) == 0
 
 

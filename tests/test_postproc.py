@@ -150,9 +150,14 @@ def test_cuda_batch_statistics_match_oracle():
     float32 inputs); tolerance 1e-5 relative to the value scale, results deterministic."""
     import torch
     from madrl_b200.postproc import center_advantages, explained_variance, moments
+    import postproc_edges as pe
     rs = np.random.RandomState(9)
-    for shape in ((1,), (3,), (50, 7, 3), (256, 4096, 5)):
-        adv = (rs.randn(*shape) * 3 + 1).astype(np.float32)
+    cases = [(shape, 1.0) for shape in ((1,), (3,), (50, 7, 3), (256, 4096, 5))]
+    # the block edge and the grid-stride edges of the moments launch, data offset by 1e4 so that a one-pass
+    # variance would miss the rtol 1e-10 below
+    cases += [((n,), 1e4) for n in pe.stride_sizes(pe.csrc_default("MADRL_MOM_BLOCKS", "postproc.cu"))]
+    for shape, offset in cases:
+        adv = (rs.randn(*shape) * 3 + offset).astype(np.float32)
         ret = rs.randn(*shape).astype(np.float32)
         a_t, r_t = torch.as_tensor(adv, device='cuda'), torch.as_tensor(ret, device='cuda')
         flat = adv.ravel().astype(np.float64)
