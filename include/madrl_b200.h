@@ -451,6 +451,28 @@ int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const 
 int madrl_paths_pack_u16(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
                          const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream);
 
+/* Padded paths: rllab's recurrent sample batch (rllab/rllab/sampler/base.py:105-161, tensor_utils.pad_tensor_n),
+ * every path zero-padded to Lmax steps.  rec int32 [P][4] = (env, agent, start step, length) of each path, in the
+ * output's path order (any order: one kernel serves every control mode); 0 <= env < E, 0 <= start,
+ * start + length <= T, 1 <= length <= Lmax, and 0 <= agent < A unless A = 1.
+ *   madrl_paths_pad_u32  src [T][E][A][D] of 4-byte words -> dst [P][Lmax][D]: row (p, i) is src row
+ *                        (start + i, env, agent) for i < length, zeros otherwise; every dst word is written
+ *                        exactly once (no separate clearing pass).  first != NULL: rows are shifted by one step
+ *                        as in madrl_paths_pack_u32.  A = 1: per-env tensors [T][E][D] (infos); the agent field is
+ *                        ignored, so every agent's path reads its env's row.
+ *   madrl_paths_pad_u16  the same for rows of D 2-byte elements (bfloat16 observations; D may be odd).
+ *   madrl_path_sums_f32  rew, ret float32 [T][E][A] -> per path: sums[p] = the float64 sum of its rewards in time
+ *                        order (Python's sum(path["rewards"])), first_ret[p] = ret at its first step (the path's
+ *                        returns[0]).  Same table conventions; A = 1 reads column 0 of [T][E][1].
+ * MADRL_EINVAL for T, E, A, D, P or Lmax < 1, more padded rows than one launch's grid covers (P * Lmax >= 2^34
+ * for D > 4 words) or a NULL required buffer. */
+int madrl_paths_pad_u32(int T, int E, int A, int D, int P, int Lmax, const void* src_dev, const void* first_dev,
+                        const int32_t* rec_dev, void* dst_dev, void* stream);
+int madrl_paths_pad_u16(int T, int E, int A, int D, int P, int Lmax, const void* src_dev, const void* first_dev,
+                        const int32_t* rec_dev, void* dst_dev, void* stream);
+int madrl_path_sums_f32(int T, int E, int A, int P, const float* rew_dev, const float* ret_dev,
+                        const int32_t* rec_dev, double* sums_dev, double* first_ret_dev, void* stream);
+
 /* rllab's LinearFeatureBaseline (rllab/rllab/baselines/linear_feature_baseline.py), decentralized mode: one
  * baseline over every (t, e, a) row of a rollout.  Row (t, e, a) uses the observation the action of step t was
  * taken in (obs_before != NULL: obs_before [E][A][D] for t = 0, obs[t-1] afterwards; NULL: obs[t]) and the time

@@ -175,6 +175,10 @@ def _declare(lib):
             getattr(lib, "madrl_lfb_predict_agents_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
         lib.madrl_moments_agents_f32.argtypes = [C.c_size_t, i32, vp, vp, vp, vp, vp]
         lib.madrl_center_advantages_agents_f32.argtypes = [C.c_size_t, i32, vp, i32, i32, vp, vp, vp]
+    if hasattr(lib, "madrl_paths_pad_u32"):    # padded paths of the recurrent sample batch (absent from older builds)
+        lib.madrl_paths_pad_u32.argtypes = [i32] * 6 + [vp] * 5
+        lib.madrl_paths_pad_u16.argtypes = lib.madrl_paths_pad_u32.argtypes
+        lib.madrl_path_sums_f32.argtypes = [i32] * 4 + [vp] * 6
 
 
 def lib():

@@ -407,6 +407,73 @@ __global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const W* __
   for (int d = 0; d < D; ++d) out[d] = in[d];
 }
 
+// ---- padded paths: rllab's recurrent sample batch (rllab/rllab/sampler/base.py:105-161) ----------
+// Every path of a record table rec [P][4] = (env, agent, start, length) becomes Lmax rows of dst [P][Lmax][D]: its
+// steps, then zeros (tensor_utils.pad_tensor_n).  Organised by DESTINATION row (p, i), so each output word is
+// written once -- the padding by the same store stream as the data, no clearing pass -- and each source row is read
+// once.  A = 1 (per-env tensors): the record's agent is ignored.  `first`: the one-step shift of paths_pack_kernel.
+template <typename W>
+__device__ __forceinline__ const W* pad_source(int E, int A, int D, const W* src, const W* first,
+                                               const int32_t* __restrict__ r, int i) {
+  const int e = __ldg(r), a = A == 1 ? 0 : __ldg(r + 1), t = __ldg(r + 2) + i;
+  const size_t row = ((size_t)t * E + e) * A + a;
+  return first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D) : src + row * D;
+}
+
+// One warp per padded row (rows wider than 4 words).
+template <typename W>
+__global__ void paths_pad_kernel(int E, int A, int D, size_t rows, int Lmax, const W* __restrict__ src,
+                                 const W* __restrict__ first, const int32_t* __restrict__ rec, W* __restrict__ dst) {
+  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // padded row (p, i)
+  const int lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  const size_t p = row / Lmax;
+  const int i = (int)(row - p * Lmax);
+  const int32_t* r = rec + 4 * p;
+  W* out = dst + row * D;
+  if (i < __ldg(r + 3)) {
+    const W* in = pad_source(E, A, D, src, first, r, i);
+    for (int d = lane; d < D; d += 32) __stcs(out + d, __ldcs(in + d));
+  } else {
+    for (int d = lane; d < D; d += 32) __stcs(out + d, (W)0);
+  }
+}
+
+// Narrow rows (rewards, returns, advantages, actions, infos: D <= 4 words): one THREAD per padded row.
+template <typename W>
+__global__ void paths_pad_narrow_kernel(int E, int A, int D, size_t rows, int Lmax, const W* __restrict__ src,
+                                        const W* __restrict__ first, const int32_t* __restrict__ rec,
+                                        W* __restrict__ dst) {
+  const size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (row >= rows) return;
+  const size_t p = row / Lmax;
+  const int i = (int)(row - p * Lmax);
+  const int32_t* r = rec + 4 * p;
+  W* out = dst + row * D;
+  if (i < __ldg(r + 3)) {
+    const W* in = pad_source(E, A, D, src, first, r, i);
+    for (int d = 0; d < D; ++d) out[d] = in[d];
+  } else {
+    for (int d = 0; d < D; ++d) out[d] = (W)0;
+  }
+}
+
+// Per path: the float64 sum of its rewards in time order (Python's sum() over the reference's float64 rewards) and
+// its first return, the two per-path inputs of process_samples' tabular statistics (base.py:144-147, :170-180).
+__global__ void path_sums_kernel(int E, int A, int P, const float* __restrict__ rew, const float* __restrict__ ret,
+                                 const int32_t* __restrict__ rec, double* __restrict__ sums,
+                                 double* __restrict__ first_ret) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= P) return;
+  const int32_t* r = rec + 4 * (size_t)p;
+  const int e = r[0], a = A == 1 ? 0 : r[1], s = r[2], L = r[3];
+  const size_t stride = (size_t)E * A, k0 = ((size_t)s * E + e) * A + a;
+  double acc = 0.0;
+  for (int i = 0; i < L; ++i) acc += (double)rew[k0 + (size_t)i * stride];
+  sums[p] = acc;
+  first_ret[p] = (double)ret[k0];
+}
+
 }  // namespace madrl
 
 using namespace madrl;
@@ -598,6 +665,46 @@ extern "C" int madrl_paths_pack_u16(int T, int E, int A, int D, const void* src_
                                     const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev,
                                     void* stream) {
   return paths_pack<uint16_t>(T, E, A, D, src_dev, first_dev, seg_start_dev, seg_len_dev, dst_dev, stream);
+}
+
+template <typename W>
+static int paths_pad(int T, int E, int A, int D, int P, int Lmax, const void* src_dev, const void* first_dev,
+                     const int32_t* rec_dev, void* dst_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && D >= 1 && P >= 1 && Lmax >= 1, "bad shape");
+  MADRL_REQUIRE(src_dev && rec_dev && dst_dev, "NULL pointer");
+  const size_t rows = (size_t)P * Lmax;
+  const size_t blocks = D <= 4 ? (rows + 255) / 256 : (rows * 32 + 255) / 256;
+  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many padded rows for one launch");
+  if (D <= 4)
+    MADRL_LAUNCH(paths_pad_narrow_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, E, A, D, rows, Lmax,
+                 (const W*)src_dev, (const W*)first_dev, rec_dev, (W*)dst_dev);
+  else
+    MADRL_LAUNCH(paths_pad_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, E, A, D, rows, Lmax,
+                 (const W*)src_dev, (const W*)first_dev, rec_dev, (W*)dst_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_paths_pad_u32(int T, int E, int A, int D, int P, int Lmax, const void* src_dev,
+                                   const void* first_dev, const int32_t* rec_dev, void* dst_dev, void* stream) {
+  return paths_pad<uint32_t>(T, E, A, D, P, Lmax, src_dev, first_dev, rec_dev, dst_dev, stream);
+}
+
+extern "C" int madrl_paths_pad_u16(int T, int E, int A, int D, int P, int Lmax, const void* src_dev,
+                                   const void* first_dev, const int32_t* rec_dev, void* dst_dev, void* stream) {
+  return paths_pad<uint16_t>(T, E, A, D, P, Lmax, src_dev, first_dev, rec_dev, dst_dev, stream);
+}
+
+extern "C" int madrl_path_sums_f32(int T, int E, int A, int P, const float* rew_dev, const float* ret_dev,
+                                   const int32_t* rec_dev, double* sums_dev, double* first_ret_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && P >= 1, "bad shape");
+  MADRL_REQUIRE(rew_dev && ret_dev && rec_dev && sums_dev && first_ret_dev, "NULL pointer");
+  MADRL_LAUNCH(path_sums_kernel, (unsigned)((P + 127) / 128), 128, 0, (cudaStream_t)stream, E, A, P, rew_dev, ret_dev,
+               rec_dev, sums_dev, first_ret_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
 }
 
 template <typename O>

@@ -15,6 +15,10 @@ right after ``env.step`` in its sampler loop, as streaming passes over ``[T, E, 
 * ``to_paths``       the per-agent ``paths`` dicts of ``dec_rollout``
                      (rllab/rllab/sampler/ma_sampler.py:52-100), built on the host from gathered
                      tensors for callers that still want rllab's list-of-paths format.
+* ``pad_paths`` / ``path_statistics`` / ``process_samples_recurrent``  the recurrent branch of
+                     ``process_samples`` (base.py:105-161; per agent, batch_ma_sampler.py:124-181): paths
+                     zero-padded to the longest one with a ``valids`` mask, and the sampler's return statistics
+                     (base.py:170-180).
 """
 import ctypes as C
 
@@ -618,3 +622,256 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
     return PackedPaths(observations=packed_obs, actions=packed_act, rewards=packed_rew, env_infos=packed_info,
                        offset=offset, length=rep(Ln), env=rep(e_idx), agent=a_idx.repeat(rec.shape[0]),
                        terminated=rep(term).bool(), info_offset=rep(e_idx * T + s))
+
+
+# ---------------------------------------------------------------- the recurrent branch of process_samples
+# rllab pads every path of a batch to the longest one for a recurrent policy (base.py:105-161,
+# tensor_utils.pad_tensor_n) and marks the real steps with ``valids``.  Here the padded tensors are written
+# straight from the rollout by madrl_paths_pad_* (one pass, each output word written once, the padding included),
+# from a per-path record table built on the device.
+
+MODES = ("decentralized", "concurrent", "centralized")
+
+
+def _check_mode(mode):
+    if mode not in MODES:
+        raise ValueError("mode must be one of %s, got %r" % (", ".join(MODES), mode))
+
+
+class _PathTable(object):
+    """The paths of one rollout (episodes cut at ``done`` and at the end of the rollout, as ``pack_paths`` cuts
+    them) as the record table of madrl_paths_pad_*: int32 [P, 4] = (env, agent, start step, length).  Order
+    (env, episode, agent), or agent-major (agent, env, episode) for concurrent control.  P and the longest length
+    L come from one 16-byte device->host read."""
+
+    def __init__(self, done, A, agent_major):
+        T, E = done.shape
+        dev = done.device
+        lib = _lib.lib()
+        seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
+        seg_l = torch.empty((T, E), dtype=torch.int32, device=dev)
+        n_ep = torch.empty((E,), dtype=torch.int32, device=dev)
+        ep_rec = torch.zeros((E, T, 3), dtype=torch.int32, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.madrl_paths_plan(T, E, A, _ptr(done.contiguous()), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep),
+                                            _ptr(ep_rec), _lib.stream(dev)))
+        n, L = (int(v) for v in torch.stack([n_ep.sum(), ep_rec[:, :, 1].max().long()]).cpu())
+        live = torch.arange(T, device=dev).unsqueeze(0) < n_ep.unsqueeze(1)
+        slot = torch.nonzero_static(live, size=n)                 # (env, episode) of every episode, in that order
+        ep = ep_rec[slot[:, 0], slot[:, 1]]
+        agents, eps = torch.arange(A, device=dev), torch.arange(n, device=dev)
+        if agent_major:
+            a, j = agents.repeat_interleave(n), eps.repeat(A)
+        else:
+            a, j = agents.repeat(n), eps.repeat_interleave(A)
+        self.rec = torch.stack([slot[j, 0], a, ep[j, 0].long(), ep[j, 1].long()], dim=1).to(torch.int32).contiguous()
+        self.terminated = ep[j, 2].bool()
+        self.T, self.E, self.A, self.P, self.L = T, E, A, n * A, L
+        self.lead = (A, n) if agent_major else (n * A,)
+
+    def pad(self, x, per_agent=True, first=None):
+        """x [T,E,A,...] (per agent) or [T,E,...] (per env) -> [*lead, L, ...], zero past each path's end."""
+        x = x.contiguous()
+        tail = tuple(x.shape[3:] if per_agent else x.shape[2:])
+        D = max(1, int(np.prod(tail)))
+        out = torch.empty((self.P, self.L) + tail, dtype=x.dtype, device=x.device)
+        lib = _lib.lib()
+        fn = lib.madrl_paths_pad_u16 if x.element_size() == 2 else lib.madrl_paths_pad_u32
+        with torch.cuda.device(x.device):
+            _lib.check(fn(self.T, self.E, self.A if per_agent else 1, D, self.P, self.L, _ptr(x),
+                          _ptr(None if first is None else first.contiguous()), _ptr(self.rec), _ptr(out),
+                          _lib.stream(x.device)))
+        return out.view(self.lead + (self.L,) + tail)
+
+    def valids(self):
+        """float32 [*lead, L]: 1 on a path's steps, 0 on its padding."""
+        L = self.L
+        v = torch.arange(L, device=self.rec.device).unsqueeze(0) < self.rec[:, 3:4]
+        return v.to(torch.float32).view(self.lead + (L,))
+
+    def sums(self, rew, ret):
+        """float64 [*lead] per path: the sum of its rewards in time order and its first return."""
+        rew, ret = rew.contiguous(), ret.contiguous()
+        s = torch.empty(self.P, dtype=torch.float64, device=rew.device)
+        f = torch.empty(self.P, dtype=torch.float64, device=rew.device)
+        with torch.cuda.device(rew.device):
+            _lib.check(_lib.lib().madrl_path_sums_f32(self.T, self.E, self.A, self.P, _ptr(rew), _ptr(ret),
+                                                      _ptr(self.rec), _ptr(s), _ptr(f), _lib.stream(rew.device)))
+        return s.view(self.lead), f.view(self.lead)
+
+    def records(self):
+        """The per-path fields of `PaddedPaths`."""
+        r = self.rec.long()
+        return {k: r[:, c].view(self.lead) for c, k in enumerate(("env", "agent", "start", "length"))} | \
+            dict(terminated=self.terminated.view(self.lead))
+
+
+class PaddedPaths(object):
+    """rllab's recurrent sample batch of one rollout, resident on the device (see `pad_paths`).
+
+    ``observations [P, L, D]``, ``actions [P, L, ...]``, ``rewards [P, L]``, ``valids [P, L]`` float32 (1 on a
+    path's steps, 0 on its padding), ``env_infos[k] [P, L, ...]``, ``agent_infos[k] [P, L, ...]``, and per path
+    ``env``, ``agent``, ``start``, ``length`` (int64) and ``terminated`` (bool) [P].  Concurrent control: every
+    field has a leading agent axis, [A, P_a, L, ...] and [A, P_a]."""
+
+    def __init__(self, **kw):
+        self.__dict__.update(kw)
+
+
+def _recurrent_inputs(mode, obs, actions, rew, done, infos, obs_before, agent_infos, obs_dtypes, rew_dtypes,
+                      t0=None):
+    """Checks the rollout tensors of the recurrent branch (every one before any pointer reaches the library) and
+    returns them in the mode's layout: centralized control is the view of one agent whose observation, action and
+    agent_infos rows are the agents' side by side, with agent 0's reward (all agents' are equal there,
+    ma_sampler.py:27-29)."""
+    _check_mode(mode)
+    T, E, A = _lib.require_tensor(obs, "obs", obs_dtypes, (None, None, None, ...), None, contiguous=False).shape[:3]
+    dev = obs.device
+    _lib.require_tensor(actions, "actions", _PACKED_DTYPES, (T, E, A, ...), dev, contiguous=False)
+    _lib.require_tensor(rew, "rew", rew_dtypes, (T, E, A), dev, contiguous=False)
+    _lib.require_tensor(done, "done", torch.uint8, (T, E), dev, contiguous=False)
+    _lib.require_tensor(obs_before, "obs_before", obs.dtype, tuple(obs.shape[1:]), dev, contiguous=False,
+                        optional=True)
+    _lib.require_tensor(t0, "t0", torch.int32, (E,), dev, contiguous=False, optional=True)
+    infos, agent_infos = dict(infos or {}), dict(agent_infos or {})
+    for k, v in infos.items():
+        _lib.require_tensor(v, "infos[%r]" % (k,), _PACKED_DTYPES, (T, E, ...), dev, contiguous=False)
+    for k, v in agent_infos.items():
+        _lib.require_tensor(v, "agent_infos[%r]" % (k,), _PACKED_DTYPES, (T, E, A, ...), dev, contiguous=False)
+    if mode == "centralized" and not torch.equal(rew, rew[..., :1].expand_as(rew)):
+        raise ValueError("centralized control needs the agents' rewards equal at every step (one reward per env)")
+    _lib.require_tensor(obs, "obs", obs.dtype, (T, E, A, ...), "cuda", contiguous=False)
+    if T * E * A >= 2 ** 31:
+        raise ValueError("T*E*A must be < 2^31, got %d" % (T * E * A))
+    if mode == "centralized":
+        side = lambda x: x.contiguous().view(T, E, 1, -1)             # noqa: E731
+        obs, actions, rew = side(obs), side(actions), rew[..., :1]
+        obs_before = None if obs_before is None else obs_before.contiguous().view(E, 1, -1)
+        agent_infos = {k: side(v) for k, v in agent_infos.items()}
+    return obs, actions, rew, done.contiguous(), infos, obs_before, agent_infos
+
+
+def _pad_all(table, obs, actions, rew, infos, obs_before, agent_infos):
+    return dict(observations=table.pad(obs, first=obs_before), actions=table.pad(actions),
+                rewards=table.pad(rew), valids=table.valids(),
+                env_infos={k: table.pad(v, per_agent=False) for k, v in infos.items()},
+                agent_infos={k: table.pad(v) for k, v in agent_infos.items()})
+
+
+def pad_paths(obs, actions, rew, done, infos=None, obs_before=None, agent_infos=None, mode="decentralized"):
+    """Rollout tensors [T,E,A,...] (CUDA) -> `PaddedPaths`: rllab's recurrent batch layout (base.py:105-161), every
+    path zero-padded to L = the longest path.
+
+    Paths are cut at ``done`` and at the end of the rollout.  ``obs_before`` [E,A,...]: as in `pack_paths`, row i
+    of a path is then the observation its action was taken in.  ``infos`` {k: [T,E,...]} are per env: each agent's
+    path holds a copy of its env's rows, as ``dec_rollout`` gives it (ma_sampler.py:79-81).  ``agent_infos``
+    {k: [T,E,A,...]}: the policy's per-agent outputs (means, log-stds), padded the same way.  Path order per
+    ``mode``:
+
+    * ``"decentralized"``  (env, episode, agent), the order of `to_paths` / `pack_paths`;
+    * ``"concurrent"``     agent a's paths in (env, episode) order, under a leading agent axis [A, P_a, L, ...]
+                           (all agents share the episode cuts, hence P_a and L);
+    * ``"centralized"``    one path per episode of the view obs [T,E,1,A*D], actions [T,E,1,A*k] (agent_infos
+                           likewise) and reward ``rew[..., 0]``; ValueError unless all agents' rewards are equal.
+
+    Tensors of 4-byte elements, and bfloat16 (2-byte) ones.  One plan launch, one 16-byte device->host read
+    (P and L), one padding launch per tensor."""
+    obs, actions, rew, done, infos, obs_before, agent_infos = _recurrent_inputs(
+        mode, obs, actions, rew, done, infos, obs_before, agent_infos, _PACKED_DTYPES, _PACKED_DTYPES)
+    table = _PathTable(done, obs.shape[2], mode == "concurrent")
+    return PaddedPaths(mode=mode, **_pad_all(table, obs, actions, rew, infos, obs_before, agent_infos),
+                       **table.records())
+
+
+_STAT_KEYS = ("AverageDiscountedReturn", "AverageReturn", "StdReturn", "MaxReturn", "MinReturn")
+
+
+def _statistics(sums, first_ret):
+    """base.py:144-147 and :170-180 over the paths of the last axis: one dict, or a list of one per row."""
+    vals = torch.stack([first_ret.mean(-1), sums.mean(-1), sums.std(-1, correction=0), sums.max(-1).values,
+                        sums.min(-1).values], dim=-1).cpu().numpy()
+    out = [dict(zip(_STAT_KEYS, map(float, row)), NumTrajs=int(sums.shape[-1])) for row in vals.reshape(-1, 5)]
+    return out if sums.dim() == 2 else out[0]
+
+
+def path_returns(rew, ret, done, per_agent=False):
+    """Per path (episodes cut at ``done``): the undiscounted return ``sum(path["rewards"])`` (float64, in time
+    order) and the first return ``path["returns"][0]`` -- float64 tensors [P] in (env, episode, agent) order, or
+    [A, P_a] with ``per_agent=True`` (agent a's paths in (env, episode) order).  rew, ret [T,E,A] float32
+    (``ret``: `gae`'s second output); centralized control passes ``rew[..., :1]`` and its returns."""
+    T, E, A = _lib.require_tensor(rew, "rew", torch.float32, (None, None, None), None, contiguous=False).shape
+    _lib.require_tensor(ret, "ret", torch.float32, (T, E, A), rew.device, contiguous=False)
+    _lib.require_tensor(done, "done", torch.uint8, (T, E), rew.device, contiguous=False)
+    _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), "cuda", contiguous=False)
+    if T * E * A >= 2 ** 31:
+        raise ValueError("T*E*A must be < 2^31, got %d" % (T * E * A))
+    return _PathTable(done, A, per_agent).sums(rew, ret)
+
+
+def path_statistics(rew, ret, done, per_agent=False):
+    """The return statistics both branches of ``process_samples`` log (base.py:144-147, :170-180):
+    ``AverageDiscountedReturn`` (mean of the paths' first returns), ``AverageReturn``, ``StdReturn`` (population),
+    ``MaxReturn``, ``MinReturn`` (over the paths' undiscounted returns) and ``NumTrajs``, as Python numbers in a
+    dict; ``per_agent=True`` (concurrent control): a list of A dicts, agent a's over its own paths.  Arguments as
+    `path_returns`.  Unlike `EpisodeStats` every path counts, including the unfinished one at the end of the
+    rollout, and nothing is averaged over agents."""
+    return _statistics(*path_returns(rew, ret, done, per_agent))
+
+
+def process_samples_recurrent(baseline, obs, actions, rew, done, discount, gae_lambda, mode, obs_before=None,
+                              t0=None, infos=None, agent_infos=None, center_adv=True, group=None):
+    """The recurrent branch of rllab's ``process_samples`` over one rollout (base.py:48-68, :105-180;
+    concurrent control: once per agent, batch_ma_sampler.py:124-188), in the reference's order: baseline
+    predictions, GAE advantages and discounted returns per path (`gae`), the explained variance, advantage
+    centring, padding (`pad_paths`), the baseline fit.
+
+    ``baseline``: a `LinearFeatureBaseline` -- pooled with ``obs_dim = D`` (decentralized), with ``n_agents = A``
+    (concurrent; ``shared=True`` is fitted first, as in `process_samples_concurrent`), pooled with
+    ``obs_dim = A*D`` (centralized).  obs [T,E,A,D] float32 or bfloat16, actions [T,E,A,...], rew [T,E,A] float32,
+    done [T,E] uint8; ``obs_before``, ``t0`` as for the baseline, ``infos``, ``agent_infos`` as for `pad_paths`.
+    ``group``: a ``torch.distributed`` group the baseline's normal equations are summed over; the statistics stay
+    per rank.
+
+    Two quirks of the reference are kept: the branch has no ``positive_adv`` (rllab ignores the flag there), and
+    centring always divides by ``std + 1e-8``.  Centring is over every sample (per agent for concurrent control)
+    and comes before the padding, so padded advantages are 0.
+
+    Returns a dict: the ``samples_data`` keys of base.py:151-161 (``observations``, ``actions``, ``advantages``,
+    ``rewards``, ``returns``, ``valids``, ``agent_infos``, ``env_infos``) padded as `pad_paths` pads them, ``paths``
+    = the `PaddedPaths` of the batch (the same tensors and the per-path records), ``values`` [T,E,A] (the
+    predictions), ``ExplainedVariance`` and the `path_statistics` keys.  Concurrent control: leading agent axes
+    and one statistic per agent (lists of A).  The entropy term needs the policy's distribution: it stays the
+    caller's, from the padded ``agent_infos`` and ``valids``."""
+    _check_mode(mode)
+    if not isinstance(baseline, LinearFeatureBaseline):
+        raise ValueError("process_samples_recurrent needs a LinearFeatureBaseline")
+    _lib.require_tensor(obs, "obs", _OBS_DTYPES, (None, None, None, None), None, contiguous=False)
+    concurrent = mode == "concurrent"
+    if concurrent != (baseline.n_agents is not None):
+        raise ValueError("mode %r needs a LinearFeatureBaseline %s n_agents" % (mode, "with" if concurrent else
+                                                                                 "without"))
+    obs, actions, rew, done, infos, obs_before, agent_infos = _recurrent_inputs(
+        mode, obs, actions, rew, done, infos, obs_before, agent_infos, _OBS_DTYPES, (torch.float32,), t0)
+    if baseline.shared:
+        _, ret = gae(rew, torch.zeros_like(rew), done, discount, gae_lambda)
+        baseline.fit(obs, done, ret, obs_before, t0, group)
+        values = baseline.predict(obs, done, obs_before, t0)
+        adv, _ = gae(rew, values, done, discount, gae_lambda)
+    else:
+        values = baseline.predict(obs, done, obs_before, t0)
+        adv, ret = gae(rew, values, done, discount, gae_lambda)
+    ev = explained_variance(values, ret, per_agent=concurrent)
+    if center_adv:
+        adv = center_advantages(adv, True, False, inplace=True, per_agent=concurrent)
+    table = _PathTable(done, obs.shape[2], concurrent)
+    data = _pad_all(table, obs, actions, rew, infos, obs_before, agent_infos)
+    data.update(advantages=table.pad(adv), returns=table.pad(ret))
+    stats = _statistics(*table.sums(rew, ret))
+    if not baseline.shared:
+        baseline.fit(obs, done, ret, obs_before, t0, group)
+    out = dict(data, paths=PaddedPaths(mode=mode, **data, **table.records()), values=values, ExplainedVariance=ev)
+    if concurrent:
+        out.update({k: [s[k] for s in stats] for k in _STAT_KEYS + ("NumTrajs",)})
+    else:
+        out.update(stats)
+    return out
