@@ -45,16 +45,20 @@ static inline int lfb_cols(int D) { return 2 * D + 5; }
 static inline int lfb_tiles(int D) { return (lfb_cols(D) + kLfbTile - 1) / kLfbTile; }
 __host__ __device__ __forceinline__ int lfb_agent_slices(int A) { return (kLfbSlices + A - 1) / A; }
 
+// Time index of the rows (t, e, .) with te = t E + e: the position in the path, plus t0[e] on env e's first path.
+template <typename I>
+__device__ __forceinline__ int lfb_index(I te, int E, const int32_t* seg_start, const int32_t* t0) {
+  const I t = te / (I)E, e = te - t * (I)E;
+  const int s = seg_start[te];
+  return (int)t - s + ((t0 != nullptr && s == 0) ? t0[e] : 0);
+}
+
 // Source row and time index of row r.
 template <typename O>
 __device__ __forceinline__ const O* lfb_row(size_t r, int E, int A, int D, const O* obs, const O* obs_before,
                                             const int32_t* seg_start, const int32_t* t0, int& idx) {
-  const size_t te = r / A;
-  const int a = (int)(r - te * A), e = (int)(te % E), t = (int)(te / E);
-  const int s = seg_start[te];
-  idx = t - s + ((t0 != nullptr && s == 0) ? t0[e] : 0);
-  if (!obs_before) return obs + r * D;
-  return t == 0 ? obs_before + ((size_t)e * A + a) * D : obs + (r - (size_t)E * A) * D;
+  idx = lfb_index(r / A, E, seg_start, t0);
+  return action_obs_row(r, (size_t)E * A, D, obs, obs_before);
 }
 
 // a = i / 100 (correctly rounded, as NumPy's arange(l) / 100.0), a^2 = a * a, a^3 = (a^2 + its rounding error) * a
@@ -89,17 +93,11 @@ __device__ __forceinline__ uint32_t lfb_fetch(int kind, int d, uint32_t r, bool 
                                               const O* obs, const O* obs_before, const int32_t* seg_start,
                                               const int32_t* t0, const float* ret) {
   if (!valid || kind == kLfbPad) return 0u;
-  const uint32_t EA = (uint32_t)E * A;
-  if (kind <= kLfbObsSq) {          // row r's source row, no division: t == 0 <=> r < E*A
-    const O* src = obs_before ? (r < EA ? obs_before + (size_t)r * D : obs + (size_t)(r - EA) * D)
-                              : obs + (size_t)r * D;
-    return __float_as_uint(obs_widen<float>(src[d]));
-  }
+  if (kind <= kLfbObsSq)            // row r's source row, no division
+    return __float_as_uint(obs_widen<float>(action_obs_row(r, (uint32_t)E * A, D, obs, obs_before)[d]));
   if (kind == kLfbY) return __float_as_uint(ret[r]);
   if (kind == kLfbOne) return 1u;
-  const uint32_t te = r / (uint32_t)A, t = te / (uint32_t)E, e = te - t * E;
-  const int s = seg_start[te];
-  return (uint32_t)((int)t - s + ((t0 != nullptr && s == 0) ? t0[e] : 0));
+  return (uint32_t)lfb_index(r / (uint32_t)A, E, seg_start, t0);
 }
 
 __device__ __forceinline__ double lfb_value(int kind, uint32_t v) {
@@ -186,9 +184,8 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
       if (obs_only[b]) {
 #pragma unroll
         for (int i = 0; i < kLfbRows / 2; ++i) {
-          const uint32_t k = r0 + k0 + 2 * i, r = row_of(k);
-          const O* src = obs_before ? (r < EA ? obs_before + (size_t)r * D : obs + (size_t)(r - EA) * D)
-                                    : obs + (size_t)r * D;
+          const uint32_t k = r0 + k0 + 2 * i;
+          const O* src = action_obs_row(row_of(k), EA, D, obs, obs_before);
           nxt[b][i] = k < r_end ? __float_as_uint(obs_widen<float>(src[d[b]])) : 0u;
         }
       } else {

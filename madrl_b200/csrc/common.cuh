@@ -261,6 +261,16 @@ template <typename O> __device__ __forceinline__ O lds_obs(uint32_t a) {
 template <typename O, typename real>
 __device__ __forceinline__ void stage_obs(uint32_t a, real v) { sts_obs(a, obs_cvt<O>(v)); }
 
+// The row of observations action r was taken in, for rollout row r = (t E + e) A + a of src [T][E][A][D], which holds
+// the observation AFTER each step.  With `first` (the observations before the rollout, [E][A][D]) that is first[e][a]
+// for t = 0 and src[t-1] afterwards (on a done step src already holds the reset observation, i.e. the next
+// episode's first one); without it, src[t] as given.  t == 0 <=> r < E A, and then r = e A + a.  I: the index type
+// of the caller's row arithmetic.
+template <typename I, typename O>
+__device__ __forceinline__ const O* action_obs_row(I r, I EA, int D, const O* src, const O* first) {
+  return first ? (r < EA ? first + (size_t)r * D : src + (size_t)(r - EA) * D) : src + (size_t)r * D;
+}
+
 // StandardizedEnv sees the TERMINAL observation of an episode before the reset one
 // (madrl_environments/__init__.py:283-291 step(), then reset()); under auto-reset the rollout's obs slot is
 // overwritten by the reset observation, so -- when the caller asked for it -- the rows of a finished env

@@ -194,8 +194,8 @@ __global__ void episode_stats_kernel(int T, int E, int A, const float* __restric
 // order by one warp (no atomics), so a given input always yields the same bits.
 //
 // Three series are derived per element from (a, b):  s0 = a,  s1 = b,  s2 = b - a  (b optional).
-// The *_agents passes take the same statistics per column of a [rows][A] tensor (one agent's samples,
-// concurrent mode), one group of kMomBlocks CTAs per column.
+// The statistics are taken per column of a [rows][A] tensor (one agent's samples, concurrent mode), one group of
+// kMomBlocks CTAs per column; the whole-batch passes are the one-column case.
 #ifndef MADRL_MOM_BLOCKS
 #define MADRL_MOM_BLOCKS 528           // 4 CTAs x 132 SMs (H100 SXM) (the CPU emulator of tests/emu builds with fewer)
 #endif
@@ -216,23 +216,17 @@ __device__ __forceinline__ double warp_min(double v) {
 }
 
 // pass 0 (means == nullptr): partial sums and minima; pass 1: partial sums of squared deviations.
-// part [kMomBlocks][2*kMomSeries].  kAgents: a, b are [n][A] and CTA blockIdx.x covers column
-// blockIdx.x / kMomBlocks (an agent) as block blockIdx.x % kMomBlocks of a whole-batch pass over that column;
-// means and part then point at that column's [MADRL_MOMENTS_STATS] and [MADRL_MOMENTS_WS] blocks.
-template <bool kAgents>
+// a, b are [n][A]; CTA blockIdx.x covers column blockIdx.x / kMomBlocks (an agent) as block blockIdx.x % kMomBlocks of
+// a whole-batch pass over that column, whose means and part [kMomBlocks][2*kMomSeries] are that column's
+// [MADRL_MOMENTS_STATS] and [MADRL_MOMENTS_WS] blocks.  The whole batch is the one-column case.
 __global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, int A, const float* __restrict__ a,
                                                                       const float* __restrict__ b,
                                                                       const double* __restrict__ means,
                                                                       double* __restrict__ part) {
-  const int col = kAgents ? (int)(blockIdx.x / kMomBlocks) : 0;
-  const unsigned blk = kAgents ? blockIdx.x - col * kMomBlocks : blockIdx.x;
-  if (kAgents) {
-    a += col;
-    if (b) b += col;
-    if (means) means += (size_t)col * MADRL_MOMENTS_STATS;
-    part += (size_t)col * MADRL_MOMENTS_WS;
-  }
-  const size_t lda = kAgents ? (size_t)A : 1;
+  const int col = (int)(blockIdx.x / kMomBlocks);
+  const unsigned blk = blockIdx.x - col * kMomBlocks;
+  if (means) means += (size_t)col * MADRL_MOMENTS_STATS;
+  part += (size_t)col * MADRL_MOMENTS_WS;
   double acc[kMomSeries] = {0.0, 0.0, 0.0};
   double mn[kMomSeries] = {INFINITY, INFINITY, INFINITY};
   double mu[kMomSeries] = {0.0, 0.0, 0.0};
@@ -240,10 +234,12 @@ __global__ void __launch_bounds__(kMomThreads) moments_partial_kernel(size_t n, 
 #pragma unroll
     for (int s = 0; s < kMomSeries; ++s) mu[s] = means[s];
   }
-  const size_t stride = (size_t)kMomBlocks * blockDim.x;
-  for (size_t i = (size_t)blk * blockDim.x + threadIdx.x; i < n; i += stride) {
-    const double va = (double)__ldcs(a + i * lda);
-    const double vb = b ? (double)__ldcs(b + i * lda) : 0.0;
+  // element i of the column sits at k = i A + col; the loop runs over k, so that no 64-bit multiply or second
+  // induction variable sits on the path to each load
+  const size_t end = n * A, step = (size_t)kMomBlocks * blockDim.x * A;
+  for (size_t k = ((size_t)blk * blockDim.x + threadIdx.x) * A + col; k < end; k += step) {
+    const double va = (double)__ldcs(a + k);
+    const double vb = b ? (double)__ldcs(b + k) : 0.0;
     const double v[kMomSeries] = {va, vb, vb - va};
 #pragma unroll
     for (int s = 0; s < kMomSeries; ++s) {
@@ -367,44 +363,41 @@ __global__ void paths_plan_kernel(int T, int E, int A, const uint8_t* __restrict
   n_episodes[e] = n;
 }
 
+// The D words of one row, moved by kLanes threads: a warp (32, lanes stride over the words: coalesced, streaming
+// accesses) or one thread (1: rows of at most 4 words -- rewards, returns, advantages, actions, infos -- with plain
+// accesses: pad_paths at the C2 shape ran about 3 % faster with them than with streaming ones on an H100 80GB HBM3 at
+// 700 W).  in == NULL writes zeros.
+template <int kLanes, typename W>
+__device__ __forceinline__ void copy_row(W* __restrict__ out, const W* __restrict__ in, int D) {
+  if (kLanes == 1) {
+    if (in)
+      for (int d = 0; d < D; ++d) out[d] = in[d];
+    else
+      for (int d = 0; d < D; ++d) out[d] = (W)0;
+    return;
+  }
+  const int lane = threadIdx.x % kLanes;
+  if (in)
+    for (int d = lane; d < D; d += kLanes) __stcs(out + d, __ldcs(in + d));
+  else
+    for (int d = lane; d < D; d += kLanes) __stcs(out + d, (W)0);
+}
+
 // W = the row element: uint32_t (4-byte words) or uint16_t (bfloat16 observations; rows of odd length).
-template <typename W>
+// `first` != NULL: observations are shifted by one step (action_obs_row).
+template <int kLanes, typename W>
 __global__ void paths_pack_kernel(int T, int E, int A, int D, const W* __restrict__ src,
                                   const W* __restrict__ first, const int32_t* __restrict__ seg_start,
                                   const int32_t* __restrict__ seg_len, W* __restrict__ dst) {
-  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // source row (t, e, a)
-  const int lane = threadIdx.x & 31;
+  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;   // source row (t, e, a)
   const size_t rows = (size_t)T * E * A;
   if (row >= rows) return;
   const int a = (int)(row % A);
   const size_t te = row / A;
   const int e = (int)(te % E), t = (int)(te / E);
   const int s = seg_start[te], L = seg_len[te];
-  // `first` != NULL: observations are shifted by one step -- the row of time t is the observation the
-  // action of time t was taken in: first[e][a] for t = 0, src[t-1] afterwards (on a done step the
-  // rollout's obs slot already holds the reset observation, i.e. the next episode's first one)
-  const W* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
-                      : src + row * D;
   W* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
-  for (int d = lane; d < D; d += 32) __stcs(out + d, __ldcs(in + d));
-}
-
-// Narrow rows (rewards, actions, infos: D <= 4 words): one THREAD per source row instead of one warp.
-template <typename W>
-__global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const W* __restrict__ src,
-                                         const W* __restrict__ first, const int32_t* __restrict__ seg_start,
-                                         const int32_t* __restrict__ seg_len, W* __restrict__ dst) {
-  const size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x;   // source row (t, e, a)
-  const size_t rows = (size_t)T * E * A;
-  if (row >= rows) return;
-  const int a = (int)(row % A);
-  const size_t te = row / A;
-  const int e = (int)(te % E), t = (int)(te / E);
-  const int s = seg_start[te], L = seg_len[te];
-  const W* in = first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D)
-                      : src + row * D;
-  W* out = dst + ((size_t)e * T * A + (size_t)s * A + (size_t)a * L + (t - s)) * D;
-  for (int d = 0; d < D; ++d) out[d] = in[d];
+  copy_row<kLanes>(out, action_obs_row(row, (size_t)E * A, D, src, first), D);
 }
 
 // ---- padded paths: rllab's recurrent sample batch (rllab/rllab/sampler/base.py:105-161) ----------
@@ -412,50 +405,20 @@ __global__ void paths_pack_narrow_kernel(int T, int E, int A, int D, const W* __
 // steps, then zeros (tensor_utils.pad_tensor_n).  Organised by DESTINATION row (p, i), so each output word is
 // written once -- the padding by the same store stream as the data, no clearing pass -- and each source row is read
 // once.  A = 1 (per-env tensors): the record's agent is ignored.  `first`: the one-step shift of paths_pack_kernel.
-template <typename W>
-__device__ __forceinline__ const W* pad_source(int E, int A, int D, const W* src, const W* first,
-                                               const int32_t* __restrict__ r, int i) {
-  const int e = __ldg(r), a = A == 1 ? 0 : __ldg(r + 1), t = __ldg(r + 2) + i;
-  const size_t row = ((size_t)t * E + e) * A + a;
-  return first ? (t == 0 ? first + ((size_t)e * A + a) * D : src + (row - (size_t)E * A) * D) : src + row * D;
-}
-
-// One warp per padded row (rows wider than 4 words).
-template <typename W>
+template <int kLanes, typename W>
 __global__ void paths_pad_kernel(int E, int A, int D, size_t rows, int Lmax, const W* __restrict__ src,
                                  const W* __restrict__ first, const int32_t* __restrict__ rec, W* __restrict__ dst) {
-  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;   // padded row (p, i)
-  const int lane = threadIdx.x & 31;
+  const size_t row = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;   // padded row (p, i)
   if (row >= rows) return;
   const size_t p = row / Lmax;
   const int i = (int)(row - p * Lmax);
   const int32_t* r = rec + 4 * p;
-  W* out = dst + row * D;
+  const W* in = nullptr;
   if (i < __ldg(r + 3)) {
-    const W* in = pad_source(E, A, D, src, first, r, i);
-    for (int d = lane; d < D; d += 32) __stcs(out + d, __ldcs(in + d));
-  } else {
-    for (int d = lane; d < D; d += 32) __stcs(out + d, (W)0);
+    const int e = __ldg(r), a = A == 1 ? 0 : __ldg(r + 1), t = __ldg(r + 2) + i;
+    in = action_obs_row(((size_t)t * E + e) * A + a, (size_t)E * A, D, src, first);
   }
-}
-
-// Narrow rows (rewards, returns, advantages, actions, infos: D <= 4 words): one THREAD per padded row.
-template <typename W>
-__global__ void paths_pad_narrow_kernel(int E, int A, int D, size_t rows, int Lmax, const W* __restrict__ src,
-                                        const W* __restrict__ first, const int32_t* __restrict__ rec,
-                                        W* __restrict__ dst) {
-  const size_t row = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (row >= rows) return;
-  const size_t p = row / Lmax;
-  const int i = (int)(row - p * Lmax);
-  const int32_t* r = rec + 4 * p;
-  W* out = dst + row * D;
-  if (i < __ldg(r + 3)) {
-    const W* in = pad_source(E, A, D, src, first, r, i);
-    for (int d = 0; d < D; ++d) out[d] = in[d];
-  } else {
-    for (int d = 0; d < D; ++d) out[d] = (W)0;
-  }
+  copy_row<kLanes>(dst + row * D, in, D);
 }
 
 // Per path: the float64 sum of its rewards in time order (Python's sum() over the reference's float64 rewards) and
@@ -558,20 +521,13 @@ extern "C" int madrl_standardize_bf16(int T, size_t n, void* x_dev, double* mean
   return standardize(T, n, (uint16_t*)x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable, stream);
 }
 
-// A == 0: the whole batch of n elements; A >= 1: the A columns of [n][A].
+// The A columns of [n][A]; the whole batch of n elements is A = 1.
 static int run_moments(size_t n, int A, const float* a, const float* b, double* stats, double* ws, cudaStream_t s) {
-  if (A == 0) {
-    MADRL_LAUNCH(moments_partial_kernel<false>, kMomBlocks, kMomThreads, 0, s, n, 1, a, b, nullptr, ws);
-    MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 0, stats);
-    MADRL_LAUNCH(moments_partial_kernel<false>, kMomBlocks, kMomThreads, 0, s, n, 1, a, b, stats, ws);
-    MADRL_LAUNCH(moments_finalize_kernel, 1, 32, 0, s, n, ws, 1, stats);
-  } else {
-    const unsigned grid = (unsigned)(kMomBlocks * A);
-    MADRL_LAUNCH(moments_partial_kernel<true>, grid, kMomThreads, 0, s, n, A, a, b, nullptr, ws);
-    MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 0, stats);
-    MADRL_LAUNCH(moments_partial_kernel<true>, grid, kMomThreads, 0, s, n, A, a, b, stats, ws);
-    MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 1, stats);
-  }
+  const unsigned grid = (unsigned)(kMomBlocks * A);
+  MADRL_LAUNCH(moments_partial_kernel, grid, kMomThreads, 0, s, n, A, a, b, nullptr, ws);
+  MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 0, stats);
+  MADRL_LAUNCH(moments_partial_kernel, grid, kMomThreads, 0, s, n, A, a, b, stats, ws);
+  MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 1, stats);
   g_launches.fetch_add(4);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
@@ -582,7 +538,7 @@ extern "C" int madrl_center_advantages_f32(size_t n, float* adv_dev, int center,
   MADRL_REQUIRE(n >= 1, "bad sizes");
   MADRL_REQUIRE(adv_dev && stats_dev && workspace_dev, "NULL buffer");
   cudaStream_t s = (cudaStream_t)stream;
-  const int rc = run_moments(n, 0, adv_dev, nullptr, stats_dev, workspace_dev, s);
+  const int rc = run_moments(n, 1, adv_dev, nullptr, stats_dev, workspace_dev, s);
   if (rc) return rc;
   if (center || positive) {
     MADRL_LAUNCH(center_apply_kernel, kMomBlocks, kMomThreads, 0, s, n, adv_dev, stats_dev, center, positive);
@@ -596,7 +552,7 @@ extern "C" int madrl_moments_f32(size_t n, const float* a_dev, const float* b_de
                                  double* workspace_dev, void* stream) {
   MADRL_REQUIRE(n >= 1, "bad sizes");
   MADRL_REQUIRE(a_dev && stats_dev && workspace_dev, "NULL buffer");
-  return run_moments(n, 0, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
+  return run_moments(n, 1, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
 }
 
 extern "C" int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
@@ -636,23 +592,29 @@ extern "C" int madrl_paths_plan(int T, int E, int A, const uint8_t* done_dev, in
   return MADRL_OK;
 }
 
+// The grid of the row-copy kernels: one thread per row of at most 4 words, one warp per wider row.
+template <typename... P, typename... Args>
+static int launch_rows(void (*one_thread)(P...), void (*one_warp)(P...), size_t rows, int D, void* stream,
+                       Args... args) {
+  const bool narrow = D <= 4;
+  const size_t blocks = ((narrow ? rows : rows * 32) + 255) / 256;
+  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many rows for one launch");
+  if (narrow)
+    MADRL_LAUNCH(one_thread, (unsigned)blocks, 256, 0, (cudaStream_t)stream, args...);
+  else
+    MADRL_LAUNCH(one_warp, (unsigned)blocks, 256, 0, (cudaStream_t)stream, args...);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
 template <typename W>
 static int paths_pack(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
                       const int32_t* seg_start_dev, const int32_t* seg_len_dev, void* dst_dev, void* stream) {
   MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && D >= 1, "bad shape");
   MADRL_REQUIRE(src_dev && seg_start_dev && seg_len_dev && dst_dev, "NULL pointer");
-  const size_t rows = (size_t)T * E * A;
-  const size_t blocks = D <= 4 ? (rows + 255) / 256 : (rows * 32 + 255) / 256;
-  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many rows for one launch");
-  if (D <= 4)
-    MADRL_LAUNCH(paths_pack_narrow_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D,
-                 (const W*)src_dev, (const W*)first_dev, seg_start_dev, seg_len_dev, (W*)dst_dev);
-  else
-    MADRL_LAUNCH(paths_pack_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, T, E, A, D, (const W*)src_dev,
-                 (const W*)first_dev, seg_start_dev, seg_len_dev, (W*)dst_dev);
-  g_launches.fetch_add(1);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
+  return launch_rows(paths_pack_kernel<1, W>, paths_pack_kernel<32, W>, (size_t)T * E * A, D, stream, T, E, A, D,
+                     (const W*)src_dev, (const W*)first_dev, seg_start_dev, seg_len_dev, (W*)dst_dev);
 }
 
 extern "C" int madrl_paths_pack_u32(int T, int E, int A, int D, const void* src_dev, const void* first_dev,
@@ -673,17 +635,8 @@ static int paths_pad(int T, int E, int A, int D, int P, int Lmax, const void* sr
   MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && D >= 1 && P >= 1 && Lmax >= 1, "bad shape");
   MADRL_REQUIRE(src_dev && rec_dev && dst_dev, "NULL pointer");
   const size_t rows = (size_t)P * Lmax;
-  const size_t blocks = D <= 4 ? (rows + 255) / 256 : (rows * 32 + 255) / 256;
-  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many padded rows for one launch");
-  if (D <= 4)
-    MADRL_LAUNCH(paths_pad_narrow_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, E, A, D, rows, Lmax,
-                 (const W*)src_dev, (const W*)first_dev, rec_dev, (W*)dst_dev);
-  else
-    MADRL_LAUNCH(paths_pad_kernel<W>, (unsigned)blocks, 256, 0, (cudaStream_t)stream, E, A, D, rows, Lmax,
-                 (const W*)src_dev, (const W*)first_dev, rec_dev, (W*)dst_dev);
-  g_launches.fetch_add(1);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
+  return launch_rows(paths_pad_kernel<1, W>, paths_pad_kernel<32, W>, rows, D, stream, E, A, D, rows, Lmax,
+                     (const W*)src_dev, (const W*)first_dev, rec_dev, (W*)dst_dev);
 }
 
 extern "C" int madrl_paths_pad_u32(int T, int E, int A, int D, int P, int Lmax, const void* src_dev,

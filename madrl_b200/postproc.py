@@ -38,6 +38,23 @@ def _obs_fn(name, dtype):
     return getattr(_lib.lib(), "madrl_%s_%s" % (name, "bf16" if dtype == torch.bfloat16 else "f32"))
 
 
+def _paths_plan(done, A):
+    """How a rollout is cut into paths (at ``done`` and at the end of the rollout): madrl_paths_plan over done [T,E]
+    uint8 on its CUDA device, enqueued without a host synchronisation.  Returns int32 seg_s, seg_l [T,E] (start and
+    length of the path holding each step), n_ep [E] (paths per env) and ep_rec [E,T,3] (per path of each env: start,
+    length, terminated; zero past the env's last path)."""
+    T, E = done.shape
+    dev = done.device
+    seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
+    seg_l = torch.empty((T, E), dtype=torch.int32, device=dev)
+    n_ep = torch.empty((E,), dtype=torch.int32, device=dev)
+    ep_rec = torch.zeros((E, T, 3), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(_lib.lib().madrl_paths_plan(T, E, A, _ptr(done.contiguous()), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep),
+                                               _ptr(ep_rec), _lib.stream(dev)))
+    return seg_s, seg_l, n_ep, ep_rec
+
+
 _OBS_DTYPES = (torch.float32, torch.bfloat16)
 _PACKED_DTYPES = (torch.float32, torch.int32, torch.uint32, torch.bfloat16)   # pack_paths moves 4- and 2-byte words
 
@@ -375,15 +392,7 @@ class LinearFeatureBaseline(object):
         _lib.require_tensor(obs, "obs", obs.dtype, (T, E, A, D), self.device, contiguous=False)
         if T * E * A >= 2 ** 31:
             raise ValueError("T*E*A must be < 2^31, got %d" % (T * E * A))
-        L = _lib.lib()
-        done = done.contiguous()
-        seg_s = torch.empty((T, E), dtype=torch.int32, device=self.device)
-        seg_l = torch.empty((T, E), dtype=torch.int32, device=self.device)
-        n_ep = torch.empty((E,), dtype=torch.int32, device=self.device)
-        ep_rec = torch.empty((E, T, 3), dtype=torch.int32, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(L.madrl_paths_plan(T, E, A, _ptr(done), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep), _ptr(ep_rec),
-                                          _lib.stream(self.device)))
+        seg_s = _paths_plan(done, A)[0]
         cont = lambda x: None if x is None else x.contiguous()          # noqa: E731
         return (T, E, A, D), cont(obs), cont(obs_before), cont(t0), seg_s
 
@@ -491,6 +500,17 @@ def process_samples_concurrent(baseline, obs, done, rew, discount, gae_lambda, o
     T, E, A, _ = _lib.require_tensor(obs, "obs", _OBS_DTYPES, (None, None, baseline.n_agents, baseline.obs_dim),
                                      None, contiguous=False).shape
     _lib.require_tensor(rew, "rew", torch.float32, (T, E, A), obs.device, contiguous=False)
+    values, adv, ret, ev = _sampler_core(baseline, obs, done, rew, discount, gae_lambda, obs_before, t0, center_adv,
+                                         positive_adv, True, group)
+    if not baseline.shared:
+        baseline.fit(obs, done, ret, obs_before, t0, group)
+    return values, adv, ret, ev
+
+
+def _sampler_core(baseline, obs, done, rew, discount, gae_lambda, obs_before, t0, center, positive, per_agent, group):
+    """What both branches of ``process_samples`` do before the baseline fit, in the reference's order: predict, `gae`,
+    the explained variance and `center_advantages` (per agent with ``per_agent``).  A shared baseline is fitted first
+    (the returns do not depend on the values); the caller fits any other one last.  -> (values, adv, ret, ev)."""
     if baseline.shared:
         _, ret = gae(rew, torch.zeros_like(rew), done, discount, gae_lambda)
         baseline.fit(obs, done, ret, obs_before, t0, group)
@@ -499,11 +519,9 @@ def process_samples_concurrent(baseline, obs, done, rew, discount, gae_lambda, o
     else:
         values = baseline.predict(obs, done, obs_before, t0)
         adv, ret = gae(rew, values, done, discount, gae_lambda)
-    ev = explained_variance(values, ret, per_agent=True)
-    if center_adv or positive_adv:
-        adv = center_advantages(adv, center_adv, positive_adv, inplace=True, per_agent=True)
-    if not baseline.shared:
-        baseline.fit(obs, done, ret, obs_before, t0, group)
+    ev = explained_variance(values, ret, per_agent=per_agent)
+    if center or positive:
+        adv = center_advantages(adv, center, positive, inplace=True, per_agent=per_agent)
     return values, adv, ret, ev
 
 
@@ -571,7 +589,8 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
     step, the reset observation on a done step) and the packed ``observations`` are shifted so that row t
     is the observation action t was taken in -- what rllab stores (ma_sampler.py:71-77).  Without it,
     ``obs`` is used as is (the host ``to_paths`` contract).  Two kernels of csrc/postproc.cu: a plan pass
-    over ``done`` and one HBM-bound row permutation per tensor; no host loop.  Tensors of 4-byte elements,
+    over ``done`` and one HBM-bound row permutation per tensor; no host loop, and one 16-byte device->host read
+    (the path count, `_PathTable`).  Tensors of 4-byte elements,
     and bfloat16 observations (2-byte rows, ``madrl_paths_pack_u16``)."""
     T, E, A = _lib.require_tensor(obs, "obs", _PACKED_DTYPES, (None, None, None, ...), None,
                                   contiguous=False).shape[:3]
@@ -585,43 +604,12 @@ def pack_paths(obs, actions, rew, done, infos=None, obs_before=None):
         obs_before = _lib.require_tensor(obs_before.to(obs.dtype).contiguous(), "obs_before", obs.dtype,
                                          tuple(obs.shape[1:]), dev)
     _lib.require_tensor(obs, "obs", obs.dtype, (T, E, A, ...), "cuda", contiguous=False)
-    L = _lib.lib()
-    done = done.contiguous()
-    seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
-    seg_l = torch.empty((T, E), dtype=torch.int32, device=dev)
-    n_ep = torch.empty((E,), dtype=torch.int32, device=dev)
-    ep_rec = torch.zeros((E, T, 3), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        st = _lib.stream(dev)
-        _lib.check(L.madrl_paths_plan(T, E, A, _ptr(done), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep), _ptr(ep_rec), st))
-
-        def pack(x, per_agent, first=None):
-            x = x.contiguous()
-            n_agents = A if per_agent else 1
-            tail = tuple(x.shape[3:] if per_agent else x.shape[2:])
-            D = max(1, int(np.prod(tail)))
-            out = torch.empty((T * E * n_agents,) + tail, dtype=x.dtype, device=dev)
-            # per-env tensors (n_agents = 1): the row offset e*T + s + (t - s) = e*T + t for any (s, L)
-            fn = L.madrl_paths_pack_u16 if x.element_size() == 2 else L.madrl_paths_pack_u32
-            _lib.check(fn(T, E, n_agents, D, _ptr(x), _ptr(first), _ptr(seg_s), _ptr(seg_l), _ptr(out), st))
-            return out
-
-        packed_obs = pack(obs, True, obs_before)
-        packed_act = pack(actions, True)
-        packed_rew = pack(rew, True)
-        packed_info = {k: pack(v, False) for k, v in (infos or {}).items()}
-    # per-path records from the (tiny) per-episode records: plain tensor ops, no host loop
-    slot = torch.arange(T, device=dev).unsqueeze(0)
-    live = slot < n_ep.unsqueeze(1)                                   # [E, T] valid episode slots
-    e_idx, _ = torch.nonzero(live, as_tuple=True)
-    rec = ep_rec[live]                                                # [n_episodes_total, 3] in (env, episode) order
-    s, Ln, term = rec[:, 0].long(), rec[:, 1].long(), rec[:, 2]
-    a_idx = torch.arange(A, device=dev)
-    offset = ((e_idx * T * A + s * A).unsqueeze(1) + a_idx.unsqueeze(0) * Ln.unsqueeze(1)).reshape(-1)
-    rep = lambda v: v.unsqueeze(1).expand(-1, A).reshape(-1)          # noqa: E731
-    return PackedPaths(observations=packed_obs, actions=packed_act, rewards=packed_rew, env_infos=packed_info,
-                       offset=offset, length=rep(Ln), env=rep(e_idx), agent=a_idx.repeat(rec.shape[0]),
-                       terminated=rep(term).bool(), info_offset=rep(e_idx * T + s))
+    table = _PathTable(done, A, agent_major=False)
+    env, agent, s, Ln = table.rec.long().t().contiguous()
+    infos = {k: table.pack(v, per_agent=False) for k, v in (infos or {}).items()}
+    return PackedPaths(observations=table.pack(obs, first=obs_before), actions=table.pack(actions),
+                       rewards=table.pack(rew), env_infos=infos, offset=env * T * A + s * A + agent * Ln, length=Ln,
+                       env=env, agent=agent, terminated=table.terminated, info_offset=env * T + s)
 
 
 # ---------------------------------------------------------------- the recurrent branch of process_samples
@@ -639,22 +627,15 @@ def _check_mode(mode):
 
 
 class _PathTable(object):
-    """The paths of one rollout (episodes cut at ``done`` and at the end of the rollout, as ``pack_paths`` cuts
-    them) as the record table of madrl_paths_pad_*: int32 [P, 4] = (env, agent, start step, length).  Order
-    (env, episode, agent), or agent-major (agent, env, episode) for concurrent control.  P and the longest length
-    L come from one 16-byte device->host read."""
+    """The paths of one rollout (episodes cut at ``done`` and at the end of the rollout, `_paths_plan`) as the
+    record table of madrl_paths_pad_*: int32 [P, 4] = (env, agent, start step, length).  Order (env, episode, agent),
+    or agent-major (agent, env, episode) for concurrent control.  P and the longest length L come from one 16-byte
+    device->host read.  ``seg_s`` / ``seg_l`` of the plan drive madrl_paths_pack_*."""
 
     def __init__(self, done, A, agent_major):
         T, E = done.shape
         dev = done.device
-        lib = _lib.lib()
-        seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
-        seg_l = torch.empty((T, E), dtype=torch.int32, device=dev)
-        n_ep = torch.empty((E,), dtype=torch.int32, device=dev)
-        ep_rec = torch.zeros((E, T, 3), dtype=torch.int32, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.madrl_paths_plan(T, E, A, _ptr(done.contiguous()), _ptr(seg_s), _ptr(seg_l), _ptr(n_ep),
-                                            _ptr(ep_rec), _lib.stream(dev)))
+        self.seg_s, self.seg_l, n_ep, ep_rec = _paths_plan(done, A)
         n, L = (int(v) for v in torch.stack([n_ep.sum(), ep_rec[:, :, 1].max().long()]).cpu())
         live = torch.arange(T, device=dev).unsqueeze(0) < n_ep.unsqueeze(1)
         slot = torch.nonzero_static(live, size=n)                 # (env, episode) of every episode, in that order
@@ -669,19 +650,30 @@ class _PathTable(object):
         self.T, self.E, self.A, self.P, self.L = T, E, A, n * A, L
         self.lead = (A, n) if agent_major else (n * A,)
 
-    def pad(self, x, per_agent=True, first=None):
-        """x [T,E,A,...] (per agent) or [T,E,...] (per env) -> [*lead, L, ...], zero past each path's end."""
+    def _copy(self, kind, x, per_agent, first, rows, sizes, plan):
+        """madrl_paths_<kind>_u32 / _u16 (by the element size) from x [T,E,A,...] (per agent) or [T,E,...] (per env:
+        each agent's path gets its env's rows) into a new [rows, ...]; ``first``: the one-step shift.  ``sizes`` and
+        ``plan`` (tensors) are the entry point's own arguments after the row width and after ``first``."""
         x = x.contiguous()
         tail = tuple(x.shape[3:] if per_agent else x.shape[2:])
-        D = max(1, int(np.prod(tail)))
-        out = torch.empty((self.P, self.L) + tail, dtype=x.dtype, device=x.device)
-        lib = _lib.lib()
-        fn = lib.madrl_paths_pad_u16 if x.element_size() == 2 else lib.madrl_paths_pad_u32
+        out = torch.empty((rows,) + tail, dtype=x.dtype, device=x.device)
+        fn = getattr(_lib.lib(), "madrl_paths_%s_%s" % (kind, "u16" if x.element_size() == 2 else "u32"))
         with torch.cuda.device(x.device):
-            _lib.check(fn(self.T, self.E, self.A if per_agent else 1, D, self.P, self.L, _ptr(x),
-                          _ptr(None if first is None else first.contiguous()), _ptr(self.rec), _ptr(out),
+            _lib.check(fn(self.T, self.E, self.A if per_agent else 1, max(1, int(np.prod(tail))), *sizes, _ptr(x),
+                          _ptr(None if first is None else first.contiguous()), *map(_ptr, plan), _ptr(out),
                           _lib.stream(x.device)))
-        return out.view(self.lead + (self.L,) + tail)
+        return out
+
+    def pack(self, x, per_agent=True, first=None):
+        """x [T,E,A,...] (per agent) -> its rows in path order (`PackedPaths`); per env, [T,E,...] -> (env, time)
+        order, since the row of (t, e) in a path starting at s is e*T + s + (t - s) = e*T + t."""
+        rows = self.T * self.E * (self.A if per_agent else 1)
+        return self._copy("pack", x, per_agent, first, rows, (), (self.seg_s, self.seg_l))
+
+    def pad(self, x, per_agent=True, first=None):
+        """x [T,E,A,...] (per agent) or [T,E,...] (per env) -> [*lead, L, ...], zero past each path's end."""
+        out = self._copy("pad", x, per_agent, first, self.P * self.L, (self.P, self.L), (self.rec,))
+        return out.view(self.lead + (self.L,) + out.shape[1:])
 
     def valids(self):
         """float32 [*lead, L]: 1 on a path's steps, 0 on its padding."""
@@ -852,17 +844,8 @@ def process_samples_recurrent(baseline, obs, actions, rew, done, discount, gae_l
                                                                                  "without"))
     obs, actions, rew, done, infos, obs_before, agent_infos = _recurrent_inputs(
         mode, obs, actions, rew, done, infos, obs_before, agent_infos, _OBS_DTYPES, (torch.float32,), t0)
-    if baseline.shared:
-        _, ret = gae(rew, torch.zeros_like(rew), done, discount, gae_lambda)
-        baseline.fit(obs, done, ret, obs_before, t0, group)
-        values = baseline.predict(obs, done, obs_before, t0)
-        adv, _ = gae(rew, values, done, discount, gae_lambda)
-    else:
-        values = baseline.predict(obs, done, obs_before, t0)
-        adv, ret = gae(rew, values, done, discount, gae_lambda)
-    ev = explained_variance(values, ret, per_agent=concurrent)
-    if center_adv:
-        adv = center_advantages(adv, True, False, inplace=True, per_agent=concurrent)
+    values, adv, ret, ev = _sampler_core(baseline, obs, done, rew, discount, gae_lambda, obs_before, t0, center_adv,
+                                         False, concurrent, group)
     table = _PathTable(done, obs.shape[2], concurrent)
     data = _pad_all(table, obs, actions, rew, infos, obs_before, agent_infos)
     data.update(advantages=table.pad(adv), returns=table.pad(ret))
