@@ -523,6 +523,65 @@ int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_de
                                   const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
                                   float* values_dev, void* stream);
 
+/* rltools' sample processing (rltools/rltools/samplers/__init__.py:35-88).
+ *   madrl_running_moments_*  nn.Standardizer's batch statistics: sums float64 [G][2][D] = the column sums of x and
+ *                            of x^2 over the rows k G + g (k < R) of group g of x [R*G][D] (float32, or bfloat16
+ *                            widened), deterministic (fixed row slices, ascending combination).  first != NULL:
+ *                            row r is read from first [shift][D] for r < shift and from x[r - shift] afterwards
+ *                            (the observation an action was taken in; shift = E*A).  ws:
+ *                            madrl_running_moments_workspace_size bytes.  MADRL_EINVAL for R, D < 1, G outside
+ *                            [1, MADRL_AGENTS_MAX], a shift outside [1, R*G] with first, or a NULL required buffer.
+ *   madrl_time_baseline_f32  q float32 [T][E][A] -> bin_sum float64 [G][L], bin_count int32 [G][L] (G = A with
+ *                            per_agent, else 1 over every agent's rows): the sum of q and the number of rows whose
+ *                            time index (as madrl_lfb_*: t - seg_start, plus t0[e] on env e's first path) is i;
+ *                            simplev float32 [T][E][A] = sum / count of the row's bin (NaN for an index >= L).
+ *                            seg_start, n_ep, ep_rec: madrl_paths_plan's outputs.  Deterministic, no atomics.  ws:
+ *                            madrl_time_baseline_workspace_size(G, L) bytes.  MADRL_EINVAL for sizes below 1,
+ *                            T*E*A >= 2^31, per_agent with A > MADRL_AGENTS_MAX or a NULL required buffer. */
+int madrl_running_moments_workspace_size(int G, int D, size_t* bytes);
+int madrl_running_moments_f32(size_t R, int G, int D, size_t shift, const float* x_dev, const float* first_dev,
+                              double* sums_dev, double* ws_dev, void* stream);
+int madrl_running_moments_bf16(size_t R, int G, int D, size_t shift, const void* x_dev, const void* first_dev,
+                               double* sums_dev, double* ws_dev, void* stream);
+int madrl_time_baseline_workspace_size(int G, int L, size_t* bytes);
+int madrl_time_baseline_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
+                            const int32_t* seg_start_dev, const int32_t* n_ep_dev, const int32_t* ep_rec_dev,
+                            const int32_t* t0_dev, double* bin_sum_dev, int32_t* bin_count_dev, float* simplev_dev,
+                            void* ws_dev, void* stream);
+
+/* rltools' LinearFeatureBaseline (rltools/rltools/baselines/linear.py): the madrl_lfb_* kernels with rltools'
+ * feature map, Df = D + 3: [(o - mu) / s, i/100, (i/100)^2, 1] with o widened to float64 and not clipped.
+ * norm float64 [2][D] ([A][2][D] for the _agents entry points) = the obsnorm's mean and stdev + eps per column
+ * (the quotient is a float64 division), or NULL for no obsnorm (the columns are o).  Rows, time indices,
+ * determinism, argument checks and the _agents grouping as for madrl_lfb_*; ws: madrl_lfbr_workspace_size /
+ * madrl_lfbr_agents_workspace_size bytes (nb = ceil((D+4)/64)). */
+int madrl_lfbr_workspace_size(int D, size_t* bytes);
+int madrl_lfbr_agents_workspace_size(int D, int A, size_t* bytes);
+int madrl_lfbr_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev,
+    double* ws_dev, void* stream);
+int madrl_lfbr_predict_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev,
+    float* values_dev, void* stream);
+int madrl_lfbr_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev,
+    double* ws_dev, void* stream);
+int madrl_lfbr_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev,
+    float* values_dev, void* stream);
+int madrl_lfbr_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev,
+    double* ws_dev, void* stream);
+int madrl_lfbr_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev,
+    float* values_dev, void* stream);
+int madrl_lfbr_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev,
+    double* ws_dev, void* stream);
+int madrl_lfbr_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev,
+    float* values_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

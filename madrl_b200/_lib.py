@@ -179,6 +179,19 @@ def _declare(lib):
         lib.madrl_paths_pad_u32.argtypes = [i32] * 6 + [vp] * 5
         lib.madrl_paths_pad_u16.argtypes = lib.madrl_paths_pad_u32.argtypes
         lib.madrl_path_sums_f32.argtypes = [i32] * 4 + [vp] * 6
+    if hasattr(lib, "madrl_time_baseline_f32"):  # rltools' sample processing (absent from older builds)
+        sz = C.c_size_t
+        lib.madrl_running_moments_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
+        lib.madrl_running_moments_f32.argtypes = [sz, i32, i32, sz] + [vp] * 5
+        lib.madrl_running_moments_bf16.argtypes = lib.madrl_running_moments_f32.argtypes
+        lib.madrl_time_baseline_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
+        lib.madrl_time_baseline_f32.argtypes = [i32] * 5 + [vp] * 10
+        lib.madrl_lfbr_workspace_size.argtypes = [i32, C.POINTER(sz)]
+        lib.madrl_lfbr_agents_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
+        for dt in ("f32", "bf16"):
+            for ag in ("", "_agents"):
+                getattr(lib, "madrl_lfbr_normal_eq%s_%s" % (ag, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 9
+                getattr(lib, "madrl_lfbr_predict%s_%s" % (ag, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 8
 
 
 def lib():

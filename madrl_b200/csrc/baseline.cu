@@ -17,6 +17,13 @@
 // *_agents entry points run the same kernels over A row groups, group a = the rows r = k A + a of agent a.  Each
 // group's normal equations read that agent's rows only, so all A systems come from one launch with the same rows,
 // tile pairs and MMAs as the pooled one; predict reads coefficient row a for agent a's rows.
+//
+// rltools' LinearFeatureBaseline (rltools/rltools/baselines/linear.py) is the same pair of kernels with another
+// feature map (the kMap template parameter, kLfbRltools; entry points madrl_lfbr_*): Df = D + 3 features
+//     [(o - mu) / s, i/100, (i/100)^2, 1 | y]
+// where mu and s are the baseline's obsnorm (nn.Standardizer) per column, passed as float64 `norm` [2][D] (mean,
+// stdev + eps; [A][2][D] per agent), o is widened to float64 and not clipped, and the quotient is a float64
+// division, as NumPy takes it.  norm == NULL is the NoOpStandardizer: the columns are o itself.
 #include "common.cuh"
 
 namespace madrl {
@@ -41,17 +48,13 @@ constexpr int kLfbSlices = MADRL_LFB_SLICES;
 // float64 sum chain is longer than that: a slice of a C2 launch is 109 000 rows.
 constexpr int kLfbFlush = 64;
 
-static inline int lfb_cols(int D) { return 2 * D + 5; }
-static inline int lfb_tiles(int D) { return (lfb_cols(D) + kLfbTile - 1) / kLfbTile; }
+// The feature maps: rllab's (Df = 2 D + 4) and rltools' (Df = D + 3).  Columns = Df + 1 (the return).
+enum LfbMap { kLfbRllab = 0, kLfbRltools = 1 };
+template <int kMap>
+__host__ __device__ __forceinline__ int lfb_cols(int D) { return kMap == kLfbRllab ? 2 * D + 5 : D + 4; }
+template <int kMap>
+static inline int lfb_tiles(int D) { return (lfb_cols<kMap>(D) + kLfbTile - 1) / kLfbTile; }
 __host__ __device__ __forceinline__ int lfb_agent_slices(int A) { return (kLfbSlices + A - 1) / A; }
-
-// Time index of the rows (t, e, .) with te = t E + e: the position in the path, plus t0[e] on env e's first path.
-template <typename I>
-__device__ __forceinline__ int lfb_index(I te, int E, const int32_t* seg_start, const int32_t* t0) {
-  const I t = te / (I)E, e = te - t * (I)E;
-  const int s = seg_start[te];
-  return (int)t - s + ((t0 != nullptr && s == 0) ? t0[e] : 0);
-}
 
 // Source row and time index of row r.
 template <typename O>
@@ -74,6 +77,26 @@ __device__ __forceinline__ void lfb_time(int idx, double& a1, double& a2, double
 }
 
 __device__ __forceinline__ double lfb_clip(float v) { return (double)(v < -10.f ? -10.f : (v > 10.f ? 10.f : v)); }
+
+// The value of observation column d (squared: rllab's second block) from the widened observation v.  rltools:
+// (v - mu[d]) / s[d] with norm = [mu | s] ([2][D]), or v itself without an obsnorm.
+template <int kMap>
+__device__ __forceinline__ double lfb_obs(float v, bool sq, int d, int D, const double* norm) {
+  if (kMap == kLfbRllab) {
+    const double x = lfb_clip(v);
+    return sq ? x * x : x;
+  }
+  const double x = (double)v;
+  return norm ? (x - norm[d]) / norm[D + d] : x;
+}
+
+// A row past the slice fetches 0, which gives every rllab feature 0; rltools' standardised 0 is not, so its rows
+// past the slice store 0 explicitly.
+template <int kMap>
+__device__ __forceinline__ double lfb_pad(bool valid, double v) {
+  if constexpr (kMap == kLfbRllab) return v;
+  else return valid ? v : 0.0;
+}
 
 // tile pair p -> (I, J), I <= J, enumerated row by row
 __device__ __forceinline__ void lfb_pair(int p, int nb, int& I, int& J) {
@@ -100,11 +123,9 @@ __device__ __forceinline__ uint32_t lfb_fetch(int kind, int d, uint32_t r, bool 
   return (uint32_t)lfb_index(r / (uint32_t)A, E, seg_start, t0);
 }
 
-__device__ __forceinline__ double lfb_value(int kind, uint32_t v) {
-  if (kind <= kLfbObsSq) {
-    const double x = lfb_clip(__int_as_float((int)v));
-    return kind == kLfbObs ? x : x * x;
-  }
+template <int kMap>
+__device__ __forceinline__ double lfb_value(int kind, uint32_t v, int d, int D, const double* norm) {
+  if (kind <= kLfbObsSq) return lfb_obs<kMap>(__int_as_float((int)v), kind != kLfbObs, d, D, norm);
   if (kind == kLfbY) return (double)__int_as_float((int)v);
   if (kind == kLfbOne) return (double)v;
   if (kind == kLfbPad) return 0.0;
@@ -115,16 +136,18 @@ __device__ __forceinline__ double lfb_value(int kind, uint32_t v) {
 
 // kAgents = false: one group (every row), kLfbSlices slices.  kAgents = true: A groups of T E rows each (row
 // k A + g of group g), lfb_agent_slices(A) slices per group.  The loop runs over the group's row counter k.
-template <typename O, bool kAgents>
+// norm: rltools' obsnorm ([groups][2][D], or NULL); the rllab map never reads it.
+template <typename O, bool kAgents, int kMap>
 __global__ void __launch_bounds__(kLfbThreads, 2)
 lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* __restrict__ obs_before,
                 const int32_t* __restrict__ seg_start, const int32_t* __restrict__ t0, const float* __restrict__ ret,
-                double* __restrict__ ws) {
+                double* __restrict__ ws, const double* __restrict__ norm) {
   __shared__ __align__(16) double sF[2][kLfbRows][kLfbLd];   // features of tiles I and J (J only if J != I)
-  const int nb = (2 * D + 5 + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
+  const int nb = (lfb_cols<kMap>(D) + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
   const int pair = blockIdx.x % P, gs = blockIdx.x / P;      // gs = group * S + slice
   const int S = kAgents ? lfb_agent_slices(A) : kLfbSlices;
   const int group = kAgents ? gs / S : 0, slice = kAgents ? gs - group * S : gs;
+  if (kMap == kLfbRltools && kAgents && norm) norm += (size_t)group * 2 * D;
   int I, J;
   lfb_pair(pair, nb, I, J);
   const uint32_t N = kAgents ? (uint32_t)T * E : (uint32_t)T * E * A;   // rows of the group
@@ -143,9 +166,15 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
 #pragma unroll
   for (int b = 0; b < 2; ++b) {
     const int tile = b == 0 ? I : J, c = tile * kLfbTile + j;
-    kind[b] = c < D ? kLfbObs : (c < 2 * D ? kLfbObsSq : (c < 2 * D + 5 ? kLfbA1 + (c - 2 * D) : kLfbPad));
-    d[b] = c < D ? c : c - D;
-    obs_only[b] = (tile + 1) * kLfbTile <= 2 * D;
+    if (kMap == kLfbRllab) {
+      kind[b] = c < D ? kLfbObs : (c < 2 * D ? kLfbObsSq : (c < 2 * D + 5 ? kLfbA1 + (c - 2 * D) : kLfbPad));
+      d[b] = c < D ? c : c - D;
+      obs_only[b] = (tile + 1) * kLfbTile <= 2 * D;
+    } else {                   // [obs | a1, a2 | 1 | y]
+      kind[b] = c < D ? kLfbObs : (c < D + 2 ? kLfbA1 + (c - D) : (c < D + 4 ? kLfbOne + (c - D - 2) : kLfbPad));
+      d[b] = c;
+      obs_only[b] = (tile + 1) * kLfbTile <= D;
+    }
   }
   const uint32_t EA = (uint32_t)E * A;
   double acc[2][4][4];
@@ -205,13 +234,14 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
       if (obs_only[b]) {
         const bool sq = kind[b] == kLfbObsSq;
 #pragma unroll
-        for (int i = 0; i < kLfbRows / 2; ++i) {
-          const double x = lfb_clip(__int_as_float((int)nxt[b][i]));
-          sts_f64(&sF[b][k0 + 2 * i][j], sq ? x * x : x);
-        }
+        for (int i = 0; i < kLfbRows / 2; ++i)
+          sts_f64(&sF[b][k0 + 2 * i][j], lfb_pad<kMap>(r0 + k0 + 2 * i < r_end,
+                                                       lfb_obs<kMap>(__int_as_float((int)nxt[b][i]), sq, d[b], D, norm)));
       } else {
 #pragma unroll
-        for (int i = 0; i < kLfbRows / 2; ++i) sts_f64(&sF[b][k0 + 2 * i][j], lfb_value(kind[b], nxt[b][i]));
+        for (int i = 0; i < kLfbRows / 2; ++i)
+          sts_f64(&sF[b][k0 + 2 * i][j], lfb_pad<kMap>(r0 + k0 + 2 * i < r_end,
+                                                       lfb_value<kMap>(kind[b], nxt[b][i], d[b], D, norm)));
       }
     }
     __syncthreads();
@@ -242,8 +272,9 @@ lfb_gram_kernel(int T, int E, int A, int D, const O* __restrict__ obs, const O* 
 // G[i][j] = G[j][i] = sum over the slices (ascending) of the partial tiles; the upper triangle of a diagonal tile
 // is mirrored, so G is exactly symmetric.  One CTA per (group, tile pair), S slices per group;
 // G: [groups][Df+1][Df+1].
+template <int kMap>
 __global__ void lfb_reduce_kernel(int D, int S, const double* __restrict__ ws, double* __restrict__ G) {
-  const int Dc = 2 * D + 5, nb = (Dc + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
+  const int Dc = lfb_cols<kMap>(D), nb = (Dc + kLfbTile - 1) / kLfbTile, P = nb * (nb + 1) / 2;
   const int pair = blockIdx.x % P, group = blockIdx.x / P;
   int I, J;
   lfb_pair(pair, nb, I, J);
@@ -260,33 +291,42 @@ __global__ void lfb_reduce_kernel(int D, int S, const double* __restrict__ ws, d
 }
 
 // One warp per row: lanes stride over the D observation values (coalesced), float64 FMAs, butterfly sum.
-// kAgents: coef is [A][Df] and row (t, e, a) uses row a.
-template <typename O, bool kAgents>
+// kAgents: coef is [A][Df] and row (t, e, a) uses row a (and, rltools, norm block a).
+template <typename O, bool kAgents, int kMap>
 __global__ void lfb_predict_kernel(int T, int E, int A, int D, const O* __restrict__ obs,
                                    const O* __restrict__ obs_before, const int32_t* __restrict__ seg_start,
                                    const int32_t* __restrict__ t0, const double* __restrict__ coef,
-                                   float* __restrict__ values) {
+                                   float* __restrict__ values, const double* __restrict__ norm) {
   const size_t r = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (r >= (size_t)T * E * A) return;                  // warp-uniform
-  if (kAgents) coef += (size_t)(r % (size_t)A) * (2 * D + 4);
+  if (kAgents) coef += (size_t)(r % (size_t)A) * (lfb_cols<kMap>(D) - 1);
   int idx;
   const O* src = lfb_row(r, E, A, D, obs, obs_before, seg_start, t0, idx);
   double acc = 0.0;
+  if (kMap == kLfbRltools && kAgents && norm) norm += (size_t)(r % (size_t)A) * 2 * D;
   for (int d = lane; d < D; d += 32) {
-    const double x = lfb_clip(obs_widen<float>(__ldcs(src + d)));
-    acc = fma(x, __ldg(coef + d), acc);
-    acc = fma(x * x, __ldg(coef + D + d), acc);
+    if constexpr (kMap == kLfbRllab) {
+      const double x = lfb_clip(obs_widen<float>(__ldcs(src + d)));
+      acc = fma(x, __ldg(coef + d), acc);
+      acc = fma(x * x, __ldg(coef + D + d), acc);
+    } else {
+      acc = fma(lfb_obs<kMap>(obs_widen<float>(__ldcs(src + d)), false, d, D, norm), __ldg(coef + d), acc);
+    }
   }
   acc = warp_allreduce_sum(acc);
   if (lane == 0) {
     double a1, a2, a3;
     lfb_time(idx, a1, a2, a3);
-    const double* ct = coef + 2 * D;
+    const double* ct = coef + (kMap == kLfbRllab ? 2 * D : D);
     acc = fma(a1, ct[0], acc);
     acc = fma(a2, ct[1], acc);
-    acc = fma(a3, ct[2], acc);
-    __stcs(values + r, (float)(acc + ct[3]));
+    if constexpr (kMap == kLfbRllab) {
+      acc = fma(a3, ct[2], acc);
+      __stcs(values + r, (float)(acc + ct[3]));
+    } else {
+      __stcs(values + r, (float)(acc + ct[2]));
+    }
   }
 }
 
@@ -297,24 +337,31 @@ using namespace madrl;
 static const int kLfbMaxD = 8192;
 
 // Bytes of scratch for `groups` row groups of S slices each.
+template <int kMap>
 static size_t lfb_ws_bytes(int D, int groups, int S) {
-  const size_t nb = (size_t)lfb_tiles(D);
+  const size_t nb = (size_t)lfb_tiles<kMap>(D);
   return (size_t)groups * S * (nb * (nb + 1) / 2) * kLfbTile * kLfbTile * sizeof(double);
 }
 
-extern "C" int madrl_lfb_workspace_size(int D, size_t* bytes) {
-  MADRL_REQUIRE(D >= 1 && D <= kLfbMaxD, "obs_dim must be in [1, %d], got %d", kLfbMaxD, D);
-  MADRL_REQUIRE(bytes, "NULL pointer");
-  *bytes = lfb_ws_bytes(D, 1, kLfbSlices);
-  return MADRL_OK;
-}
-
-extern "C" int madrl_lfb_agents_workspace_size(int D, int A, size_t* bytes) {
+template <int kMap>
+static int lfb_workspace_size(int D, int A, size_t* bytes) {
   MADRL_REQUIRE(D >= 1 && D <= kLfbMaxD, "obs_dim must be in [1, %d], got %d", kLfbMaxD, D);
   MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
   MADRL_REQUIRE(bytes, "NULL pointer");
-  *bytes = lfb_ws_bytes(D, A, lfb_agent_slices(A));
+  *bytes = lfb_ws_bytes<kMap>(D, A, A == 1 ? kLfbSlices : lfb_agent_slices(A));
   return MADRL_OK;
+}
+
+extern "C" int madrl_lfb_workspace_size(int D, size_t* bytes) { return lfb_workspace_size<kLfbRllab>(D, 1, bytes); }
+
+extern "C" int madrl_lfb_agents_workspace_size(int D, int A, size_t* bytes) {
+  return lfb_workspace_size<kLfbRllab>(D, A, bytes);
+}
+
+extern "C" int madrl_lfbr_workspace_size(int D, size_t* bytes) { return lfb_workspace_size<kLfbRltools>(D, 1, bytes); }
+
+extern "C" int madrl_lfbr_agents_workspace_size(int D, int A, size_t* bytes) {
+  return lfb_workspace_size<kLfbRltools>(D, A, bytes);
 }
 
 static int lfb_check(int T, int E, int A, int D) {
@@ -324,99 +371,144 @@ static int lfb_check(int T, int E, int A, int D) {
   return MADRL_OK;
 }
 
-template <typename O, bool kAgents>
+template <typename O, bool kAgents, int kMap>
 static int lfb_normal_eq(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
-                         const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev,
-                         double* ws_dev, void* stream) {
+                         const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
+                         const double* norm_dev, double* G_dev, double* ws_dev, void* stream) {
   const int rc = lfb_check(T, E, A, D);
   if (rc) return rc;
   if (kAgents)
     MADRL_REQUIRE(A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
   MADRL_REQUIRE(obs_dev && seg_start_dev && ret_dev && G_dev && ws_dev, "NULL buffer");
-  const int nb = lfb_tiles(D), P = nb * (nb + 1) / 2;
+  const int nb = lfb_tiles<kMap>(D), P = nb * (nb + 1) / 2;
   const int groups = kAgents ? A : 1, S = kAgents ? lfb_agent_slices(A) : kLfbSlices;
   cudaStream_t s = (cudaStream_t)stream;
-  MADRL_LAUNCH((lfb_gram_kernel<O, kAgents>), (unsigned)(P * S * groups), kLfbThreads, 0, s, T, E, A, D,
-               (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, ret_dev, ws_dev);
-  MADRL_LAUNCH(lfb_reduce_kernel, (unsigned)(P * groups), 128, 0, s, D, S, ws_dev, G_dev);
+  MADRL_LAUNCH((lfb_gram_kernel<O, kAgents, kMap>), (unsigned)(P * S * groups), kLfbThreads, 0, s, T, E, A, D,
+               (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, ret_dev, ws_dev, norm_dev);
+  MADRL_LAUNCH(lfb_reduce_kernel<kMap>, (unsigned)(P * groups), 128, 0, s, D, S, ws_dev, G_dev);
   g_launches.fetch_add(2);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
 }
 
-extern "C" int madrl_lfb_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
-                                       const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
-                                       double* G_dev, double* ws_dev, void* stream) {
-  return lfb_normal_eq<float, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
-                                     ws_dev, stream);
-}
-
-extern "C" int madrl_lfb_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
-                                        const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev,
-                                        double* G_dev, double* ws_dev, void* stream) {
-  return lfb_normal_eq<uint16_t, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
-                                        ws_dev, stream);
-}
-
-extern "C" int madrl_lfb_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev,
-                                              const float* obs_before_dev, const int32_t* seg_start_dev,
-                                              const int32_t* t0_dev, const float* ret_dev, double* G_dev,
-                                              double* ws_dev, void* stream) {
-  return lfb_normal_eq<float, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
-                                    ws_dev, stream);
-}
-
-extern "C" int madrl_lfb_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev,
-                                               const void* obs_before_dev, const int32_t* seg_start_dev,
-                                               const int32_t* t0_dev, const float* ret_dev, double* G_dev,
-                                               double* ws_dev, void* stream) {
-  return lfb_normal_eq<uint16_t, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, G_dev,
-                                       ws_dev, stream);
-}
-
-template <typename O, bool kAgents>
+template <typename O, bool kAgents, int kMap>
 static int lfb_predict(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
-                       const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev,
-                       void* stream) {
+                       const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev,
+                       const double* coef_dev, float* values_dev, void* stream) {
   const int rc = lfb_check(T, E, A, D);
   if (rc) return rc;
   if (kAgents)
     MADRL_REQUIRE(A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
   MADRL_REQUIRE(obs_dev && seg_start_dev && coef_dev && values_dev, "NULL buffer");
   const size_t rows = (size_t)T * E * A;
-  MADRL_LAUNCH((lfb_predict_kernel<O, kAgents>), (unsigned)((rows * 32 + 255) / 256), 256, 0, (cudaStream_t)stream,
-               T, E, A, D, (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev);
+  MADRL_LAUNCH((lfb_predict_kernel<O, kAgents, kMap>), (unsigned)((rows * 32 + 255) / 256), 256, 0,
+               (cudaStream_t)stream, T, E, A, D, (const O*)obs_dev, (const O*)obs_before_dev, seg_start_dev, t0_dev,
+               coef_dev, values_dev, norm_dev);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
 }
 
+extern "C" int madrl_lfb_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<float, false, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, nullptr,
+      G_dev, ws_dev, stream);
+}
+
 extern "C" int madrl_lfb_predict_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
-                                     const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
-                                     float* values_dev, void* stream) {
-  return lfb_predict<float, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev,
-                                   stream);
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<float, false, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, nullptr, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfb_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<uint16_t, false, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, nullptr,
+      G_dev, ws_dev, stream);
 }
 
 extern "C" int madrl_lfb_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
-                                      const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev,
-                                      float* values_dev, void* stream) {
-  return lfb_predict<uint16_t, false>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev,
-                                      values_dev, stream);
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<uint16_t, false, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, nullptr, coef_dev,
+      values_dev, stream);
 }
 
-extern "C" int madrl_lfb_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev,
-                                            const float* obs_before_dev, const int32_t* seg_start_dev,
-                                            const int32_t* t0_dev, const double* coef_dev, float* values_dev,
-                                            void* stream) {
-  return lfb_predict<float, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev, values_dev,
-                                  stream);
+extern "C" int madrl_lfb_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<float, true, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, nullptr,
+      G_dev, ws_dev, stream);
 }
 
-extern "C" int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev,
-                                             const void* obs_before_dev, const int32_t* seg_start_dev,
-                                             const int32_t* t0_dev, const double* coef_dev, float* values_dev,
-                                             void* stream) {
-  return lfb_predict<uint16_t, true>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, coef_dev,
-                                     values_dev, stream);
+extern "C" int madrl_lfb_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<float, true, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, nullptr, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfb_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<uint16_t, true, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, nullptr,
+      G_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<uint16_t, true, kLfbRllab>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, nullptr, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfbr_normal_eq_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<float, false, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, norm_dev,
+      G_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_lfbr_predict_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<float, false, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, norm_dev, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfbr_normal_eq_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<uint16_t, false, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, norm_dev,
+      G_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_lfbr_predict_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<uint16_t, false, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, norm_dev, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfbr_normal_eq_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<float, true, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, norm_dev,
+      G_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_lfbr_predict_agents_f32(int T, int E, int A, int D, const float* obs_dev, const float* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<float, true, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, norm_dev, coef_dev,
+      values_dev, stream);
+}
+
+extern "C" int madrl_lfbr_normal_eq_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const float* ret_dev, const double* norm_dev, double* G_dev, double* ws_dev,
+    void* stream) {
+  return lfb_normal_eq<uint16_t, true, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, ret_dev, norm_dev,
+      G_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_lfbr_predict_agents_bf16(int T, int E, int A, int D, const void* obs_dev, const void* obs_before_dev,
+    const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev, float* values_dev, void* stream) {
+  return lfb_predict<uint16_t, true, kLfbRltools>(T, E, A, D, obs_dev, obs_before_dev, seg_start_dev, t0_dev, norm_dev, coef_dev,
+      values_dev, stream);
 }

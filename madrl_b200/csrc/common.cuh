@@ -271,6 +271,15 @@ __device__ __forceinline__ const O* action_obs_row(I r, I EA, int D, const O* sr
   return first ? (r < EA ? first + (size_t)r * D : src + (size_t)(r - EA) * D) : src + (size_t)r * D;
 }
 
+// Time index of the rows (t, e, .) with te = t E + e: the position in the path, plus t0[e] on env e's first path
+// (seg_start from madrl_paths_plan).  The linear baselines' time features and the time-dependent baseline's bins.
+template <typename I>
+__device__ __forceinline__ int lfb_index(I te, int E, const int32_t* seg_start, const int32_t* t0) {
+  const I t = te / (I)E, e = te - t * (I)E;
+  const int s = seg_start[te];
+  return (int)t - s + ((t0 != nullptr && s == 0) ? t0[e] : 0);
+}
+
 // StandardizedEnv sees the TERMINAL observation of an episode before the reset one
 // (madrl_environments/__init__.py:283-291 step(), then reset()); under auto-reset the rollout's obs slot is
 // overwritten by the reset observation, so -- when the caller asked for it -- the rows of a finished env

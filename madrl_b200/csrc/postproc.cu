@@ -437,6 +437,135 @@ __global__ void path_sums_kernel(int E, int A, int P, const float* __restrict__ 
   first_ret[p] = (double)ret[k0];
 }
 
+
+// ---- rltools' sample processing (rltools/rltools/samplers/__init__.py:35-88) -----------------------------------
+// Running standardiser (nn.Standardizer, rltools/rltools/nn.py:533-592): the float64 column sums of x and x^2 over
+// the rows of a batch, from which the caller forms the batch means of update().  Rows r = k G + g of group g
+// (G = 1: every row; G = A: agent g's rows of a [..][A][D] tensor), read through action_obs_row (shift = the rows
+// before the first step).  Fixed grid: each group's rows are cut into rm_slices(G) slices, a CTA owns 32 columns
+// of one slice (8 warps over its rows, lane = column), and the slice partials are summed in ascending order by a
+// second pass: same inputs, same bits, on any SM count.  Squares of widened float32 values are exact in float64.
+#ifndef MADRL_RM_SLICES
+#define MADRL_RM_SLICES 64             // (the CPU emulator tests of tests/test_emulated_rltools.py build with fewer)
+#endif
+constexpr int kRmSlices = MADRL_RM_SLICES;
+constexpr int kRmWarps = 8;
+__host__ __device__ __forceinline__ int rm_slices(int G) { return (kRmSlices + G - 1) / G; }
+
+template <typename O>
+__global__ void __launch_bounds__(kRmWarps * 32) running_moments_partial_kernel(size_t R, int G, int D, size_t shift,
+                                                                                const O* __restrict__ x,
+                                                                                const O* __restrict__ first,
+                                                                                double* __restrict__ ws) {
+  const int CB = (D + 31) / 32, S = rm_slices(G);
+  const int cb = (int)(blockIdx.x % CB), gs = (int)(blockIdx.x / CB), g = gs / S, sl = gs - g * S;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, d = cb * 32 + lane;
+  const size_t k1 = R * (sl + 1) / S;
+  double s1 = 0.0, s2 = 0.0;
+  if (d < D)
+    for (size_t k = R * sl / S + w; k < k1; k += kRmWarps) {
+      const double v = (double)obs_widen<float>(action_obs_row(k * G + g, shift, D, x, first)[d]);
+      s1 += v;
+      s2 += v * v;
+    }
+  __shared__ double sh[kRmWarps][2][32];
+  sh[w][0][lane] = s1;
+  sh[w][1][lane] = s2;
+  __syncthreads();
+  if (w < 2 && d < D) {
+    double t = 0.0;
+    for (int i = 0; i < kRmWarps; ++i) t += sh[i][w][lane];
+    ws[((size_t)gs * 2 + w) * D + d] = t;
+  }
+}
+
+// sums[g][j][d] (j = 0: x, 1: x^2) = the slices' partials in ascending order.
+__global__ void running_moments_finalize_kernel(int G, int D, const double* __restrict__ ws, double* __restrict__ sums) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)G * 2 * D) return;
+  const int S = rm_slices(G);
+  const size_t g = i / (2 * (size_t)D), jd = i - g * 2 * D;
+  double t = 0.0;
+  for (int sl = 0; sl < S; ++sl) t += ws[((size_t)g * S + sl) * 2 * D + jd];
+  sums[i] = t;
+}
+
+// Time-dependent baseline (samplers/__init__.py:46-52): bin i of group g holds the float64 sum of q and the count
+// of the rows with time index i (lfb_index: the baseline's own rule), i.e. of the paths that reach i; G = 1 pools
+// every agent's rows, G = A keeps one set of bins per agent.  The envs are cut into tb_slices(G) fixed slices; a
+// thread owns one (group, slice, bin) and walks its slice's envs and their paths in order (madrl_paths_plan's
+// records), so each partial has one fixed order; the second pass sums them over the slices in ascending order and
+// the third writes mean = sum / count back to every row.  No atomics: same inputs, same bits.  Each thread scans
+// every path record of its slice for its one bin, so the work is O(L x paths), not O(rows): cheap while paths are
+// few per env, more when one env runs the whole horizon (L = T) while the others end often.
+#ifndef MADRL_TB_SLICES
+#define MADRL_TB_SLICES 32             // (the CPU emulator tests of tests/test_emulated_rltools.py build with fewer)
+#endif
+constexpr int kTbSlices = MADRL_TB_SLICES;
+constexpr int kTbThreads = 128;
+__host__ __device__ __forceinline__ int tb_slices(int G) { return (kTbSlices + G - 1) / G; }
+
+__global__ void time_baseline_partial_kernel(int T, int E, int A, int G, int L, const float* __restrict__ q,
+                                             const int32_t* __restrict__ n_ep, const int32_t* __restrict__ ep_rec,
+                                             const int32_t* __restrict__ t0, double* __restrict__ ws_sum,
+                                             int32_t* __restrict__ ws_cnt) {
+  const int LB = (L + kTbThreads - 1) / kTbThreads, S = tb_slices(G);
+  const int lb = (int)(blockIdx.x % LB), gs = (int)(blockIdx.x / LB), g = gs / S, sl = gs - g * S;
+  const int i = lb * kTbThreads + threadIdx.x;
+  if (i >= L) return;
+  const int e1 = (int)((int64_t)E * (sl + 1) / S);
+  double sum = 0.0;
+  int32_t cnt = 0;
+  for (int e = (int)((int64_t)E * sl / S); e < e1; ++e) {
+    const int n = n_ep[e];
+    for (int j = 0; j < n; ++j) {
+      const int32_t* rec = ep_rec + 3 * ((size_t)e * T + j);
+      const int pos = i - ((j == 0 && t0 != nullptr) ? t0[e] : 0);
+      if (pos < 0 || pos >= rec[1]) continue;
+      const float* qr = q + ((size_t)(rec[0] + pos) * E + e) * A;
+      if (G == 1) {
+        for (int a = 0; a < A; ++a) sum += (double)qr[a];
+        cnt += A;
+      } else {
+        sum += (double)qr[g];
+        cnt += 1;
+      }
+    }
+  }
+  ws_sum[(size_t)gs * L + i] = sum;
+  ws_cnt[(size_t)gs * L + i] = cnt;
+}
+
+__global__ void time_baseline_bins_kernel(int G, int L, const double* __restrict__ ws_sum,
+                                          const int32_t* __restrict__ ws_cnt, double* __restrict__ bin_sum,
+                                          int32_t* __restrict__ bin_cnt) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)G * L) return;
+  const int S = tb_slices(G);
+  const size_t g = i / L, b = i - g * L;
+  double sum = 0.0;
+  int32_t cnt = 0;
+  for (int sl = 0; sl < S; ++sl) {
+    sum += ws_sum[((size_t)g * S + sl) * L + b];
+    cnt += ws_cnt[((size_t)g * S + sl) * L + b];
+  }
+  bin_sum[i] = sum;
+  bin_cnt[i] = cnt;
+}
+
+// simplev[t][e][a] = the mean of its bin (nanmean's sum / count), float32.  A row whose index is past the L bins
+// (an L too small for the rollout) gets NaN rather than another bin's value.
+__global__ void time_baseline_apply_kernel(int T, int E, int A, int G, int L, const int32_t* __restrict__ seg_start,
+                                           const int32_t* __restrict__ t0, const double* __restrict__ bin_sum,
+                                           const int32_t* __restrict__ bin_cnt, float* __restrict__ simplev) {
+  const size_t r = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= (size_t)T * E * A) return;
+  const size_t te = r / A;
+  const int idx = lfb_index(te, E, seg_start, t0);
+  const size_t b = (G == 1 ? 0 : (r - te * A) * (size_t)L) + idx;
+  simplev[r] = (idx >= 0 && idx < L) ? (float)(bin_sum[b] / (double)bin_cnt[b]) : __int_as_float(0x7fc00000);
+}
+
 }  // namespace madrl
 
 using namespace madrl;
@@ -684,4 +813,75 @@ extern "C" int madrl_standardize_obs_terminal_bf16(int T, int E, size_t per_env,
                                                    double alpha, double eps, void* stream) {
   return standardize_obs_terminal(T, E, per_env, (uint16_t*)x_dev, (uint16_t*)term_dev, done_dev, mean_dev, var_dev,
                                   alpha, eps, stream);
+}
+
+template <typename O>
+static int running_moments(size_t R, int G, int D, size_t shift, const void* x_dev, const void* first_dev,
+                           double* sums_dev, double* ws_dev, void* stream) {
+  MADRL_REQUIRE(R >= 1 && D >= 1, "bad sizes");
+  MADRL_REQUIRE(G >= 1 && G <= MADRL_AGENTS_MAX, "groups must be in [1, %d], got %d", MADRL_AGENTS_MAX, G);
+  MADRL_REQUIRE(!first_dev || (shift >= 1 && shift <= R * G), "shift must be in [1, rows] with a first row block");
+  MADRL_REQUIRE(x_dev && sums_dev && ws_dev, "NULL buffer");
+  const size_t blocks = (size_t)((D + 31) / 32) * rm_slices(G) * G;
+  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many columns for one launch");
+  cudaStream_t s = (cudaStream_t)stream;
+  MADRL_LAUNCH(running_moments_partial_kernel<O>, (unsigned)blocks, kRmWarps * 32, 0, s, R, G, D, shift,
+               (const O*)x_dev, (const O*)first_dev, ws_dev);
+  const size_t n = (size_t)G * 2 * D;
+  MADRL_LAUNCH(running_moments_finalize_kernel, (unsigned)((n + 255) / 256), 256, 0, s, G, D, ws_dev, sums_dev);
+  g_launches.fetch_add(2);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_running_moments_workspace_size(int G, int D, size_t* bytes) {
+  MADRL_REQUIRE(G >= 1 && G <= MADRL_AGENTS_MAX && D >= 1, "bad sizes");
+  MADRL_REQUIRE(bytes, "NULL pointer");
+  *bytes = (size_t)rm_slices(G) * G * 2 * D * sizeof(double);
+  return MADRL_OK;
+}
+
+extern "C" int madrl_running_moments_f32(size_t R, int G, int D, size_t shift, const float* x_dev,
+                                         const float* first_dev, double* sums_dev, double* ws_dev, void* stream) {
+  return running_moments<float>(R, G, D, shift, x_dev, first_dev, sums_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_running_moments_bf16(size_t R, int G, int D, size_t shift, const void* x_dev,
+                                          const void* first_dev, double* sums_dev, double* ws_dev, void* stream) {
+  return running_moments<uint16_t>(R, G, D, shift, x_dev, first_dev, sums_dev, ws_dev, stream);
+}
+
+extern "C" int madrl_time_baseline_workspace_size(int G, int L, size_t* bytes) {
+  MADRL_REQUIRE(G >= 1 && G <= MADRL_AGENTS_MAX && L >= 1, "bad sizes");
+  MADRL_REQUIRE(bytes, "NULL pointer");
+  *bytes = (size_t)tb_slices(G) * G * L * (sizeof(double) + sizeof(int32_t));
+  return MADRL_OK;
+}
+
+extern "C" int madrl_time_baseline_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
+                                       const int32_t* seg_start_dev, const int32_t* n_ep_dev,
+                                       const int32_t* ep_rec_dev, const int32_t* t0_dev, double* bin_sum_dev,
+                                       int32_t* bin_count_dev, float* simplev_dev, void* ws_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && L >= 1, "bad sizes");
+  MADRL_REQUIRE((size_t)T * E * A < ((size_t)1 << 31), "T*E*A must be < 2^31");
+  MADRL_REQUIRE(!per_agent || A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
+  MADRL_REQUIRE(q_dev && seg_start_dev && n_ep_dev && ep_rec_dev && bin_sum_dev && bin_count_dev && simplev_dev &&
+                ws_dev, "NULL buffer");
+  const int G = per_agent ? A : 1, S = tb_slices(G);
+  const size_t part = (size_t)S * G * L;
+  double* ws_sum = (double*)ws_dev;
+  int32_t* ws_cnt = (int32_t*)(ws_sum + part);
+  cudaStream_t s = (cudaStream_t)stream;
+  const size_t blocks = (size_t)((L + kTbThreads - 1) / kTbThreads) * S * G;
+  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many bins for one launch");
+  MADRL_LAUNCH(time_baseline_partial_kernel, (unsigned)blocks, kTbThreads, 0, s, T, E, A, G, L, q_dev, n_ep_dev,
+               ep_rec_dev, t0_dev, ws_sum, ws_cnt);
+  const size_t nb = (size_t)G * L, rows = (size_t)T * E * A;
+  MADRL_LAUNCH(time_baseline_bins_kernel, (unsigned)((nb + 255) / 256), 256, 0, s, G, L, ws_sum, ws_cnt, bin_sum_dev,
+               bin_count_dev);
+  MADRL_LAUNCH(time_baseline_apply_kernel, (unsigned)((rows + 255) / 256), 256, 0, s, T, E, A, G, L, seg_start_dev,
+               t0_dev, bin_sum_dev, bin_count_dev, simplev_dev);
+  g_launches.fetch_add(3);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
 }

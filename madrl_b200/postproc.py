@@ -346,6 +346,13 @@ class LinearFeatureBaseline(object):
         self._coeffs = None
         self._carry = None
 
+    # The kernels' feature map: madrl_lfb_* (rllab's); a subclass with another map names its entry points and the
+    # extra arguments they take after the returns (normal equations) or t0 (predict).
+    _kernels = "lfb"
+
+    def _map_args(self):
+        return ()
+
     def _coef_shape(self):
         return (self.n_features,) if self.n_agents is None else (self.n_agents, self.n_features)
 
@@ -405,16 +412,16 @@ class LinearFeatureBaseline(object):
         nbytes = C.c_size_t()
         per_agent = self.n_agents is not None
         if per_agent:
-            _lib.check(L.madrl_lfb_agents_workspace_size(D, A, C.byref(nbytes)))
+            _lib.check(getattr(L, "madrl_%s_agents_workspace_size" % self._kernels)(D, A, C.byref(nbytes)))
         else:
-            _lib.check(L.madrl_lfb_workspace_size(D, C.byref(nbytes)))
+            _lib.check(getattr(L, "madrl_%s_workspace_size" % self._kernels)(D, C.byref(nbytes)))
         ws = torch.empty(nbytes.value // 8, dtype=torch.float64, device=self.device)
         Dc = self.n_features + 1
         G = torch.empty(((A,) if per_agent else ()) + (Dc, Dc), dtype=torch.float64, device=self.device)
-        fn = _obs_fn("lfb_normal_eq_agents" if per_agent else "lfb_normal_eq", obs.dtype)
+        fn = _obs_fn(self._kernels + ("_normal_eq_agents" if per_agent else "_normal_eq"), obs.dtype)
         with torch.cuda.device(self.device):
-            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(returns), _ptr(G),
-                          _ptr(ws), _lib.stream(self.device)))
+            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(returns),
+                          *self._map_args(), _ptr(G), _ptr(ws), _lib.stream(self.device)))
         return G
 
     def _host_lstsq(self, M, b):
@@ -474,10 +481,10 @@ class LinearFeatureBaseline(object):
         values = torch.empty((T, E, A), dtype=torch.float32, device=self.device)
         if self._coeffs is None:
             return values.zero_()
-        fn = _obs_fn("lfb_predict" if self.n_agents is None else "lfb_predict_agents", obs.dtype)
+        fn = _obs_fn(self._kernels + ("_predict" if self.n_agents is None else "_predict_agents"), obs.dtype)
         with torch.cuda.device(self.device):
-            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), _ptr(self._coeffs),
-                          _ptr(values), _lib.stream(self.device)))
+            _lib.check(fn(T, E, A, D, _ptr(obs), _ptr(obs_before), _ptr(seg_s), _ptr(t0), *self._map_args(),
+                          _ptr(self._coeffs), _ptr(values), _lib.stream(self.device)))
         return values
 
 
