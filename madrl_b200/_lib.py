@@ -96,102 +96,131 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
-def _declare_engines(lib):
-    """argtypes of the env families' entry points (madrl_{ww,pursuit,hostage}_*)."""
-    vp, i32, u64 = C.c_void_p, C.c_int, C.c_uint64
-    for fam, cfg, lay in (("ww", WWConfig, WWLayout), ("hostage", HWConfig, HWLayout),
-                          ("pursuit", PEConfig, PELayout)):
-        f = lambda name: getattr(lib, "madrl_%s_%s" % (fam, name))   # noqa: E731
-        f("state_layout").argtypes = [C.POINTER(cfg), C.POINTER(lay)]
-        # pursuit: the map pool comes before the state blob
-        f("create").argtypes = [C.POINTER(cfg)] + ([vp] if fam == "pursuit" else []) + [vp, C.POINTER(vp)]
-        f("destroy").argtypes = [vp]
-        f("state_ptr").argtypes = [vp]
-        f("state_ptr").restype = vp
-        f("seed").argtypes = [vp, u64, vp]
-        f("set_launch").argtypes = [vp, i32, i32]
-        f("set_terminal_obs").argtypes = [vp, vp]
-        f("reset").argtypes = [vp, vp, vp, vp]
-        f("rollout").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, vp]
-        f("step").argtypes = [vp, vp, vp, vp, vp, vp, i32, vp]
-        f("reset_host").argtypes = [vp, vp, vp]
-        f("rollout_host").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32]
-        f("rollout_host2").argtypes = [vp, i32, vp, vp, vp, vp, vp, i32, i32]
-        # absent from libraries built before the bfloat16 observation format (timed side by side by scripts/)
-        if hasattr(lib, "madrl_%s_set_obs_format" % fam):
-            f("set_obs_format").argtypes = [vp, i32]
-    if hasattr(lib, "madrl_ww_default_blocks_per_sm"):   # absent from older builds timed by scripts/
-        lib.madrl_ww_default_blocks_per_sm.argtypes = [vp, i32]
-    lib.madrl_ww_set_peers.argtypes = [vp, i32, i32, i32, C.POINTER(vp), C.POINTER(vp), C.POINTER(vp)]
-    lib.madrl_ww_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]
-    lib.madrl_pursuit_set_params.argtypes = [vp, C.c_double, C.c_double]
-    lib.madrl_pursuit_rollout_heuristic.argtypes = [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]
+def _signatures():
+    """(restype, argtypes) of every function of include/madrl_b200.h, grouped as the header groups them.
+    Every pointer is a c_void_p except the config / layout structs, the out-parameters callers pass with
+    byref (handles, sizes, device pointers), madrl_abi_sizes' array, and the error message and IPC handles
+    (bytes).  tests/test_abi_signatures_cpu.py checks the table against the header."""
+    vp, i32, sz, f64, u32, u64, P = C.c_void_p, C.c_int, C.c_size_t, C.c_double, C.c_uint32, C.c_uint64, C.POINTER
+    sig = {
+        "madrl_last_error": (C.c_char_p, []),
+        "madrl_version": (i32, []),
+        "madrl_abi_sizes": (None, [P(C.c_int32)]),
+        "madrl_launch_count": (u64, []),
+        "madrl_set_host_chunk_bytes": (None, [sz]),
+        # CUDA-IPC buffers
+        "madrl_ipc_alloc": (i32, [sz, P(vp), C.c_char_p]),
+        "madrl_ipc_open": (i32, [C.c_char_p, P(vp)]),
+        "madrl_ipc_close": (i32, [vp]),
+        "madrl_ipc_free": (i32, [vp]),
+        # stream-ordered primitives of the multi-GPU exchange
+        "madrl_stream_memops_available": (i32, []),
+        "madrl_copy_async": (i32, [vp, vp, sz, vp]),
+        "madrl_stream_write32": (i32, [vp, vp, u32]),
+        "madrl_stream_wait_geq32": (i32, [vp, vp, u32]),
+    }
+    # the env families: the same entry points apart from their structs, Pursuit's map pool and a few extras
+    for fam, cfg, lay in (("ww", WWConfig, WWLayout), ("pursuit", PEConfig, PELayout),
+                          ("hostage", HWConfig, HWLayout)):
+        pool = [vp] if fam == "pursuit" else []
+        sig.update(("madrl_%s_%s" % (fam, name), s) for name, s in (
+            ("state_layout", (i32, [P(cfg), P(lay)])),
+            ("create", (i32, [P(cfg)] + pool + [vp, P(vp)])),
+            ("destroy", (i32, [vp])),
+            ("state_ptr", (vp, [vp])),
+            ("seed", (i32, [vp, u64, vp])),
+            ("set_launch", (i32, [vp, i32, i32])),
+            ("set_terminal_obs", (i32, [vp, vp])),
+            ("set_obs_format", (i32, [vp, i32])),
+            ("reset", (i32, [vp, vp, vp, vp])),
+            ("rollout", (i32, [vp, i32, vp, vp, vp, vp, vp, i32, vp])),
+            ("step", (i32, [vp, vp, vp, vp, vp, vp, i32, vp])),
+            ("reset_host", (i32, [vp, vp, vp])),
+            ("rollout_host", (i32, [vp, i32, vp, vp, vp, vp, vp, i32])),
+            ("rollout_host2", (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32]))))
+    sig.update({
+        "madrl_ww_default_blocks_per_sm": (i32, [vp, i32]),
+        "madrl_ww_set_peers": (i32, [vp, i32, i32, i32, P(vp), P(vp), P(vp)]),
+        "madrl_ww_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
+        "madrl_pursuit_set_params": (i32, [vp, f64, f64]),
+        "madrl_pursuit_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        # hand-written policies
+        "madrl_ww_heuristic_actions": (i32, [i32, sz, i32, i32, vp, vp, vp]),
+        "madrl_pursuit_heuristic_actions": (i32, [sz, i32, i32, i32, i32, vp, vp, vp, vp, vp]),
+        # trajectory post-processing
+        "madrl_gae_f32": (i32, [i32, i32, i32, vp, vp, vp, vp, f64, f64, vp, vp, vp]),
+        "madrl_frame_stack_f32": (i32, [i32] * 5 + [vp] * 5),
+        "madrl_frame_stack_bf16": (i32, [i32] * 5 + [vp] * 5),
+        "madrl_standardize_f32": (i32, [i32, sz, vp, vp, vp, f64, f64, i32, f64, i32, vp]),
+        "madrl_standardize_bf16": (i32, [i32, sz, vp, vp, vp, f64, f64, i32, f64, i32, vp]),
+        "madrl_standardize_obs_terminal_f32": (i32, [i32, i32, sz] + [vp] * 5 + [f64, f64, vp]),
+        "madrl_standardize_obs_terminal_bf16": (i32, [i32, i32, sz] + [vp] * 5 + [f64, f64, vp]),
+        "madrl_episode_stats_f32": (i32, [i32, i32, i32, vp, vp, f64, i32, vp, vp, vp, vp, vp, vp]),
+        # moments and advantage centring
+        "madrl_moments_f32": (i32, [sz, vp, vp, vp, vp, vp]),
+        "madrl_center_advantages_f32": (i32, [sz, vp, i32, i32, vp, vp, vp]),
+        "madrl_moments_agents_f32": (i32, [sz, i32, vp, vp, vp, vp, vp]),
+        "madrl_center_advantages_agents_f32": (i32, [sz, i32, vp, i32, i32, vp, vp, vp]),
+        # path packing and padding
+        "madrl_paths_plan": (i32, [i32, i32, i32] + [vp] * 6),
+        "madrl_paths_pack_u32": (i32, [i32] * 4 + [vp] * 6),
+        "madrl_paths_pack_u16": (i32, [i32] * 4 + [vp] * 6),
+        "madrl_paths_pad_u32": (i32, [i32] * 6 + [vp] * 5),
+        "madrl_paths_pad_u16": (i32, [i32] * 6 + [vp] * 5),
+        "madrl_path_sums_f32": (i32, [i32] * 4 + [vp] * 6),
+        # rllab's linear feature baseline, pooled and per agent
+        "madrl_lfb_workspace_size": (i32, [i32, P(sz)]),
+        "madrl_lfb_normal_eq_f32": (i32, [i32] * 4 + [vp] * 8),
+        "madrl_lfb_normal_eq_bf16": (i32, [i32] * 4 + [vp] * 8),
+        "madrl_lfb_predict_f32": (i32, [i32] * 4 + [vp] * 7),
+        "madrl_lfb_predict_bf16": (i32, [i32] * 4 + [vp] * 7),
+        "madrl_lfb_agents_workspace_size": (i32, [i32, i32, P(sz)]),
+        "madrl_lfb_normal_eq_agents_f32": (i32, [i32] * 4 + [vp] * 8),
+        "madrl_lfb_normal_eq_agents_bf16": (i32, [i32] * 4 + [vp] * 8),
+        "madrl_lfb_predict_agents_f32": (i32, [i32] * 4 + [vp] * 7),
+        "madrl_lfb_predict_agents_bf16": (i32, [i32] * 4 + [vp] * 7),
+        # rltools' sample processing
+        "madrl_running_moments_workspace_size": (i32, [i32, i32, P(sz)]),
+        "madrl_running_moments_f32": (i32, [sz, i32, i32, sz] + [vp] * 5),
+        "madrl_running_moments_bf16": (i32, [sz, i32, i32, sz] + [vp] * 5),
+        "madrl_time_baseline_workspace_size": (i32, [i32, i32, P(sz)]),
+        "madrl_time_baseline_f32": (i32, [i32] * 5 + [vp] * 10),
+        # rltools' linear feature baseline
+        "madrl_lfbr_workspace_size": (i32, [i32, P(sz)]),
+        "madrl_lfbr_agents_workspace_size": (i32, [i32, i32, P(sz)]),
+    })
+    for ag in ("", "_agents"):
+        for dt in ("f32", "bf16"):
+            sig["madrl_lfbr_normal_eq%s_%s" % (ag, dt)] = (i32, [i32] * 4 + [vp] * 9)
+            sig["madrl_lfbr_predict%s_%s" % (ag, dt)] = (i32, [i32] * 4 + [vp] * 8)
+    return sig
 
 
-def _declare(lib):
-    vp, i32 = C.c_void_p, C.c_int
-    _declare_engines(lib)
-    lib.madrl_last_error.restype = C.c_char_p
-    lib.madrl_version.restype = C.c_int
-    lib.madrl_abi_sizes.argtypes = [C.POINTER(C.c_int32)]
-    lib.madrl_abi_sizes.restype = None
-    lib.madrl_launch_count.restype = C.c_uint64
-    lib.madrl_set_host_chunk_bytes.argtypes = [C.c_size_t]
-    lib.madrl_set_host_chunk_bytes.restype = None
-    lib.madrl_ipc_alloc.argtypes = [C.c_size_t, C.POINTER(vp), C.c_char_p]
-    lib.madrl_ipc_open.argtypes = [C.c_char_p, C.POINTER(vp)]
-    lib.madrl_ipc_close.argtypes = [vp]
-    lib.madrl_ipc_free.argtypes = [vp]
-    lib.madrl_stream_memops_available.restype = C.c_int
-    lib.madrl_copy_async.argtypes = [vp, vp, C.c_size_t, vp]
-    lib.madrl_stream_write32.argtypes = [vp, vp, C.c_uint32]
-    lib.madrl_stream_wait_geq32.argtypes = [vp, vp, C.c_uint32]
-    lib.madrl_ww_heuristic_actions.argtypes = [i32, C.c_size_t, i32, i32, vp, vp, vp]
-    lib.madrl_pursuit_heuristic_actions.argtypes = [C.c_size_t, i32, i32, i32, i32, vp, vp, vp, vp, vp]
-    lib.madrl_gae_f32.argtypes = [i32, i32, i32, vp, vp, vp, vp, C.c_double, C.c_double, vp, vp, vp]
-    lib.madrl_frame_stack_f32.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
-    lib.madrl_standardize_f32.argtypes = [i32, C.c_size_t, vp, vp, vp, C.c_double, C.c_double, i32,
-                                          C.c_double, i32, vp]
-    lib.madrl_episode_stats_f32.argtypes = [i32, i32, i32, vp, vp, C.c_double, i32, vp, vp, vp, vp, vp, vp]
-    lib.madrl_standardize_obs_terminal_f32.argtypes = [i32, i32, C.c_size_t, vp, vp, vp, vp, vp, C.c_double, C.c_double, vp]
-    lib.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    lib.madrl_paths_pack_u32.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    lib.madrl_moments_f32.argtypes = [C.c_size_t, vp, vp, vp, vp, vp]
-    lib.madrl_center_advantages_f32.argtypes = [C.c_size_t, vp, i32, i32, vp, vp, vp]
-    if hasattr(lib, "madrl_frame_stack_bf16"):   # bfloat16 observation passes (absent from older builds)
-        lib.madrl_frame_stack_bf16.argtypes = lib.madrl_frame_stack_f32.argtypes
-        lib.madrl_standardize_bf16.argtypes = lib.madrl_standardize_f32.argtypes
-        lib.madrl_standardize_obs_terminal_bf16.argtypes = lib.madrl_standardize_obs_terminal_f32.argtypes
-        lib.madrl_paths_pack_u16.argtypes = lib.madrl_paths_pack_u32.argtypes
-    if hasattr(lib, "madrl_lfb_normal_eq_f32"):  # linear feature baseline (absent from older builds)
-        lib.madrl_lfb_workspace_size.argtypes = [i32, C.POINTER(C.c_size_t)]
-        for dt in ("f32", "bf16"):
-            getattr(lib, "madrl_lfb_normal_eq_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
-            getattr(lib, "madrl_lfb_predict_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
-    if hasattr(lib, "madrl_lfb_normal_eq_agents_f32"):  # per-agent baselines (absent from older builds)
-        lib.madrl_lfb_agents_workspace_size.argtypes = [i32, i32, C.POINTER(C.c_size_t)]
-        for dt in ("f32", "bf16"):
-            getattr(lib, "madrl_lfb_normal_eq_agents_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
-            getattr(lib, "madrl_lfb_predict_agents_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
-        lib.madrl_moments_agents_f32.argtypes = [C.c_size_t, i32, vp, vp, vp, vp, vp]
-        lib.madrl_center_advantages_agents_f32.argtypes = [C.c_size_t, i32, vp, i32, i32, vp, vp, vp]
-    if hasattr(lib, "madrl_paths_pad_u32"):    # padded paths of the recurrent sample batch (absent from older builds)
-        lib.madrl_paths_pad_u32.argtypes = [i32] * 6 + [vp] * 5
-        lib.madrl_paths_pad_u16.argtypes = lib.madrl_paths_pad_u32.argtypes
-        lib.madrl_path_sums_f32.argtypes = [i32] * 4 + [vp] * 6
-    if hasattr(lib, "madrl_time_baseline_f32"):  # rltools' sample processing (absent from older builds)
-        sz = C.c_size_t
-        lib.madrl_running_moments_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
-        lib.madrl_running_moments_f32.argtypes = [sz, i32, i32, sz] + [vp] * 5
-        lib.madrl_running_moments_bf16.argtypes = lib.madrl_running_moments_f32.argtypes
-        lib.madrl_time_baseline_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
-        lib.madrl_time_baseline_f32.argtypes = [i32] * 5 + [vp] * 10
-        lib.madrl_lfbr_workspace_size.argtypes = [i32, C.POINTER(sz)]
-        lib.madrl_lfbr_agents_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
-        for dt in ("f32", "bf16"):
-            for ag in ("", "_agents"):
-                getattr(lib, "madrl_lfbr_normal_eq%s_%s" % (ag, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 9
-                getattr(lib, "madrl_lfbr_predict%s_%s" % (ag, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 8
+SIGNATURES = _signatures()
+
+
+def declare(lib):
+    """Set restype and argtypes of every SIGNATURES function `lib` exports.  Absent ones are skipped, so that
+    MADRL_B200_LIB can load libraries built before an entry point existed (timed side by side by scripts/)."""
+    for name, (restype, argtypes) in SIGNATURES.items():
+        f = getattr(lib, name, None)
+        if f is not None:
+            f.restype, f.argtypes = restype, argtypes
+
+
+# The env families' entry points are part of the full table now; test drivers written against the former
+# engine-only declaration call it under this name.
+_declare_engines = declare
+
+
+def check_struct_sizes(lib, path):
+    """Raise EngineError unless `lib` was compiled with the config / layout structs this binding declares."""
+    sizes = (C.c_int32 * 6)()
+    lib.madrl_abi_sizes(sizes)
+    want = [C.sizeof(t) for t in (WWConfig, WWLayout, PEConfig, PELayout, HWConfig, HWLayout)]
+    if list(sizes) != want:
+        raise EngineError("%s was built against another include/madrl_b200.h: struct sizes %s, this "
+                          "binding expects %s" % (path, list(sizes), want))
 
 
 def lib():
@@ -210,13 +239,8 @@ def lib():
             lib_ = C.CDLL(path)
         except OSError as e:
             raise EngineError("cannot load %s: %s" % (path, e))
-        _declare(lib_)
-        sizes = (C.c_int32 * 6)()
-        lib_.madrl_abi_sizes(sizes)
-        want = [C.sizeof(t) for t in (WWConfig, WWLayout, PEConfig, PELayout, HWConfig, HWLayout)]
-        if list(sizes) != want:
-            raise EngineError("%s was built against another include/madrl_b200.h: struct sizes %s, this "
-                              "binding expects %s" % (path, list(sizes), want))
+        declare(lib_)
+        check_struct_sizes(lib_, path)
         _lib = lib_
     return _lib
 

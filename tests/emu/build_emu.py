@@ -1,6 +1,6 @@
-"""TEST INFRASTRUCTURE: compile the env kernels of madrl_b200/csrc with g++ against the fake
+"""TEST INFRASTRUCTURE: compile the kernels of madrl_b200/csrc with g++ against the fake
 <cuda_runtime.h> of tests/emu/include into a CPU library with the product's C ABI
-(tests/emu/_build/libmadrl_b200_emu[_<tag>].so).  Used only by tests/test_emulated_kernels.py."""
+(tests/emu/_build/libmadrl_b200_emu_<tag>.so), loaded by tests/emu/driver.py."""
 import hashlib
 import os
 import subprocess
@@ -11,10 +11,15 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 CSRC = os.path.join(ROOT, "madrl_b200", "csrc")
 OUT = os.path.join(HERE, "_build")
-SOURCES = ["common.cu", "waterworld.cu", "pursuit.cu", "hostage.cu", "postproc.cu", "heuristics.cu"]
-# postproc.cu: its shared arrays are block-static, not `extern`; the fixed reduction grid (528 blocks of
-# 256 threads on the GPU) is narrowed so that a launch does not create 150 000 fibers
-PER_FILE_FLAGS = {"postproc.cu": ["-D__shared__=static", "-DMADRL_MOM_BLOCKS=6"]}
+# every csrc/*.cu but exchange.cu, which needs the CUDA driver API
+SOURCES = ["common.cu", "waterworld.cu", "pursuit.cu", "hostage.cu", "postproc.cu", "heuristics.cu", "baseline.cu"]
+# The fixed reduction grids of postproc.cu and baseline.cu (on the GPU: 528 moment blocks of 256 threads, 64, 32
+# and 48 row slices), narrowed so that a launch does not create a hundred thousand fibers.  Tests that put their
+# sizes at the grids' edges read them here.
+GRID = {"MADRL_MOM_BLOCKS": 6, "MADRL_RM_SLICES": 3, "MADRL_TB_SLICES": 3, "MADRL_LFB_SLICES": 3}
+# the shared arrays of these two files are block-static, not `extern`
+PER_FILE_FLAGS = {f: ["-D__shared__=static"] + ["-D%s=%d" % kv for kv in GRID.items()]
+                  for f in ("postproc.cu", "baseline.cu")}
 CXXFLAGS = ["-std=c++17", "-O1", "-g", "-fPIC", "-Wno-unknown-pragmas", "-Wno-attributes", "-x", "c++",
             "-I", os.path.join(HERE, "include")]
 
@@ -46,9 +51,11 @@ def build(defines=(), force=False):
         return obj
 
     srcs = [os.path.join(CSRC, s) for s in SOURCES] + [os.path.join(HERE, "emu_runtime.cpp")]
-    with ThreadPoolExecutor(max_workers=6) as pool:
+    with ThreadPoolExecutor(max_workers=len(srcs)) as pool:
         objs = list(pool.map(one, srcs))
-    subprocess.check_call([cxx, "-shared", "-o", lib] + objs)
+    tmp = lib + ".%d.tmp" % os.getpid()
+    subprocess.check_call([cxx, "-shared", "-o", tmp] + objs)
+    os.replace(tmp, lib)
     return lib
 
 

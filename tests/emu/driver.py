@@ -1,13 +1,17 @@
 """TEST INFRASTRUCTURE: ctypes drivers for the warp-emulator build of the kernels
-(tests/emu/build_emu.py).  The emulator library exports the product's C ABI; "device" pointers are
-host pointers, so the entry points are called directly with NumPy arrays.  The engines take the
-arguments of madrl_b200.{waterworld,pursuit,hostage}.Batched* and build their config structs with the
-same functions (ww_config / pe_config / hw_config), so the tests read like the GPU ones and check the
-product's argument mapping.
+(tests/emu/build_emu.py).  The emulator library exports the product's C ABI and is declared with the
+product's signature table (madrl_b200/_lib.py); "device" pointers are host pointers, so the entry points
+are called directly with NumPy arrays.  The engines take the arguments of
+madrl_b200.{waterworld,pursuit,hostage}.Batched* and build their config structs with the same functions
+(ww_config / pe_config / hw_config), so the tests read like the GPU ones and check the product's argument
+mapping.
 """
 import ctypes as C
+import os
+import shutil
 
 import numpy as np
+import pytest
 
 from madrl_b200 import _lib as L
 from madrl_b200.hostage import hw_config
@@ -18,13 +22,23 @@ from . import build_emu
 
 _libs = {}
 
+needs_cxx = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
+
+
+def open_lib(path):
+    """The emulator library at `path`, declared as the product library is."""
+    lib = C.CDLL(path)
+    L.declare(lib)
+    L.check_struct_sizes(lib, path)
+    lib.madrl_emu_race_count.restype = C.c_long
+    lib.madrl_emu_race_reset.restype = None
+    return lib
+
 
 def load(defines=()):
     key = tuple(sorted(defines))
     if key not in _libs:
-        lib = C.CDLL(build_emu.build(list(key)))
-        _declare(lib)
-        _libs[key] = lib
+        _libs[key] = open_lib(build_emu.build(list(key)))
     return _libs[key]
 
 
@@ -39,14 +53,18 @@ def races(reset=True):
     return n
 
 
-def _declare(lib):
-    L._declare_engines(lib)
-    lib.madrl_last_error.restype = C.c_char_p
-    lib.madrl_emu_race_count.restype = C.c_long
-
-
-def _p(a):
+def ptr(a):
+    """A NumPy array's address as a pointer argument (None -> NULL)."""
     return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
+
+
+def paths_plan(lib, done, A):
+    """madrl_paths_plan of done uint8 [T, E] -> (seg_start, seg_len, n_episodes, ep_rec)."""
+    T, E = done.shape
+    seg_s, seg_l = np.full((T, E), -1, np.int32), np.full((T, E), -1, np.int32)
+    n_ep, ep_rec = np.zeros(E, np.int32), np.zeros((E, T, 3), np.int32)
+    assert lib.madrl_paths_plan(T, E, A, ptr(done), ptr(seg_s), ptr(seg_l), ptr(n_ep), ptr(ep_rec), None) == 0
+    return seg_s, seg_l, n_ep, ep_rec
 
 
 GUARD = 1 << 16   # bytes of canary on either side of every output buffer
@@ -84,7 +102,7 @@ class _Engine(object):
         self.obs_dim = int(self.layout.obs_dim)
         self.blob = np.zeros(int(self.layout.total_bytes), np.uint8)
         h = C.c_void_p()
-        self._check(self._f("create")(C.byref(self.cfg), *create_args, _p(self.blob), C.byref(h)))
+        self._check(self._f("create")(C.byref(self.cfg), *create_args, ptr(self.blob), C.byref(h)))
         self._h = h
 
     def __del__(self):
@@ -105,7 +123,7 @@ class _Engine(object):
     def reset(self, mask=None):
         obs = Guarded((self.n_envs, self.n_agents, self.obs_dim), self.obs_dtype, 0)
         m = None if mask is None else np.ascontiguousarray(mask, np.uint8)
-        self._check(self._f("reset")(self._h, _p(m), _p(obs.arr), None))
+        self._check(self._f("reset")(self._h, ptr(m), ptr(obs.arr), None))
         return obs.check("obs")
 
     def rollout(self, actions, auto_reset=True, host=False):
@@ -114,11 +132,11 @@ class _Engine(object):
         E, A = self.n_envs, self.n_agents
         bufs = [Guarded((T, E, A, self.obs_dim), self.obs_dtype, np.nan), Guarded((T, E, A), self.obs_dtype, np.nan),
                 Guarded((T, E), np.uint8, 255), Guarded((T, E) + self.info_shape, np.int32, -1)]
-        ptrs = [_p(b.arr) for b in bufs]
+        ptrs = [ptr(b.arr) for b in bufs]
         if host:
-            self._check(self._f("rollout_host")(self._h, T, _p(actions), *ptrs, int(auto_reset)))
+            self._check(self._f("rollout_host")(self._h, T, ptr(actions), *ptrs, int(auto_reset)))
         else:
-            self._check(self._f("rollout")(self._h, T, _p(actions), *ptrs, int(auto_reset), None))
+            self._check(self._f("rollout")(self._h, T, ptr(actions), *ptrs, int(auto_reset), None))
         return tuple(b.check(n) for b, n in zip(bufs, ("obs", "rew", "done", "info")))
 
 
@@ -130,20 +148,19 @@ class _Engine(object):
         bufs = [Guarded((T, E, A) + self.act_shape, self.act_dtype, -7),
                 Guarded((T, E, A, self.obs_dim), self.obs_dtype, np.nan), Guarded((T, E, A), self.obs_dtype, np.nan),
                 Guarded((T, E), np.uint8, 255), Guarded((T, E) + self.info_shape, np.int32, -1)]
-        ptrs = [_p(b.arr) for b in bufs]
+        ptrs = [ptr(b.arr) for b in bufs]
         extra = [int(bool(kw.get("py2_division", True)))] if self.fam == "pursuit" else []
-        self._check(self._f("rollout_heuristic")(self._h, T, _p(obs0), *ptrs, int(auto_reset), *extra, None))
+        self._check(self._f("rollout_heuristic")(self._h, T, ptr(obs0), *ptrs, int(auto_reset), *extra, None))
         return tuple(b.check(n) for b, n in zip(bufs, ("actions", "obs", "rew", "done", "info")))
 
 
 def ww_heuristic_actions(obs, n_sensors, defines=()):
     """madrl_ww_heuristic_actions through the emulator: obs [n, D] float32 / float64 -> actions [n, 2]."""
     lib = load(defines)
-    lib.madrl_ww_heuristic_actions.argtypes = [C.c_int, C.c_size_t, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
     obs = np.ascontiguousarray(obs)
     out = Guarded((obs.shape[0], 2), obs.dtype, np.nan)
-    rc = lib.madrl_ww_heuristic_actions(int(obs.dtype == np.float64), obs.shape[0], n_sensors, obs.shape[1], _p(obs),
-                                        _p(out.arr), None)
+    rc = lib.madrl_ww_heuristic_actions(int(obs.dtype == np.float64), obs.shape[0], n_sensors, obs.shape[1], ptr(obs),
+                                        ptr(out.arr), None)
     assert rc == 0, lib.madrl_last_error().decode()
     return out.check("actions")
 
@@ -151,13 +168,12 @@ def ww_heuristic_actions(obs, n_sensors, defines=()):
 def pursuit_heuristic_actions(obs, obs_range, flatten, fallback, py2_division=True, defines=()):
     """madrl_pursuit_heuristic_actions through the emulator: obs [n, D] float32 -> actions [n] int32."""
     lib = load(defines)
-    lib.madrl_pursuit_heuristic_actions.argtypes = [C.c_size_t] + [C.c_int] * 4 + [C.c_void_p] * 5
     obs = np.ascontiguousarray(obs, np.float32)
     fb = np.ascontiguousarray(fallback, np.int32)
     lut = np.zeros(128, np.uint8)
     out = Guarded((obs.shape[0],), np.int32, -9)
     rc = lib.madrl_pursuit_heuristic_actions(obs.shape[0], obs_range, int(flatten), obs.shape[1], int(py2_division),
-                                             _p(obs), _p(fb), _p(lut), _p(out.arr), None)
+                                             ptr(obs), ptr(fb), ptr(lut), ptr(out.arr), None)
     assert rc == 0, lib.madrl_last_error().decode()
     return out.check("actions")
 
@@ -215,7 +231,7 @@ class EmuPursuit(_Engine):
         self.cfg = pe_config(n_envs, self.map_pool, *args, **kw)
         self.n_envs, self.n_pursuers, self.n_evaders = n_envs, self.cfg.n_pursuers, self.cfg.n_evaders
         self.n_agents = self.n_pursuers
-        self._finish((_p(self.map_pool),))
+        self._finish((ptr(self.map_pool),))
 
     def state(self, e):
         Ly, E, Np = self.layout, self.n_envs, self.n_pursuers

@@ -18,12 +18,9 @@ sys.path.insert(0, ROOT)
 CODE = r'''
 import sys
 sys.path.insert(0, %(tests)r); sys.path.insert(0, %(root)r)
-import ctypes as C
 from emu import driver
 import test_emulated_kernels as T
-lib = C.CDLL(%(lib)r)
-driver._declare(lib)
-driver._libs[tuple(sorted(T.VARIANTS[%(variant)r]))] = lib
+driver._libs[tuple(sorted(T.VARIANTS[%(variant)r]))] = driver.open_lib(%(lib)r)
 import pytest
 sys.exit(pytest.main([%(testfile)r, %(heurfile)r, "-x", "-q", "-k", %(variant)r + " or policy or generator or closed_loop",
                       "-p", "no:cacheprovider"]))

@@ -5,12 +5,15 @@ warp emulator of tests/emu against the oracle, and the argument validation and h
 madrl_b200.postproc."""
 import ctypes as C
 import os
-import shutil
 
 import numpy as np
 import pytest
 import torch
 
+import postproc_edges as pe
+from emu import driver
+from emu.driver import needs_cxx
+from emu.driver import ptr as _p
 from oracle import baseline_oracle as bo
 from oracle import concurrent_baseline_oracle as cbo
 from oracle import postproc_oracle as po
@@ -18,7 +21,6 @@ from oracle import postproc_oracle as po
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "linear_baseline_concurrent_ref.npz")
 CASES = ("ragged", "beyond_clip")
 FLAVOURS = ("independent", "shared")
-have_cxx = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
 
 
 def _golden():
@@ -105,86 +107,14 @@ def test_golden_cases_cover_agents_ragged_paths_constants_and_clipping():
 
 # ---------------------------------------------------------------- the kernels in the warp emulator
 
-def _p(a):
-    return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
-
-
-# As tests/test_linear_baseline_cpu.py: an emulator library of the sources the passes need, with block-static
-# shared arrays, 3 row slices instead of 48 and 6 moment blocks instead of 528 (fewer fibers per launch).
-EMU_SOURCES = {"common.cu": [], "postproc.cu": ["-D__shared__=static", "-DMADRL_MOM_BLOCKS=6"],
-               "baseline.cu": ["-D__shared__=static", "-DMADRL_LFB_SLICES=3"]}
-
-
-def _build_emu_lib():
-    import subprocess
-    from concurrent.futures import ThreadPoolExecutor
-    from emu import build_emu as be
-    out = os.path.join(be.OUT, "libmadrl_b200_emu_lfb_agents.so")
-    deps = be._deps() + [os.path.abspath(__file__)]
-    if os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
-        return out
-    objdir = os.path.join(be.OUT, "obj_lfb_agents")
-    os.makedirs(objdir, exist_ok=True)
-    cxx = os.environ.get("CXX", "g++")
-    srcs = [(os.path.join(be.CSRC, f), fl) for f, fl in EMU_SOURCES.items()] + [(os.path.join(be.HERE, "emu_runtime.cpp"), [])]
-
-    def one(job):
-        src, flags = job
-        obj = os.path.join(objdir, os.path.basename(src) + ".o")
-        res = subprocess.run([cxx] + be.CXXFLAGS + flags + ["-c", "-o", obj, src], stdout=subprocess.PIPE,
-                             stderr=subprocess.STDOUT, text=True)
-        assert res.returncode == 0, res.stdout
-        return obj
-    with ThreadPoolExecutor(max_workers=4) as pool:
-        objs = list(pool.map(one, srcs))
-    tmp = out + ".%d.tmp" % os.getpid()
-    subprocess.check_call([cxx, "-shared", "-o", tmp] + objs)
-    os.replace(tmp, out)
-    return out
-
-
-def _races(L):
-    n = int(L.madrl_emu_race_count())
-    L.madrl_emu_race_reset()
-    return n
-
-
 @pytest.fixture(scope="module")
 def lib():
-    L = C.CDLL(_build_emu_lib())
-    L.madrl_emu_race_count.restype = C.c_long
-    vp, i32, sz = C.c_void_p, C.c_int, C.c_size_t
-    L.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_lfb_workspace_size.argtypes = [i32, C.POINTER(sz)]
-    L.madrl_lfb_agents_workspace_size.argtypes = [i32, i32, C.POINTER(sz)]
-    for dt in ("f32", "bf16"):
-        for kind in ("", "agents_"):
-            getattr(L, "madrl_lfb_normal_eq_%s%s" % (kind, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 8
-            getattr(L, "madrl_lfb_predict_%s%s" % (kind, dt)).argtypes = [i32, i32, i32, i32] + [vp] * 7
-    L.madrl_moments_f32.argtypes = [sz, vp, vp, vp, vp, vp]
-    L.madrl_center_advantages_f32.argtypes = [sz, vp, i32, i32, vp, vp, vp]
-    L.madrl_moments_agents_f32.argtypes = [sz, i32, vp, vp, vp, vp, vp]
-    L.madrl_center_advantages_agents_f32.argtypes = [sz, i32, vp, i32, i32, vp, vp, vp]
-    return L
-
-
-def _bf16_bits(x):
-    u = x.astype(np.float32).view(np.uint32).astype(np.uint64)
-    b = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
-    return b, (b.astype(np.uint32) << 16).view(np.float32)
-
-
-def _seg_start(lib, done, A):
-    T, E = done.shape
-    seg_s, seg_l = np.empty((T, E), np.int32), np.empty((T, E), np.int32)
-    n_ep, ep_rec = np.empty(E, np.int32), np.empty((E, T, 3), np.int32)
-    assert lib.madrl_paths_plan(T, E, A, _p(done), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
-    return seg_s
+    return driver.load(())
 
 
 def _run(lib, obs, obs_before, done, ret, t0, coef, bf16, per_agent):
     T, E, A, D = obs.shape
-    seg_s = _seg_start(lib, done, A)
+    seg_s = driver.paths_plan(lib, done, A)[0]
     nbytes = C.c_size_t()
     if per_agent:
         assert lib.madrl_lfb_agents_workspace_size(D, A, C.byref(nbytes)) == 0
@@ -211,7 +141,7 @@ EMU_SHAPES = [  # T, E, A, D, p_done, obs_before, t0
 ]
 
 
-@have_cxx
+@needs_cxx
 @pytest.mark.parametrize("shape", EMU_SHAPES, ids=lambda s: "T%dE%dA%dD%d%s%s" % (s[:4] + ("_before" if s[5] else "",
                                                                                           "_t0" if s[6] else "")))
 def test_emulated_agent_kernels_match_oracle(lib, shape):
@@ -225,7 +155,7 @@ def test_emulated_agent_kernels_match_oracle(lib, shape):
     ret = rs.randn(T, E, A).astype(np.float32)
     t0 = rs.randint(0, 300, size=E).astype(np.int32) if with_t0 else None
     coef = rs.randn(A, 2 * D + 4)
-    _races(lib)
+    driver.races()
     G, vals = _run(lib, obs, obs_before, done, ret, t0, coef, False, True)
     F = cbo.agent_features(obs, done, obs_before, t0)
     for a in range(A):
@@ -237,15 +167,15 @@ def test_emulated_agent_kernels_match_oracle(lib, shape):
         tol = np.spacing(np.abs(want.astype(np.float32))) + 1e-12 * np.abs(F[a] * coef[a]).sum(axis=1)
         assert np.all(np.abs(vals[:, :, a].reshape(-1).astype(np.float64) - want) <= tol)
     # bfloat16 observations: the call on the widened float32 input, bit for bit
-    o, o_w = _bf16_bits(obs)
-    ob, ob_w = _bf16_bits(obs_before) if with_before else (None, None)
+    o, o_w = pe.bf16_bits(obs)
+    ob, ob_w = pe.bf16_bits(obs_before) if with_before else (None, None)
     for x, y in zip(_run(lib, o, ob, done, ret, t0, coef, True, True), _run(lib, o_w, ob_w, done, ret, t0, coef,
                                                                             False, True)):
         assert np.array_equal(x, y)
-    assert _races(lib) == 0
+    assert driver.races() == 0
 
 
-@have_cxx
+@needs_cxx
 @pytest.mark.parametrize("bf16", [False, True], ids=["f32", "bf16"])
 def test_emulated_one_agent_equals_pooled_bitwise(lib, bf16):
     rs = np.random.RandomState(5)
@@ -253,7 +183,7 @@ def test_emulated_one_agent_equals_pooled_bitwise(lib, bf16):
     obs = (rs.randn(T, E, 1, D) * 6).astype(np.float32)
     obs_before = (rs.randn(E, 1, D) * 6).astype(np.float32)
     if bf16:
-        obs, obs_before = _bf16_bits(obs)[0], _bf16_bits(obs_before)[0]
+        obs, obs_before = pe.bf16_bits(obs)[0], pe.bf16_bits(obs_before)[0]
     done = (rs.rand(T, E) < 0.2).astype(np.uint8)
     ret = rs.randn(T, E, 1).astype(np.float32)
     t0 = rs.randint(0, 50, size=E).astype(np.int32)
@@ -277,10 +207,10 @@ def test_emulated_one_agent_equals_pooled_bitwise(lib, bf16):
         assert lib.madrl_center_advantages_agents_f32(x_a.size, 1, _p(x_a), center, positive, _p(stats_a), _p(ws),
                                                       None) == 0
         assert np.array_equal(x_a, x_p)
-    assert _races(lib) == 0
+    assert driver.races() == 0
 
 
-@have_cxx
+@needs_cxx
 @pytest.mark.parametrize("A", [1, 3, 7])
 def test_emulated_agent_moments_and_centring(lib, A):
     rs = np.random.RandomState(A)
@@ -288,7 +218,7 @@ def test_emulated_agent_moments_and_centring(lib, A):
     a = (rs.randn(rows, A) * np.arange(1, A + 1) + np.arange(A) * 3).astype(np.float32)
     b = (a + rs.randn(rows, A)).astype(np.float32)
     stats, ws = np.empty((A, 9)), np.empty(4096 * A)
-    _races(lib)
+    driver.races()
     assert lib.madrl_moments_agents_f32(rows, A, _p(a), _p(b), _p(stats), _p(ws), None) == 0
     for c in range(A):
         s = [a[:, c].astype(np.float64), b[:, c].astype(np.float64)]
@@ -308,10 +238,10 @@ def test_emulated_agent_moments_and_centring(lib, A):
             if positive:
                 want = po.shift_advantages_to_positive(want)
             assert np.all(np.abs(x[:, c] - want) <= np.spacing(np.abs(want).astype(np.float32)) + 1e-12), c
-    assert _races(lib) == 0
+    assert driver.races() == 0
 
 
-@have_cxx
+@needs_cxx
 def test_emulated_agent_workspace_and_bad_sizes(lib):
     nbytes = C.c_size_t()
     assert lib.madrl_lfb_agents_workspace_size(213, 5, C.byref(nbytes)) == 0

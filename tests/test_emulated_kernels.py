@@ -5,18 +5,20 @@ the kernels and of the host launch code without a GPU, for the default build and
 experiment flags that are still off in the product; the `-m gpu` tests remain the parity proof of
 what nvcc makes of the same source.  Nothing in madrl_b200/ can load the emulator library."""
 import os
-import shutil
 
 import numpy as np
 import pytest
 
 from conftest import ROOT
+from emu import driver
+from emu.driver import Guarded
+from emu.driver import ptr as _p
 from oracle.hostage_oracle import HostageOracle
 from oracle.philox import Stream
 from oracle.pursuit_oracle import PursuitOracle
 from oracle.waterworld_oracle import WaterworldOracle
 
-pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
+pytestmark = driver.needs_cxx
 
 # build variants: the product defaults
 VARIANTS = {"default": ()}
@@ -33,7 +35,6 @@ def f32(x):
 def no_shared_memory_hazards():
     """Every emulated launch is also race-checked: two lanes touching the same shared-memory byte,
     one of them writing, without a __syncwarp / __syncthreads in between, fail the test."""
-    from emu import driver
     driver.races()
     yield
     assert driver.races() == 0, "shared-memory hazard reported by the emulator (see stderr)"
@@ -520,7 +521,6 @@ def test_host_code_validation_seed_and_curriculum_knobs():
     through madrl_last_error; seed() re-keys the stream and restarts the counters; Pursuit's
     set_params (catchr, constraint_window: the curriculum knobs of pursuit_evade.py:264-272) takes
     effect at the next step / reset."""
-    import ctypes as C
     from emu.driver import EmuPursuit, EmuWaterworld
     with pytest.raises(RuntimeError, match="n_pursuers"):
         EmuWaterworld(4, 40, 5)
@@ -543,7 +543,6 @@ def test_host_code_validation_seed_and_curriculum_knobs():
     maps = small_map()
     cfg = dict(n_evaders=4, n_pursuers=6, obs_range=3, surround=True, reward_mech='local', catchr=0.1, term_pursuit=5.0)
     pe = EmuPursuit(2, maps, seed=3, **cfg)
-    lib.madrl_pursuit_set_params.argtypes = [C.c_void_p, C.c_double, C.c_double]
     assert lib.madrl_pursuit_set_params(pe._h, 0.25, 1.0) == 0
     pe.reset()
     act = np.random.RandomState(0).randint(0, 5, size=(6, 2, 6)).astype(np.int32)
@@ -607,8 +606,6 @@ def test_waterworld_fused_peer_gather_layout(variant):
     for rank in range(n_ranks):
         eng = EmuWaterworld(E, seed=8, env_id_base=rank * E, max_path_length=9, defines=VARIANTS[variant], **cfg)
         arr = lambda k: (C.c_void_p * 2)(*[d[k].ctypes.data for d in dests])   # noqa: E731
-        eng.lib.madrl_ww_set_peers.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p),
-                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]
         assert eng.lib.madrl_ww_set_peers(eng._h, 2, rank, t_max, arr('rew'), arr('done'), arr('info')) == 0
         eng.reset()
         act = np.random.RandomState(rank).randn(T, E, 5, 2) * 0.5
@@ -680,8 +677,7 @@ def test_random_configurations_with_horizon_and_auto_reset(variant, case):
 def test_host_entry_points_equal_device_entry_points():
     """*_reset_host / *_rollout_host (staging copies inside the library) against the device-pointer
     entry points, Pursuit and Hostage (Waterworld: see the auto-reset test above)."""
-    import ctypes as C
-    from emu.driver import EmuHostage, EmuPursuit, Guarded, _p
+    from emu.driver import EmuHostage, EmuPursuit
     maps = pool16()
     mk = [lambda: EmuPursuit(4, maps, seed=3, max_path_length=6, **C3),
           lambda: EmuHostage(4, 10, 16, 16, 4, 2, seed=3, max_path_length=6, fp64=False)]
@@ -701,8 +697,7 @@ def test_pipelined_host_rollout_chunks_and_obs_last_mode():
     """csrc/host_pipeline.cuh: the host-buffer rollout cut into several chunks (chunk size forced down)
     must equal the single device launch for every family, and MADRL_HOST_OBS_LAST returns rewards /
     dones / infos of every step + only the last step's observations."""
-    import ctypes as C
-    from emu.driver import EmuHostage, EmuPursuit, EmuWaterworld, Guarded, _p
+    from emu.driver import EmuHostage, EmuPursuit, EmuWaterworld
     maps = pool16()
     mk = [lambda: EmuWaterworld(3, seed=4, max_path_length=7, fp64=False, **WW["c2"]),
           lambda: EmuPursuit(3, maps, seed=4, max_path_length=7, **C3),
@@ -721,7 +716,6 @@ def test_pipelined_host_rollout_chunks_and_obs_last_mode():
             for x, y in zip(ref, b.rollout(act, host=True)):
                 assert np.array_equal(x, y)
             f = getattr(c.lib, "madrl_%s_rollout_host2" % c.fam)
-            f.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
             E, A = c.n_envs, c.n_agents
             bufs = [Guarded((E, A, c.obs_dim), c.obs_dtype, np.nan), Guarded((T, E, A), c.obs_dtype, np.nan),
                     Guarded((T, E), np.uint8, 255), Guarded((T, E) + c.info_shape, np.int32, -1)]
@@ -739,8 +733,7 @@ def test_terminal_observations_are_kept_on_the_side(family):
     """madrl_*_set_terminal_obs: with auto-reset the obs slot of a done step holds the reset observation;
     the side tensor receives the observation the env returned before it was reset (what
     StandardizedEnv.step sees first, madrl_environments/__init__.py:283-291); other slots stay untouched."""
-    import ctypes as C
-    from emu.driver import EmuHostage, EmuPursuit, EmuWaterworld, Guarded, _p
+    from emu.driver import EmuHostage, EmuPursuit, EmuWaterworld
     mpl, T, E = 5, 17, 3
     if family == "waterworld":
         mk = lambda **kw: EmuWaterworld(E, seed=6, fp64=True, **WW["c2"], **kw)          # noqa: E731
@@ -756,7 +749,6 @@ def test_terminal_observations_are_kept_on_the_side(family):
     obs_a, rew_a, done_a, _ = a.rollout(act, auto_reset=True)
     term = Guarded(obs_a.shape, obs_a.dtype, -7.0)
     f = getattr(b.lib, "madrl_%s_set_terminal_obs" % b.fam)
-    f.argtypes = [C.c_void_p, C.c_void_p]
     assert f(b._h, _p(term.arr)) == 0
     obs_b, rew_b, done_b, _ = b.rollout(act, auto_reset=True)
     assert f(b._h, None) == 0

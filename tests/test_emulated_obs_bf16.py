@@ -3,14 +3,17 @@ of the three env kernels against the fp32 ones.  Observations must be the fp32 o
 even, bit for bit; state, rewards, dones and infos must not change at all."""
 import ctypes as C
 import os
-import shutil
 
 import numpy as np
 import pytest
 
+import postproc_edges as pe
 from conftest import ROOT  # noqa: F401  (puts the repository on sys.path)
+from emu import driver
+from emu.driver import Guarded
+from emu.driver import ptr as _p
 
-pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
+pytestmark = driver.needs_cxx
 
 OBS_NATIVE, OBS_BF16 = 0, 1
 
@@ -27,11 +30,11 @@ HW_ARGS = (10, 16, 16, 4, 2)
 
 
 def bf16_bits(x):
-    """Round-to-nearest-even float32 -> bfloat16 bits (what torch's .to(torch.bfloat16) does)."""
+    """The round-to-nearest-even bfloat16 bits of float32 x (postproc_edges.bf16_bits), which must hold no NaN: an
+    fp32 output slot a kernel left unwritten (NaN-filled) fails here."""
     x = np.ascontiguousarray(x, np.float32)
     assert not np.isnan(x).any()
-    u = x.view(np.uint32).astype(np.uint64)
-    return ((u + 0x7fff + ((u >> 16) & 1)) >> 16).astype(np.uint16)
+    return pe.bf16_bits(x)[0]
 
 
 def widen(b):
@@ -44,7 +47,6 @@ def pool16():
 
 @pytest.fixture(autouse=True)
 def no_shared_memory_hazards():
-    from emu import driver
     driver.races()
     yield
     assert driver.races() == 0, "shared-memory hazard reported by the emulator (see stderr)"
@@ -56,19 +58,16 @@ class Pair(object):
     def __init__(self, make):
         self.a, self.b = make(), make()
         f = getattr(self.b.lib, "madrl_%s_set_obs_format" % self.b.fam)
-        f.argtypes = [C.c_void_p, C.c_int]
         assert f(self.b._h, OBS_BF16) == 0
         self.E, self.A, self.D = self.a.n_envs, self.a.n_agents, self.a.obs_dim
 
     def obs_bufs(self, shape):
-        from emu.driver import Guarded
         return Guarded(shape, np.float32, np.nan), Guarded(shape, np.uint16, 0xFFFF)
 
     def check_state(self):
         assert np.array_equal(self.a.blob, self.b.blob), "state blobs differ"
 
     def reset(self, mask=None):
-        from emu.driver import _p
         m = None if mask is None else np.ascontiguousarray(mask, np.uint8)
         oa, ob = self.obs_bufs((self.E, self.A, self.D))
         for eng, o in ((self.a, oa), (self.b, ob)):
@@ -77,7 +76,6 @@ class Pair(object):
 
     def rollout(self, act, auto_reset=True, term=False):
         """Both engines, device entry point; with `term`, terminal observations kept on the side."""
-        from emu.driver import Guarded, _p
         T = act.shape[0]
         outs, terms = [], []
         for eng, dt in ((self.a, np.float32), (self.b, np.uint16)):
@@ -173,7 +171,6 @@ def _host_pair(fam):
 @pytest.mark.parametrize("fam", ["ww", "pursuit", "hostage"])
 def test_host_entry_points_copy_bf16_rows(fam):
     """reset_host and the chunked rollout_host2 (with and without MADRL_HOST_OBS_LAST) move 2-byte rows."""
-    from emu.driver import Guarded, _p
     p, act = _host_pair(fam)
     T, E, A, D = act.shape[0], p.E, p.A, p.D
     a, b = p.a, p.b
@@ -184,7 +181,6 @@ def test_host_entry_points_copy_bf16_rows(fam):
     assert np.array_equal(bf16_bits(oa.check("obs")), ob.check("obs"))
     p.check_state()
     f = b._f("rollout_host2")
-    f.argtypes = [C.c_void_p, C.c_int] + [C.c_void_p] * 5 + [C.c_int, C.c_int]
     b.lib.madrl_set_host_chunk_bytes(E * A * D * 2 * 3)          # ~3 steps per chunk
     try:
         for flags in (0, 1):
@@ -210,7 +206,6 @@ def test_host_entry_points_copy_bf16_rows(fam):
 
 
 def _heuristic(eng, T, obs0, act_dtype, act_shape, obs_dtype, extra=()):
-    from emu.driver import Guarded, _p
     E, A, D = eng.n_envs, eng.n_agents, eng.obs_dim
     bufs = [Guarded((T, E, A) + act_shape, act_dtype, -7), Guarded((T, E, A, D), obs_dtype, 0x7777),
             Guarded((T, E, A), np.float32, np.nan), Guarded((T, E), np.uint8, 255),
@@ -261,13 +256,11 @@ def test_set_obs_format_rejects_fp64_and_unknown_formats():
     from emu.driver import EmuHostage, EmuPursuit, EmuWaterworld
     for eng in (EmuWaterworld(2, fp64=True, **WW["c2"]), EmuHostage(2, *HW_ARGS, fp64=True)):
         f = eng._f("set_obs_format")
-        f.argtypes = [C.c_void_p, C.c_int]
         assert f(eng._h, OBS_BF16) == -1 and b"fp32" in eng.lib.madrl_last_error()
         assert f(eng._h, OBS_NATIVE) == 0
     for eng in (EmuWaterworld(2, fp64=False, **WW["c2"]), EmuPursuit(2, pool16(), **C3),
                 EmuHostage(2, *HW_ARGS, fp64=False)):
         f = eng._f("set_obs_format")
-        f.argtypes = [C.c_void_p, C.c_int]
         assert f(eng._h, 2) == -1 and b"format" in eng.lib.madrl_last_error()
         assert f(eng._h, -1) == -1
         assert f(eng._h, OBS_BF16) == 0 and f(eng._h, OBS_NATIVE) == 0
@@ -275,7 +268,7 @@ def test_set_obs_format_rejects_fp64_and_unknown_formats():
 
 def test_bf16_rows_with_peer_exchange_are_rejected():
     """The fused peer exchange is built for native observations only."""
-    from emu.driver import EmuWaterworld, Guarded, _p
+    from emu.driver import EmuWaterworld
     p = Pair(lambda: EmuWaterworld(2, seed=1, fp64=False, **WW["c2"]))
     p.reset()
     eng = p.b
@@ -301,25 +294,10 @@ def test_bf16_rounding_helper_matches_torch():
 
 
 # ------------------------------------------------------------------ post-processing on bf16 observations
-def _postproc_lib():
-    from emu import driver
-    L = driver.load(())
-    vp, i32, dbl, sz = C.c_void_p, C.c_int, C.c_double, C.c_size_t
-    for suf in ("f32", "bf16"):
-        getattr(L, "madrl_frame_stack_" + suf).argtypes = [i32] * 5 + [vp] * 5
-        getattr(L, "madrl_standardize_" + suf).argtypes = [i32, sz, vp, vp, vp, dbl, dbl, i32, dbl, i32, vp]
-        getattr(L, "madrl_standardize_obs_terminal_" + suf).argtypes = [i32, i32, sz] + [vp] * 5 + [dbl, dbl, vp]
-    for suf in ("u32", "u16"):
-        getattr(L, "madrl_paths_pack_" + suf).argtypes = [i32] * 4 + [vp] * 6
-    L.madrl_paths_plan.argtypes = [i32, i32, i32] + [vp] * 6
-    return L
-
-
 def test_bf16_postproc_kernels_equal_f32_on_widened_input():
     """frame_stack / standardize / standardize_obs_terminal / paths_pack_u16 on bf16 observations equal
     the f32 passes run on the widened values, rounded to nearest even (D odd, as C2's 213)."""
-    from emu.driver import _p
-    L = _postproc_lib()
+    L = driver.load(())
     rs = np.random.RandomState(3)
     T, E, A, D, B = 9, 3, 2, 13, 4
     xb = bf16_bits(rs.randn(T, E, A, D).astype(np.float32) * np.float32(3))
@@ -350,9 +328,7 @@ def test_bf16_postproc_kernels_equal_f32_on_widened_input():
     assert np.array_equal(bf16_bits(x32), x16) and np.array_equal(bf16_bits(t32), t16)
     assert np.array_equal(st[0][0], st[1][0]) and np.array_equal(st[0][1], st[1][1])
     # path packing of 2-byte rows (odd D), with and without the one-step shift
-    seg_s, seg_l = np.zeros((T, E), np.int32), np.zeros((T, E), np.int32)
-    n_ep, ep_rec = np.zeros(E, np.int32), np.zeros((E, T, 3), np.int32)
-    assert L.madrl_paths_plan(T, E, A, _p(done), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
+    seg_s, seg_l = driver.paths_plan(L, done, A)[:2]
     first = bf16_bits(rs.randn(E, A, D).astype(np.float32))
     for f16, f32 in ((None, None), (first, widen(first))):
         p32 = np.zeros((T * E * A, D), np.float32)

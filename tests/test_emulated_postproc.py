@@ -2,44 +2,21 @@
 standardiser, episode statistics, whole-batch moments / advantage centring) executed on the CPU by
 the warp emulator of tests/emu and compared with oracle/postproc_oracle.py -- the GPU test
 tests/test_postproc.py::test_cuda_* at small sizes, through the same C ABI."""
-import ctypes as C
-import os
-import shutil
-
 import numpy as np
 import pytest
 
 import postproc_edges as pe
-from emu import build_emu
+from emu import build_emu, driver
 from emu.driver import Guarded
+from emu.driver import ptr as _p
 from oracle import postproc_oracle as po
 
-pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
-
-
-def _p(a):
-    return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
+pytestmark = driver.needs_cxx
 
 
 @pytest.fixture(scope="module")
 def lib():
-    from emu import driver
-    L = driver.load(())
-    vp, i32, dbl = C.c_void_p, C.c_int, C.c_double
-    L.madrl_gae_f32.argtypes = [i32, i32, i32, vp, vp, vp, vp, dbl, dbl, vp, vp, vp]
-    L.madrl_frame_stack_f32.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
-    L.madrl_standardize_f32.argtypes = [i32, C.c_size_t, vp, vp, vp, dbl, dbl, i32, dbl, i32, vp]
-    L.madrl_episode_stats_f32.argtypes = [i32, i32, i32, vp, vp, dbl, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_moments_f32.argtypes = [C.c_size_t, vp, vp, vp, vp, vp]
-    L.madrl_center_advantages_f32.argtypes = [C.c_size_t, vp, i32, i32, vp, vp, vp]
-    L.madrl_moments_agents_f32.argtypes = [C.c_size_t, i32, vp, vp, vp, vp, vp]
-    L.madrl_center_advantages_agents_f32.argtypes = [C.c_size_t, i32, vp, i32, i32, vp, vp, vp]
-    L.madrl_frame_stack_bf16.argtypes = [i32, i32, i32, i32, i32, vp, vp, vp, vp, vp]
-    L.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_paths_pack_u32.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_paths_pack_u16.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_standardize_obs_terminal_f32.argtypes = [i32, i32, C.c_size_t] + [vp] * 5 + [dbl, dbl, vp]
-    return L
+    return driver.load(())
 
 
 def _data():
@@ -150,9 +127,6 @@ def test_path_packing_kernels_equal_host_to_paths(lib):
     loop of madrl_b200.postproc.to_paths: same paths in the same order, with and without the one-step
     observation shift."""
     from madrl_b200.postproc import to_paths
-    vp, i32 = C.c_void_p, C.c_int
-    lib.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    lib.madrl_paths_pack_u32.argtypes = [i32, i32, i32, i32, vp, vp, vp, vp, vp, vp]
     rs = np.random.RandomState(4)
     for T, E, A, D, p_done in ((30, 5, 3, 7, 0.12), (9, 2, 1, 40, 0.4), (17, 3, 4, 1, 0.0)):
         obs = rs.randn(T, E, A, D).astype(np.float32)
@@ -161,9 +135,7 @@ def test_path_packing_kernels_equal_host_to_paths(lib):
         rew = rs.randn(T, E, A).astype(np.float32)
         info = rs.randint(0, 9, size=(T, E)).astype(np.int32)
         done = (rs.rand(T, E) < p_done).astype(np.uint8)
-        seg_s, seg_l = np.full((T, E), -1, np.int32), np.full((T, E), -1, np.int32)
-        n_ep, ep_rec = np.zeros(E, np.int32), np.zeros((E, T, 3), np.int32)
-        assert lib.madrl_paths_plan(T, E, A, _p(done), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
+        seg_s, seg_l, n_ep, ep_rec = driver.paths_plan(lib, done, A)
 
         def pack(x, n_agents, first=None, per_agent=True):
             tail = x.shape[3:] if per_agent else x.shape[2:]
@@ -198,8 +170,6 @@ def test_standardizer_with_terminal_observations_follows_the_reference_order(lib
     """madrl_standardize_obs_terminal_f32 vs the StandardizedEnv oracle (pinned to the real wrapper in
     tests/test_postproc.py): at a done step the estimate sees the terminal observation first, then the
     reset observation (step() then reset(), madrl_environments/__init__.py:283-291)."""
-    lib.madrl_standardize_obs_terminal_f32.argtypes = [C.c_int, C.c_int, C.c_size_t] + [C.c_void_p] * 5 + \
-        [C.c_double, C.c_double, C.c_void_p]
     d = _data()
     T, E, A, D = d['T'], d['E'], d['A'], d['D']
     rs = np.random.RandomState(8)
@@ -221,10 +191,9 @@ def test_standardizer_with_terminal_observations_follows_the_reference_order(lib
 
 # ---------------------------------------------------------------- the edges of tests/test_postproc_edges_gpu.py
 # The same cases and checks (tests/postproc_edges.py), with the size edges of this build: its moments grid is
-# MADRL_MOM_BLOCKS CTAs of 256 threads (build_emu.PER_FILE_FLAGS), so its stride edge is that times 256.
+# MADRL_MOM_BLOCKS CTAs of 256 threads (build_emu.GRID), so its stride edge is that times 256.
 
-EMU_MOM_BLOCKS = int(next(f.split("=")[1] for f in build_emu.PER_FILE_FLAGS["postproc.cu"]
-                          if f.startswith("-DMADRL_MOM_BLOCKS=")))
+EMU_MOM_BLOCKS = build_emu.GRID["MADRL_MOM_BLOCKS"]
 
 
 def test_moments_at_the_grid_stride_edges(lib):
@@ -354,9 +323,7 @@ def test_path_packing_word_counts(lib, itemsize):
         for shifted in (False, True):
             T, E, A, p_done = pe.PACK_SHAPES[(k + shifted) % len(pe.PACK_SHAPES)]
             c = pe.pack_case(T, E, A, D, p_done, itemsize, 10 * D + shifted)
-            seg_s, seg_l = np.full((T, E), -1, np.int32), np.full((T, E), -1, np.int32)
-            n_ep, ep_rec = np.zeros(E, np.int32), np.zeros((E, T, 3), np.int32)
-            assert lib.madrl_paths_plan(T, E, A, _p(c["done"]), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
+            seg_s, seg_l, n_ep, ep_rec = driver.paths_plan(lib, c["done"], A)
             p_obs = Guarded((T * E * A, D), c["obs"].dtype, 0)
             assert pack(T, E, A, D, _p(c["obs"]), _p(c["obs_before"] if shifted else None), _p(seg_s), _p(seg_l),
                         _p(p_obs.arr), None) == 0

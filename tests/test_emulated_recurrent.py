@@ -4,32 +4,20 @@ with rllab's padding as oracle/recurrent_oracle.py restates it: wide and narrow 
 widths, with and without the one-step observation shift, per-env rows (A = 1), record tables in every control
 mode's order and in a shuffled one, and P * L off the block size.  Every output sits in a canary-guarded buffer
 pre-filled with non-zero words, so a padding word the kernel fails to write, or a write outside the buffer, fails."""
-import ctypes as C
-import os
-import shutil
-
 import numpy as np
 import pytest
 
+from emu import driver
 from emu.driver import Guarded
+from emu.driver import ptr as _p
 from oracle import recurrent_oracle as ro
 
-pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
-
-
-def _p(a):
-    return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
+pytestmark = driver.needs_cxx
 
 
 @pytest.fixture(scope="module")
 def lib():
-    from emu import driver
-    L = driver.load(())
-    vp, i32 = C.c_void_p, C.c_int
-    L.madrl_paths_pad_u32.argtypes = [i32] * 6 + [vp] * 5
-    L.madrl_paths_pad_u16.argtypes = [i32] * 6 + [vp] * 5
-    L.madrl_path_sums_f32.argtypes = [i32] * 4 + [vp] * 6
-    return L
+    return driver.load(())
 
 
 def episodes(done):

@@ -5,93 +5,24 @@ agent, with t0), and rltools' feature map of the linear-baseline kernels (madrl_
 The shapes cross the row-slice, warp-stride and 32-column edges of the kernels; A runs from 1 to 8.  Outputs sit in
 canary-guarded buffers, and every new entry point's argument checks (MADRL_EINVAL, no launch) are exercised."""
 import ctypes as C
-import os
-import shutil
 
 import numpy as np
 import pytest
 import torch
 
+import postproc_edges as pe
+from emu import driver
 from emu.driver import Guarded
+from emu.driver import ptr as _p
 from oracle import rltools_oracle as ro
 
-pytestmark = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
-
-# Own emulator build (as tests/test_linear_baseline_cpu.py does): block-static shared arrays, and few fixed slices
-# so that a launch stays small and the slice edges fall inside these tests' shapes.
-SLICES = 3
-EMU_SOURCES = {"common.cu": [],
-               "postproc.cu": ["-D__shared__=static", "-DMADRL_MOM_BLOCKS=6", "-DMADRL_RM_SLICES=%d" % SLICES,
-                               "-DMADRL_TB_SLICES=%d" % SLICES],
-               "baseline.cu": ["-D__shared__=static", "-DMADRL_LFB_SLICES=%d" % SLICES]}
-
-
-def _build_emu_lib():
-    import subprocess
-    from concurrent.futures import ThreadPoolExecutor
-    from emu import build_emu as be
-    out = os.path.join(be.OUT, "libmadrl_b200_emu_rltools.so")
-    deps = be._deps() + [os.path.abspath(__file__)]
-    if os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
-        return out
-    objdir = os.path.join(be.OUT, "obj_rltools")
-    os.makedirs(objdir, exist_ok=True)
-    cxx = os.environ.get("CXX", "g++")
-    srcs = [(os.path.join(be.CSRC, f), fl) for f, fl in EMU_SOURCES.items()] + \
-        [(os.path.join(be.HERE, "emu_runtime.cpp"), [])]
-
-    def one(job):
-        src, flags = job
-        obj = os.path.join(objdir, os.path.basename(src) + ".o")
-        res = subprocess.run([cxx] + be.CXXFLAGS + flags + ["-c", "-o", obj, src], stdout=subprocess.PIPE,
-                             stderr=subprocess.STDOUT, text=True)
-        assert res.returncode == 0, res.stdout
-        return obj
-    with ThreadPoolExecutor(max_workers=4) as pool:
-        objs = list(pool.map(one, srcs))
-    tmp = out + ".%d.tmp" % os.getpid()
-    subprocess.check_call([cxx, "-shared", "-o", tmp] + objs)
-    os.replace(tmp, out)
-    return out
+pytestmark = driver.needs_cxx
 
 
 @pytest.fixture(scope="module")
 def lib():
-    L = C.CDLL(_build_emu_lib())
-    vp, i32, sz = C.c_void_p, C.c_int, C.c_size_t
-    L.madrl_emu_race_count.restype = C.c_long
-    L.madrl_last_error.restype = C.c_char_p
-    L.madrl_paths_plan.argtypes = [i32, i32, i32] + [vp] * 6
-    L.madrl_running_moments_workspace_size.argtypes = [i32, i32, vp]
-    L.madrl_running_moments_f32.argtypes = [sz, i32, i32, sz] + [vp] * 5
-    L.madrl_running_moments_bf16.argtypes = L.madrl_running_moments_f32.argtypes
-    L.madrl_time_baseline_workspace_size.argtypes = [i32, i32, vp]
-    L.madrl_time_baseline_f32.argtypes = [i32] * 5 + [vp] * 10
-    L.madrl_lfbr_workspace_size.argtypes = [i32, vp]
-    L.madrl_lfbr_agents_workspace_size.argtypes = [i32, i32, vp]
-    for dt in ("f32", "bf16"):
-        for ag in ("", "_agents"):
-            getattr(L, "madrl_lfbr_normal_eq%s_%s" % (ag, dt)).argtypes = [i32] * 4 + [vp] * 9
-            getattr(L, "madrl_lfbr_predict%s_%s" % (ag, dt)).argtypes = [i32] * 4 + [vp] * 8
-    return L
-
-
-def _p(a):
-    return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
-
-
-def _bf16(x):
-    u = np.asarray(x, np.float32).view(np.uint32).astype(np.uint64)
-    b = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
-    return b, (b.astype(np.uint32) << 16).view(np.float32)
-
-
-def _plan(lib, done, A):
-    T, E = done.shape
-    seg_s, seg_l = np.empty((T, E), np.int32), np.empty((T, E), np.int32)
-    n_ep, ep_rec = np.empty(E, np.int32), np.zeros((E, T, 3), np.int32)
-    assert lib.madrl_paths_plan(T, E, A, _p(done), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
-    return seg_s, n_ep, ep_rec
+    """The emulator build, whose few row slices (build_emu.GRID) put the slice edges inside these tests' shapes."""
+    return driver.load(())
 
 
 def _index(done, t0):
@@ -131,7 +62,7 @@ def test_running_moments_equal_numpy_sums(lib, G, bf16):
     rs = np.random.RandomState(10 * G + bf16)
     for R, D in MOMENT_SHAPES:
         x = (rs.randn(R * G, D) * 3 + 1).astype(np.float32)
-        bits, x = _bf16(x) if bf16 else (x, x)
+        bits, x = pe.bf16_bits(x) if bf16 else (x, x)
         got = _moments(lib, bits, G, bf16=bf16)
         x64 = x.astype(np.float64).reshape(R, G, D)
         want = np.stack([x64.sum(0), (x64 * x64).sum(0)], 1)
@@ -196,7 +127,7 @@ def test_time_baseline_against_numpy(lib, A):
             done[0, 0] = done[T - 1, E - 1] = 1            # length-1 paths at t = 0 and t = T-1
         q = rs.randn(T, E, A).astype(np.float32)
         for t0 in (None, rs.randint(0, 6, E).astype(np.int32)):
-            seg_s, n_ep, ep_rec = _plan(lib, done, A)
+            seg_s, _, n_ep, ep_rec = driver.paths_plan(lib, done, A)
             idx = _index(done, t0)
             L = int(idx.max()) + 1
             for per_agent in (0, 1):
@@ -226,7 +157,7 @@ def test_time_baseline_is_the_reference_nanmean(lib):
     T, E, A = 12, 5, 3
     done = (rs.rand(T, E) < 0.25).astype(np.uint8)
     q = rs.randn(T, E, A).astype(np.float32)
-    seg_s, n_ep, ep_rec = _plan(lib, done, A)
+    seg_s, _, n_ep, ep_rec = driver.paths_plan(lib, done, A)
     L = int(_index(done, None).max()) + 1
     nbytes = C.c_size_t()
     assert lib.madrl_time_baseline_workspace_size(1, L, C.byref(nbytes)) == 0
@@ -242,7 +173,7 @@ def test_time_baseline_is_the_reference_nanmean(lib):
 def _lfbr(lib, obs, obs_before, done, q, norm, coef, A_groups, bf16):
     """madrl_lfbr normal equations and predictions of the emulator build."""
     T, E, A, D = obs.shape
-    seg_s, _, _ = _plan(lib, done, A)
+    seg_s = driver.paths_plan(lib, done, A)[0]
     nbytes = C.c_size_t()
     if A_groups:
         assert lib.madrl_lfbr_agents_workspace_size(D, A, C.byref(nbytes)) == 0
@@ -252,7 +183,8 @@ def _lfbr(lib, obs, obs_before, done, q, norm, coef, A_groups, bf16):
     Dc = D + 4
     G = Guarded(((A,) if A_groups else ()) + (Dc, Dc), np.float64, np.nan)
     sfx = ("_agents" if A_groups else "") + ("_bf16" if bf16 else "_f32")
-    src, first = (_bf16(obs)[0], None if obs_before is None else _bf16(obs_before)[0]) if bf16 else (obs, obs_before)
+    src, first = (pe.bf16_bits(obs)[0], None if obs_before is None else pe.bf16_bits(obs_before)[0]) if bf16 \
+        else (obs, obs_before)
     assert getattr(lib, "madrl_lfbr_normal_eq" + sfx)(T, E, A, D, _p(src), _p(first), _p(seg_s), None, _p(q),
                                                       _p(norm), _p(G.arr), _p(ws), None) == 0
     vals = Guarded((T, E, A), np.float32, np.nan)
@@ -273,8 +205,8 @@ def test_rltools_feature_map_against_numpy(lib, A, D, obsnorm, shifted, bf16):
     obs = (rs.randn(T, E, A, D) * 2 + 0.5).astype(np.float32)
     ob = (rs.randn(E, A, D) * 2 + 0.5).astype(np.float32) if shifted else None
     if bf16:
-        obs = _bf16(obs)[1]
-        ob = None if ob is None else _bf16(ob)[1]
+        obs = pe.bf16_bits(obs)[1]
+        ob = None if ob is None else pe.bf16_bits(ob)[1]
     done = (rs.rand(T, E) < 0.2).astype(np.uint8)
     q = rs.randn(T, E, A).astype(np.float32)
     seen = (np.concatenate([ob[None], obs[:-1]]) if shifted else obs).astype(np.float64)

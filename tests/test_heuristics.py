@@ -8,19 +8,17 @@ kernels (madrl_ww_rollout_heuristic / madrl_pursuit_rollout_heuristic):
     tests/test_heuristics_gpu.py.
 """
 import os
-import shutil
 
 import numpy as np
 import pytest
 
 from conftest import ROOT
+from emu.driver import needs_cxx
 from oracle import ref_records as R
 from oracle.heuristics_oracle import (pursuit_action, pursuit_action_table, policy_draw, waterworld_action)
 from oracle.philox import Stream
 from oracle.pursuit_oracle import PursuitOracle
 from oracle.waterworld_oracle import WaterworldOracle
-
-needs_cxx = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
 
 
 def f32(x):
@@ -134,9 +132,8 @@ def test_emulated_waterworld_policy_fp32():
     assert checked > 0.5 * T * E * cfg['n_pursuers']
 
 
+@needs_cxx
 def test_waterworld_policy_needs_the_speed_feature_layout():
-    if shutil.which(os.environ.get("CXX", "g++")) is None:
-        pytest.skip("no host C++ compiler")
     from emu.driver import EmuWaterworld
     eng = EmuWaterworld(2, n_pursuers=3, n_evaders=3, speed_features=False)
     with pytest.raises(RuntimeError, match="speed_features"):

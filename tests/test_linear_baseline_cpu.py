@@ -4,18 +4,19 @@ csrc/baseline.cu executed by the warp emulator of tests/emu against the oracle, 
 madrl_b200.postproc.LinearFeatureBaseline."""
 import ctypes as C
 import os
-import shutil
 
 import numpy as np
 import pytest
 import torch
 
 import postproc_edges as pe
+from emu import build_emu, driver
+from emu.driver import needs_cxx
+from emu.driver import ptr as _p
 from oracle import baseline_oracle as bo
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "linear_baseline_ref.npz")
 CASES = ("ragged", "rank_deficient", "beyond_clip")
-have_cxx = pytest.mark.skipif(shutil.which(os.environ.get("CXX", "g++")) is None, reason="no host C++ compiler")
 
 
 def _case(name):
@@ -74,77 +75,14 @@ def test_chained_launches_with_t0_equal_one_long_launch():
 
 # ---------------------------------------------------------------- the kernels in the warp emulator
 
-def _p(a):
-    return C.c_void_p(a.ctypes.data) if a is not None else C.c_void_p(0)
-
-
-# The emulator library of tests/emu/build_emu.py is built from its fixed source list; these tests compile their own
-# one with the same compiler flags and fiber runtime: the sources the baseline passes need (common.cu for the error
-# state, postproc.cu for paths_plan, baseline.cu) with baseline.cu's block-static shared tiles and 3 row slices
-# instead of 48, so that a launch does not create thousands of fibers.
-EMU_SOURCES = {"common.cu": [], "postproc.cu": ["-D__shared__=static", "-DMADRL_MOM_BLOCKS=6"],
-               "baseline.cu": ["-D__shared__=static", "-DMADRL_LFB_SLICES=3"]}
-
-
-def _build_emu_lib():
-    import subprocess
-    from concurrent.futures import ThreadPoolExecutor
-    from emu import build_emu as be
-    out = os.path.join(be.OUT, "libmadrl_b200_emu_lfb.so")
-    deps = be._deps() + [os.path.abspath(__file__)]
-    if os.path.exists(out) and all(os.path.getmtime(d) <= os.path.getmtime(out) for d in deps):
-        return out
-    objdir = os.path.join(be.OUT, "obj_lfb")
-    os.makedirs(objdir, exist_ok=True)
-    cxx = os.environ.get("CXX", "g++")
-    srcs = [(os.path.join(be.CSRC, f), fl) for f, fl in EMU_SOURCES.items()] + [(os.path.join(be.HERE, "emu_runtime.cpp"), [])]
-
-    def one(job):
-        src, flags = job
-        obj = os.path.join(objdir, os.path.basename(src) + ".o")
-        res = subprocess.run([cxx] + be.CXXFLAGS + flags + ["-c", "-o", obj, src], stdout=subprocess.PIPE,
-                             stderr=subprocess.STDOUT, text=True)
-        assert res.returncode == 0, res.stdout
-        return obj
-    with ThreadPoolExecutor(max_workers=4) as pool:
-        objs = list(pool.map(one, srcs))
-    tmp = out + ".%d.tmp" % os.getpid()
-    subprocess.check_call([cxx, "-shared", "-o", tmp] + objs)
-    os.replace(tmp, out)
-    return out
-
-
-def _races(L):
-    n = int(L.madrl_emu_race_count())
-    L.madrl_emu_race_reset()
-    return n
-
-
 @pytest.fixture(scope="module")
 def lib():
-    L = C.CDLL(_build_emu_lib())
-    L.madrl_emu_race_count.restype = C.c_long
-    vp, i32 = C.c_void_p, C.c_int
-    L.madrl_paths_plan.argtypes = [i32, i32, i32, vp, vp, vp, vp, vp, vp]
-    L.madrl_lfb_workspace_size.argtypes = [i32, C.POINTER(C.c_size_t)]
-    for dt in ("f32", "bf16"):
-        getattr(L, "madrl_lfb_normal_eq_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 8
-        getattr(L, "madrl_lfb_predict_" + dt).argtypes = [i32, i32, i32, i32] + [vp] * 7
-    return L
-
-
-def _bf16_bits(x):
-    """Round-to-nearest-even bfloat16 bits of float32 x (uint16) and their exact float32 widening."""
-    u = x.astype(np.float32).view(np.uint32).astype(np.uint64)
-    b = ((u + 0x7FFF + ((u >> 16) & 1)) >> 16).astype(np.uint16)
-    return b, (b.astype(np.uint32) << 16).view(np.float32)
+    return driver.load(())
 
 
 def _run(lib, obs, obs_before, done, ret, t0, coef, bf16):
     T, E, A, D = obs.shape
-    seg_s, seg_l = np.empty((T, E), np.int32), np.empty((T, E), np.int32)
-    n_ep, ep_rec = np.empty(E, np.int32), np.empty((E, T, 3), np.int32)
-    assert lib.madrl_paths_plan(T, E, A, _p(done), _p(seg_s), _p(seg_l), _p(n_ep), _p(ep_rec), None) == 0
+    seg_s = driver.paths_plan(lib, done, A)[0]
     nbytes = C.c_size_t()
     assert lib.madrl_lfb_workspace_size(D, C.byref(nbytes)) == 0
     ws = np.empty(nbytes.value // 8)
@@ -168,7 +106,7 @@ EMU_SHAPES = [  # T, E, A, D, p_done, obs_before, t0
 ]
 
 
-@have_cxx
+@needs_cxx
 @pytest.mark.parametrize("shape", EMU_SHAPES, ids=lambda s: "T%dE%dA%dD%d%s%s" % (s[:4] + ("_before" if s[5] else "",
                                                                                           "_t0" if s[6] else "")))
 def test_emulated_kernels_match_oracle(lib, shape):
@@ -181,12 +119,12 @@ def test_emulated_kernels_match_oracle(lib, shape):
     ret = rs.randn(T, E, A).astype(np.float32)
     t0 = rs.randint(0, 300, size=E).astype(np.int32) if with_t0 else None
     coef = rs.randn(2 * D + 4)
-    _races(lib)
+    driver.races()
     results = {}
     for bf16 in (False, True):
         if bf16:
-            o, o_w = _bf16_bits(obs)
-            ob, ob_w = _bf16_bits(obs_before) if with_before else (None, None)
+            o, o_w = pe.bf16_bits(obs)
+            ob, ob_w = pe.bf16_bits(obs_before) if with_before else (None, None)
             results["bf16"] = _run(lib, o, ob, done, ret, t0, coef, True)
             results["f32_widened"] = _run(lib, o_w, ob_w, done, ret, t0, coef, False)
             o_ref, ob_ref = o_w, ob_w
@@ -204,10 +142,10 @@ def test_emulated_kernels_match_oracle(lib, shape):
         assert np.all(np.abs(vals.reshape(-1).astype(np.float64) - want) <= tol)
     for a, b in zip(results["bf16"], results["f32_widened"]):                 # bf16 == the call on obs.float()
         assert np.array_equal(a, b)
-    assert _races(lib) == 0
+    assert driver.races() == 0
 
 
-@have_cxx
+@needs_cxx
 @pytest.mark.parametrize("bf16", [False, True], ids=["f32", "bf16"])
 def test_emulated_single_row_reads_out_the_exact_features(lib, bf16):
     """One row: G = outer(f, f) bit for bit, f = [clip(o), clip(o)^2, a, a^2, a^3, 1, y] with the correctly rounded
@@ -216,7 +154,7 @@ def test_emulated_single_row_reads_out_the_exact_features(lib, bf16):
     (tests/test_postproc_edges_gpu.py sweeps more obs_dims and indices on the device)."""
     rs = np.random.RandomState(3 + bf16)
     done = np.zeros((1, 1), np.uint8)
-    _races(lib)
+    driver.races()
     for D in (30, 31, 32):
         for before in (False, True):
             for k, t0 in enumerate((1, 99, 767, 50004)):
@@ -230,14 +168,14 @@ def test_emulated_single_row_reads_out_the_exact_features(lib, bf16):
                                    np.eye(2 * D + 4)[j], bf16)
                     assert np.array_equal(G, np.outer(f, f)), (D, before, t0)
                     assert vals.item() == np.float32(f[j]), (D, before, t0, j)
-    assert _races(lib) == 0
+    assert driver.races() == 0
 
 
-@have_cxx
+@needs_cxx
 def test_emulated_workspace_and_bad_sizes(lib):
     nbytes = C.c_size_t()
     assert lib.madrl_lfb_workspace_size(213, C.byref(nbytes)) == 0
-    assert nbytes.value == 3 * 28 * 64 * 64 * 8                           # emulator build: 3 row slices; 431 -> 7 tiles
+    assert nbytes.value == build_emu.GRID["MADRL_LFB_SLICES"] * 28 * 64 * 64 * 8        # 431 columns -> 7 tiles
     assert lib.madrl_lfb_workspace_size(0, C.byref(nbytes)) != 0
     assert lib.madrl_lfb_workspace_size(8193, C.byref(nbytes)) != 0
     x = np.zeros(64, np.float32)
