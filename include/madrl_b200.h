@@ -53,7 +53,8 @@ int madrl_version(void);
 /* sizeof(madrl_{ww,pursuit,hostage}_{config,layout}) as this library was compiled: a foreign-language
  * binding compares them with its own struct definitions before the first call. */
 void madrl_abi_sizes(int32_t* out6);
-/* Number of kernels launched by this library since load (bench.py's gpu_launches). */
+/* Number of kernels launched by this library since load (bench.py's gpu_launches).  A launch recorded into a CUDA
+ * graph during stream capture counts once, at capture; replays of the graph do not count. */
 uint64_t madrl_launch_count(void);
 /* Device->host bytes per pipeline chunk of the `*_rollout_host` entry points (0 = default 32 MB). */
 void madrl_set_host_chunk_bytes(size_t bytes);
@@ -88,6 +89,19 @@ int madrl_stream_wait_geq32(void* stream, void* addr_dev, uint32_t value);
  * an fp64 handle.  Waterworld's fused peer exchange (madrl_ww_set_peers) needs NATIVE observations. */
 #define MADRL_OBS_NATIVE 0
 #define MADRL_OBS_BF16 1
+
+/* L2 cache policy of the observation stores (madrl_{ww,pursuit,hostage}_set_obs_cache).  STREAM (the default):
+ * evict-first stores, right for long open-loop trajectories that nothing reads back soon.  KEEP: normal-priority
+ * stores, for a closed loop whose policy reads each step's observations right after the launch.  The mode applies
+ * to the observation rows of the `*_rollout` / `*_step` entry points (and the _host variants, which call them);
+ * resets, the heuristic-policy and peer-exchange rollouts and the set_terminal_obs copies always stream.  Every
+ * value written is the same in both modes.  MADRL_EINVAL for an unknown mode, a NULL handle or KEEP on an fp64
+ * handle.
+ * CUDA-graph capture: between their argument checks and the launch, `*_rollout` and `*_step` make no host
+ * synchronisation, allocation or host copy, so they may be captured into a graph on a capturing stream; the graph
+ * then holds the pointers, T and the handle's settings of the capture. */
+#define MADRL_OBS_CACHE_STREAM 0
+#define MADRL_OBS_CACHE_KEEP 1
 
 /* ------------------------------------------------------------------ MAWaterWorld ------------ */
 typedef struct madrl_ww_config {
@@ -143,6 +157,7 @@ int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T);
  * other slots are left untouched).  NULL switches it off. */
 int madrl_ww_set_terminal_obs(madrl_ww* h, void* term_obs_dev);
 int madrl_ww_set_obs_format(madrl_ww* h, int format);
+int madrl_ww_set_obs_cache(madrl_ww* h, int mode);
 /* Fused per-rollout exchange for env-sharded multi-GPU runs: after this call every rollout also
  * stores its reward / done / info rows into slot `slot` of each of the `n_dest` listed gather
  * buffers (peer-mapped device pointers: CUDA-IPC mappings of other ranks' buffers over NVLink; one
@@ -247,6 +262,7 @@ int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_p
 int madrl_pursuit_set_terminal_obs(madrl_pursuit* h, void* term_obs_dev);
 /* obs buffers below are float, or bfloat16 after set_obs_format(MADRL_OBS_BF16). */
 int madrl_pursuit_set_obs_format(madrl_pursuit* h, int format);
+int madrl_pursuit_set_obs_cache(madrl_pursuit* h, int mode);
 /* Curriculum knobs that survive pickling in the reference (pursuit_evade.py:264-272,397-411). */
 int madrl_pursuit_set_params(madrl_pursuit* h, double catchr, double constraint_window);
 /* reset(): obs_dev float [E][Np][obs_dim]. */
@@ -321,6 +337,7 @@ int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, int blocks_p
  * other slots are left untouched).  NULL switches it off. */
 int madrl_hostage_set_terminal_obs(madrl_hostage* h, void* term_obs_dev);
 int madrl_hostage_set_obs_format(madrl_hostage* h, int format);
+int madrl_hostage_set_obs_cache(madrl_hostage* h, int mode);
 /* obs_dev real [E][n_good][obs_dim] */
 int madrl_hostage_reset(madrl_hostage* h, const uint8_t* mask_dev, void* obs_dev, void* stream);
 /* actions_dev real [T][E][n_good][2]; obs_dev real [T][E][n_good][obs_dim]; rew_dev real

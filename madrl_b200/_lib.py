@@ -19,6 +19,8 @@ class EngineError(RuntimeError):
 
 # observation formats (madrl_*_set_obs_format)
 OBS_NATIVE, OBS_BF16 = 0, 1
+# L2 policy of the rollouts' observation stores (madrl_*_set_obs_cache)
+OBS_CACHE_STREAM, OBS_CACHE_KEEP = 0, 1
 
 
 class WWConfig(C.Structure):
@@ -132,6 +134,7 @@ def _signatures():
             ("set_launch", (i32, [vp, i32, i32])),
             ("set_terminal_obs", (i32, [vp, vp])),
             ("set_obs_format", (i32, [vp, i32])),
+            ("set_obs_cache", (i32, [vp, i32])),
             ("reset", (i32, [vp, vp, vp, vp])),
             ("rollout", (i32, [vp, i32, vp, vp, vp, vp, vp, i32, vp])),
             ("step", (i32, [vp, vp, vp, vp, vp, vp, i32, vp])),

@@ -51,6 +51,14 @@ __device__ __forceinline__ void store_stream(T* p, T v) {
   __stcs(p, v);
 }
 
+// Observation store of an env kernel: evict-first, or with KEEP (madrl_*_set_obs_cache(MADRL_OBS_CACHE_KEEP)) a
+// plain store at normal L2 priority, for a policy that reads this step's rows right after the launch.
+template <bool KEEP, typename T>
+__device__ __forceinline__ void store_obs(T* p, T v) {
+  if constexpr (KEEP) *p = v;
+  else store_stream(p, v);
+}
+
 // Vector type of an (x, y) pair of `real`.
 template <typename real> struct Vec2;
 template <> struct Vec2<float> { typedef float2 type; };
@@ -178,6 +186,11 @@ __device__ __forceinline__ void bulk_store_stream(void* dst, uint32_t src, uint3
                "cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, pol;\n\t"
                "cp.async.bulk.commit_group; }" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
 }
+// The same without a cache hint: the rows stay in L2 at normal priority (store_obs<true>).
+__device__ __forceinline__ void bulk_store_keep(void* dst, uint32_t src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;\n\t"
+               "cp.async.bulk.commit_group;" ::"l"(dst), "r"(src), "r"(bytes) : "memory");
+}
 // Every bulk group / all but the most recent one have finished reading their shared source.
 __device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 __device__ __forceinline__ void bulk_wait_read_all_but_1() { asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory"); }
@@ -221,6 +234,7 @@ static inline void bulk_store_stream(void* dst, uint32_t src, uint32_t bytes) {
   smem_access(src, bytes, SMEM_READ);
   memcpy(dst, emu_at(src), bytes);
 }
+static inline void bulk_store_keep(void* dst, uint32_t src, uint32_t bytes) { bulk_store_stream(dst, src, bytes); }
 static inline void bulk_wait_read_all() {}
 static inline void bulk_wait_read_all_but_1() {}
 static inline void bulk_wait_all() {}
@@ -234,6 +248,12 @@ static inline uint16_t bf16_rn(float v) {
 }
 static inline uint32_t bf16x2_rn(float lo, float hi) { return (uint32_t)bf16_rn(lo) | ((uint32_t)bf16_rn(hi) << 16); }
 #endif  // MADRL_EMU_PTX_HELPERS
+
+template <bool KEEP>
+__device__ __forceinline__ void bulk_store_obs(void* dst, uint32_t src, uint32_t bytes) {
+  if constexpr (KEEP) bulk_store_keep(dst, src, bytes);
+  else bulk_store_stream(dst, src, bytes);
+}
 
 // Observation element type O of an env kernel: its `real`, or uint16_t = bfloat16 bits (with real = float
 // only; madrl_*_set_obs_format).  Features are computed in `real` either way and converted once, at the

@@ -22,6 +22,7 @@ struct EngineCore {
   HostPipe pipe;             // staging + streams of the host-buffer entry points (lazily created)
   void* term_obs = nullptr;  // set_terminal_obs (NULL = off)
   int obs_format = MADRL_OBS_NATIVE;   // set_obs_format: element type of every observation buffer
+  int obs_cache = MADRL_OBS_CACHE_STREAM;   // set_obs_cache: L2 policy of the rollouts' observation stores
 
   // bytes of one observation element: `native` (the handle's real) or 2 (bfloat16)
   size_t obs_elem_bytes(size_t native) const { return obs_format == MADRL_OBS_BF16 ? 2 : native; }
@@ -100,6 +101,14 @@ inline int engine_set_obs_format(EngineCore* h, int format, bool fp64) {
   return MADRL_OK;
 }
 
+inline int engine_set_obs_cache(EngineCore* h, int mode, bool fp64) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(mode == MADRL_OBS_CACHE_STREAM || mode == MADRL_OBS_CACHE_KEEP, "unknown observation cache mode %d", mode);
+  MADRL_REQUIRE(!(mode == MADRL_OBS_CACHE_KEEP && fp64), "MADRL_OBS_CACHE_KEEP needs an fp32 handle (fp64 = 0)");
+  h->obs_cache = mode;
+  return MADRL_OK;
+}
+
 // `warps_per_block` is range-checked for ABI stability and otherwise ignored: blocks are one warp.
 inline int engine_set_launch(EngineCore* h, int warps_per_block, int blocks_per_sm) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
@@ -125,7 +134,7 @@ int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStrea
   int grid = E;
   if (grid > h->sms * resident) grid = h->sms * resident;
   MADRL_LAUNCH(kfn, grid, 32, smem, stream, p);
-  g_launches.fetch_add(1);
+  g_launches.fetch_add(1);   // under stream capture: counted once, when recorded, not at each graph replay
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
 }

@@ -52,7 +52,8 @@ __device__ __forceinline__ real unit_at(uint64_t seed, uint32_t env_id, uint64_t
   return (real)(stream_word(seed, env_id, 0u, n) >> 8) * (real)(1.0 / 16777216.0);
 }
 
-template <typename real, typename O, int OPL, int KCH, int KC>
+// KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
+template <typename real, typename O, int OPL, int KCH, int KC, bool KEEP = false>
 __global__ void __launch_bounds__(32, (OPL <= 2 ? 28 : 16))
 hw_kernel(const __grid_constant__ HWParams<real, O> p) {
   const real INF = real_inf<real>();
@@ -296,11 +297,11 @@ hw_kernel(const __grid_constant__ HWParams<real, O> p) {
             }
             if (k < K) {
               O* o = obs_row + 32 * kc;
-              store_stream(o + 0 * K, obs_cvt<O>(fC));
-              store_stream(o + 1 * K, obs_cvt<O>(sC));
-              store_stream(o + 2 * K, obs_cvt<O>(bH[kc] < INF ? bH[kc] : z));
-              store_stream(o + 3 * K, obs_cvt<O>(bK[kc] < INF ? bK[kc] : z));
-              store_stream(o + 4 * K, obs_cvt<O>(bB[kc] < INF ? bB[kc] : z));
+              store_obs<KEEP>(o + 0 * K, obs_cvt<O>(fC));
+              store_obs<KEEP>(o + 1 * K, obs_cvt<O>(sC));
+              store_obs<KEEP>(o + 2 * K, obs_cvt<O>(bH[kc] < INF ? bH[kc] : z));
+              store_obs<KEEP>(o + 3 * K, obs_cvt<O>(bK[kc] < INF ? bK[kc] : z));
+              store_obs<KEEP>(o + 4 * K, obs_cvt<O>(bB[kc] < INF ? bB[kc] : z));
             }
           }
         }
@@ -340,12 +341,12 @@ hw_kernel(const __grid_constant__ HWParams<real, O> p) {
         // (post), id; lane i writes rescuer i's.  whoEnc / whoC are exactly the any-collision masks.
         if (lane < p.Nr) {
           O* tp = obs_t + (size_t)lane * (p.D - 1) + 5 * K;   // obs_t already carries +lane
-          store_stream(tp, obs_cvt<O>((real)((whoEnc >> lane) & 1u)));
-          store_stream(tp + 1, obs_cvt<O>((real)((whoC >> lane) & 1u)));
-          store_stream(tp + 2, obs_cvt<O>((real)((coll_ke >> lane) & 1u)));
-          store_stream(tp + 3, obs_cvt<O>((real)((coll_bo >> lane) & 1u)));
-          store_stream(tp + 4, obs_cvt<O>(gate_post ? (real)1 : (real)0));
-          if (p.addid) store_stream(tp + 5, obs_cvt<O>((real)(lane + 1)));
+          store_obs<KEEP>(tp, obs_cvt<O>((real)((whoEnc >> lane) & 1u)));
+          store_obs<KEEP>(tp + 1, obs_cvt<O>((real)((whoC >> lane) & 1u)));
+          store_obs<KEEP>(tp + 2, obs_cvt<O>((real)((coll_ke >> lane) & 1u)));
+          store_obs<KEEP>(tp + 3, obs_cvt<O>((real)((coll_bo >> lane) & 1u)));
+          store_obs<KEEP>(tp + 4, obs_cvt<O>(gate_post ? (real)1 : (real)0));
+          if (p.addid) store_obs<KEEP>(tp + 5, obs_cvt<O>((real)(lane + 1)));
         }
         if (coll_bo) flags |= 2;
         if (coll_ke) flags |= 1;
@@ -481,12 +482,19 @@ extern "C" int madrl_hostage_set_obs_format(madrl_hostage* h, int format) {
   return engine_set_obs_format(h, format, h != nullptr && h->cfg.fp64);
 }
 
+extern "C" int madrl_hostage_set_obs_cache(madrl_hostage* h, int mode) {
+  return engine_set_obs_cache(h, mode, h != nullptr && h->cfg.fp64);
+}
+
 extern "C" int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
 template <typename real, typename O, int OPL, int KCH, int KC>
 static int hw_launch_inst(madrl_hostage* h, const HWParams<real, O>& p, cudaStream_t stream) {
+  if constexpr (sizeof(real) == 4)   // set_obs_cache refuses KEEP on fp64 handles
+    if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
+      return engine_launch(h, hw_kernel<real, O, OPL, KCH, KC, true>, 0, p.E, stream, p);
   return engine_launch(h, hw_kernel<real, O, OPL, KCH, KC>, 0, p.E, stream, p);
 }
 

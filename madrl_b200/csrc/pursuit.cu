@@ -103,7 +103,8 @@ __device__ __forceinline__ double numpy_mean(const double* a, int n) {
 // (a separate instantiation: the open-loop kernel carries none of its instructions).
 // FLAT = flatten=True layout (3R^2 [+1]); false = the (R, R, 4) conv layout: compile-time, so the window loop has no
 // layout branch.
-template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
+// KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP = false>
 __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEParams<O> p) {
   extern __shared__ __align__(16) uint32_t smem_u32[];
   const int lane = threadIdx.x, wib = 0;
@@ -409,9 +410,9 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
                 const int w = lane + 32 * it;
                 if (w < RR) {
                   const float v0 = inb[it] ? ((wv[it] & 0xff) ? p.one_val : 0.0f) : p.wall_val;   // pe:433,438
-                  store_stream(row + w, obs_cvt<O>(v0));
-                  store_stream(row + RR + w, obs_cvt<O>(v1[it]));
-                  store_stream(row + 2 * RR + w, obs_cvt<O>(v2[it]));
+                  store_obs<KEEP>(row + w, obs_cvt<O>(v0));
+                  store_obs<KEEP>(row + RR + w, obs_cvt<O>(v1[it]));
+                  store_obs<KEEP>(row + 2 * RR + w, obs_cvt<O>(v2[it]));
                 }
               }
             } else {
@@ -427,15 +428,15 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
                   const float v0 = inb[it] ? ((wv[it] & 0xff) ? p.one_val : 0.0f) : p.wall_val;
                   const float v3 = w == centre ? idval : 0.0f;
                   if constexpr (sizeof(O) == 2)
-                    __stcs(reinterpret_cast<unsigned long long*>(row) + w,
-                           (unsigned long long)bf16x2_rn(v0, v1[it]) | ((unsigned long long)bf16x2_rn(v2[it], v3) << 32));
+                    store_obs<KEEP>(reinterpret_cast<unsigned long long*>(row) + w,
+                                    (unsigned long long)bf16x2_rn(v0, v1[it]) | ((unsigned long long)bf16x2_rn(v2[it], v3) << 32));
                   else
-                    __stcs(reinterpret_cast<float4*>(row) + w, make_float4(v0, v1[it], v2[it], v3));
+                    store_obs<KEEP>(reinterpret_cast<float4*>(row) + w, make_float4(v0, v1[it], v2[it], v3));
                 }
               }
             }
           }
-          if (FLAT && n_tail && lane < Np) store_stream(obs_t + (size_t)lane * p.D + 3 * RR, obs_cvt<O>(my_idv));   // pe:444-445
+          if (FLAT && n_tail && lane < Np) store_obs<KEEP>(obs_t + (size_t)lane * p.D + 3 * RR, obs_cvt<O>(my_idv));   // pe:444-445
         }
         need_reset = false;
         if (!pass) {
@@ -629,6 +630,10 @@ extern "C" int madrl_pursuit_set_obs_format(madrl_pursuit* h, int format) {
   return engine_set_obs_format(h, format, false);
 }
 
+extern "C" int madrl_pursuit_set_obs_cache(madrl_pursuit* h, int mode) {
+  return engine_set_obs_cache(h, mode, false);
+}
+
 extern "C" int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
@@ -668,6 +673,9 @@ template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
 static int pe_launch_inst3(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)p.smem_per_warp;   // block LUT + per-warp regions
   MADRL_REQUIRE(smem <= 200 * 1024, "map too large for shared memory (%zu B per block)", smem);
+  if constexpr (!POLICY)   // the heuristic-policy rollouts always stream
+    if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
+      return engine_launch(h, pe_kernel<O, EPL, CPL, RC, false, FLAT, true>, smem, p.E, stream, p);
   return engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT>, smem, p.E, stream, p);
 }
 

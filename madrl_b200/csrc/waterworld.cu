@@ -148,19 +148,19 @@ __device__ __forceinline__ uint32_t obs_row_stage(bool whole_step, uint32_t stag
 // (HBM then sees whole sectors from one writer), the <= 16 bytes outside it on either side by
 // direct stores of one lane per element.  Full writes, no read-back, so the rows are bit-identical
 // to per-lane stores.
-template <typename O>
+template <bool KEEP, typename O>
 __device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int lane) {
   fence_async_shared();   // this lane's shared stores -> visible to the async proxy ...
   __syncwarp();           // ... before lane 0 issues the copy; the edge lanes read other lanes' values
   const uintptr_t g0 = (uintptr_t)row, g1 = g0 + (uintptr_t)n * sizeof(O);
   const uintptr_t a0 = (g0 + 15u) & ~(uintptr_t)15u, a1 = g1 & ~(uintptr_t)15u;
   const bool bulk = a1 > a0;
-  if (lane == 0 && bulk) bulk_store_stream((void*)a0, slot + (uint32_t)(a0 - (g0 & ~(uintptr_t)15u)), (uint32_t)(a1 - a0));
+  if (lane == 0 && bulk) bulk_store_obs<KEEP>((void*)a0, slot + (uint32_t)(a0 - (g0 & ~(uintptr_t)15u)), (uint32_t)(a1 - a0));
   const int head = bulk ? (int)((a0 - g0) / sizeof(O)) : n;
   const int tail = bulk ? (int)((g1 - a1) / sizeof(O)) : 0;
   if (lane < head + tail) {
     const int i = lane < head ? lane : n - tail + (lane - head);
-    store_stream(row + i, lds_obs<O>(slot + ((uint32_t)g0 & 15u) + (uint32_t)(i * sizeof(O))));
+    store_obs<KEEP>(row + i, lds_obs<O>(slot + ((uint32_t)g0 & 15u) + (uint32_t)(i * sizeof(O))));
   }
 }
 
@@ -171,7 +171,8 @@ __device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int 
 // carries none of its registers).
 // POLICY = the actions come from the in-kernel heuristic policy instead of the action tensor (again a
 // separate instantiation: the open-loop kernel carries none of its instructions).
-template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false>
+// KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false, bool KEEP = false>
 __global__ void __launch_bounds__(32, (OPL <= 4 ? 28 : 16))
 ww_kernel(const __grid_constant__ WWParams<real, O> p) {
   const real INF = real_inf<real>();
@@ -542,7 +543,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
           }
           }
           if (!p.stage_step) {
-            obs_row_store(stage + slot_off, obs_row, n_feat * K, lane);
+            obs_row_store<KEEP>(stage + slot_off, obs_row, n_feat * K, lane);
             slot_off = slot_bytes - slot_off;
           }
           if constexpr (POLICY) {   // sum over the sensors; lane pi keeps pursuer pi's next action
@@ -590,12 +591,12 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             stage_obs<O>(a + (uint32_t)sizeof(O), vP);
             if (p.addid) stage_obs<O>(a + 2 * (uint32_t)sizeof(O), id);
           } else {
-            store_stream(obs_t + i, obs_cvt<O>(vE));
-            store_stream(obs_t + i + 1, obs_cvt<O>(vP));
-            if (p.addid) store_stream(obs_t + i + 2, obs_cvt<O>(id));
+            store_obs<KEEP>(obs_t + i, obs_cvt<O>(vE));
+            store_obs<KEEP>(obs_t + i + 1, obs_cvt<O>(vP));
+            if (p.addid) store_obs<KEEP>(obs_t + i + 2, obs_cvt<O>(id));
           }
         }
-        if (p.stage_step) obs_row_store(stage, obs_t, p.Np * p.D, lane);
+        if (p.stage_step) obs_row_store<KEEP>(stage, obs_t, p.Np * p.D, lane);
         if (!pass && lane < p.Np) {
           real r = pen;
           if (p.reward_global) {
@@ -777,6 +778,10 @@ extern "C" int madrl_ww_set_obs_format(madrl_ww* h, int format) {
   return engine_set_obs_format(h, format, h != nullptr && h->cfg.fp64);
 }
 
+extern "C" int madrl_ww_set_obs_cache(madrl_ww* h, int mode) {
+  return engine_set_obs_cache(h, mode, h != nullptr && h->cfg.fp64);
+}
+
 extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm) {
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
@@ -810,11 +815,11 @@ extern "C" int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T) {
   return ww_default_blocks_per_sm(h, T);
 }
 
-template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY>
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY, bool KEEP = false>
 static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, int cap, cudaStream_t stream) {
   const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(O))
                                                                         : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(O)));
-  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY>, smem, p.E, stream, p, cap);
+  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY, KEEP>, smem, p.E, stream, p, cap);
 }
 
 // The fused peer exchange is instantiated for native observations only (bf16 rollouts with peers are
@@ -825,8 +830,11 @@ static int ww_launch_inst(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t 
   if constexpr (sizeof(O) == sizeof(real))
     if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, false>(h, p, 0, stream);
   // only the plain open-loop rollout was measured with the default cap
-  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, p.mode == 0 ? ww_default_blocks_per_sm(h, p.T) : 0,
-                                                               stream);
+  const int cap = p.mode == 0 ? ww_default_blocks_per_sm(h, p.T) : 0;
+  if constexpr (sizeof(real) == 4)   // set_obs_cache refuses KEEP on fp64 handles
+    if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
+      return ww_launch_inst2<real, O, OPL, KCH, KC, false, false, true>(h, p, cap, stream);
+  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, cap, stream);
 }
 
 template <typename real, typename O>

@@ -77,12 +77,22 @@ class BatchedEngine(object):
         self._term_obs = term_obs
         _lib.check(self._fn("set_terminal_obs")(self._h, _ptr(term_obs)))
 
+    # Counts the calls that change host-side handle settings a rollout launch copies into its kernel parameters
+    # (seed, set_launch, the families' set_params / set_peers): a CUDA graph holding earlier launches is stale
+    # once it changes (closed_loop.PolicyRollout re-captures).
+    launch_settings = 0
+
+    def _launch_settings_changed(self):
+        self.launch_settings += 1
+
     def set_launch(self, warps_per_block=0, blocks_per_sm=0):
         _lib.check(self._fn("set_launch")(self._h, warps_per_block, blocks_per_sm))
+        self._launch_settings_changed()
 
     def seed(self, seed=None):
         with torch.cuda.device(self.device):
             _lib.check(self._fn("seed")(self._h, 0 if seed is None else int(seed), _lib.stream(self.device)))
+        self._launch_settings_changed()
         return [seed]
 
     def reset(self, mask=None, out=None):
@@ -150,11 +160,24 @@ class BatchedEngine(object):
                                                      _lib.stream(self.device)))
         return act, obs, rew, done, info
 
-    def step(self, actions, auto_reset=False):
-        """One lockstep step.  actions [E, A, *act_tail] (or anything reshapeable to it)."""
+    def set_obs_cache(self, mode):
+        """L2 policy of the observation stores of rollout() and step(): _lib.OBS_CACHE_STREAM (the default,
+        evict-first) or _lib.OBS_CACHE_KEEP (normal priority, for a policy that reads each step's observations
+        right after it; float32 engines only).  The values written are the same either way."""
+        _lib.check(self._fn("set_obs_cache")(self._h, int(mode)))
+        self.obs_cache = int(mode)
+
+    obs_cache = _lib.OBS_CACHE_STREAM
+
+    def step(self, actions, auto_reset=False, out=None):
+        """One lockstep step.  actions [E, A, *act_tail] (or anything reshapeable to it).  `out`: caller buffers
+        (obs [E, A, D], rew [E, A], done [E], info [E, *info_tail]) written instead of new tensors; the
+        returned values are then views of them."""
         a = torch.as_tensor(actions, device=self.device, dtype=self._act_dtype).reshape(
             (1, self.n_envs, self._n_acting) + self._act_tail)
-        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset)
+        if out is not None:
+            out = tuple(t.unsqueeze(0) if isinstance(t, torch.Tensor) else t for t in out)
+        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset, out=out)
         if len(self._info_keys) == 1:
             return obs[0], rew[0], done[0], {self._info_keys[0]: info[0]}
         return obs[0], rew[0], done[0], {k: info[0, :, i] for i, k in enumerate(self._info_keys)}

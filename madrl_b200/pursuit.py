@@ -108,6 +108,7 @@ class BatchedPursuitEvade(BatchedEngine):
         if constraint_window is not None:
             self.cfg.constraint_window = float(constraint_window)
         _lib.check(self._L.madrl_pursuit_set_params(self._h, self.cfg.catchr, self.cfg.constraint_window))
+        self._launch_settings_changed()
 
     def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, py2_division=True,
                           actions_out=None):

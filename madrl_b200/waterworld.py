@@ -118,10 +118,12 @@ class BatchedMAWaterWorld(BatchedEngine):
         self._peer_keepalive = (rew_peers, done_peers, info_peers)
         _lib.check(self._L.madrl_ww_set_peers(self._h, n, rank, t_max, arr(rew_peers), arr(done_peers),
                                               arr(info_peers)))
+        self._launch_settings_changed()
 
     def clear_peers(self):
         self._peer_keepalive = None
         _lib.check(self._L.madrl_ww_set_peers(self._h, 0, 0, 0, None, None, None))
+        self._launch_settings_changed()
 
     def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, actions_out=None):
         """T lockstep steps in one launch with the reference's hand-written policy
