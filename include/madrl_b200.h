@@ -413,6 +413,25 @@ int madrl_standardize_obs_terminal_f32(int T, int E, size_t per_env, float* x_de
 int madrl_standardize_obs_terminal_bf16(int T, int E, size_t per_env, void* x_dev, void* term_dev,
                                         const uint8_t* done_dev, double* mean_dev, double* var_dev,
                                         double alpha, double eps, void* stream);
+/* One closed-loop step of StandardizedEnv inside ObservationBuffer (madrl_b200.closed_loop.PolicyRollout), run
+ * after a one-step rollout launch: the values of madrl_standardize_obs_terminal_* then madrl_frame_stack_* at
+ * T = 1, bit for bit, in one pass.  obs, term [E][A][D] (the step's observations and terminal observations);
+ * done uint8 [E]; prev, out [E][A][D][B] (the stack the policy read at this step, and the next one); mean, var
+ * float64 [E][A][D] (the running estimates) or both NULL.
+ *   obsnorm (mean, var given): where done[e] is set the estimate is updated with term, which is written back
+ *                              standardised; then with obs, which is written back standardised, in place.
+ *   stack:                     out = the (standardised) obs in every slot where done[e] is set, otherwise prev
+ *                              shifted left by one slot with it in slot B-1.  With B = 1, prev is not read and
+ *                              out may be NULL (obsnorm only).
+ * MADRL_EINVAL for E, A or D < 1, B outside [1, 8], NULL obs or done, only one of mean / var, mean without term,
+ * or B > 1 without prev and out. */
+int madrl_obs_wrap_step_f32(int E, int A, int D, int B, float* obs_dev, float* term_dev, const uint8_t* done_dev,
+                            const float* prev_dev, float* out_dev, double* mean_dev, double* var_dev, double alpha,
+                            double eps, void* stream);
+/* Same over bfloat16 obs, term, prev and out, rounded as madrl_standardize_bf16. */
+int madrl_obs_wrap_step_bf16(int E, int A, int D, int B, void* obs_dev, void* term_dev, const uint8_t* done_dev,
+                             const void* prev_dev, void* out_dev, double* mean_dev, double* var_dev, double alpha,
+                             double eps, void* stream);
 /* DiagnosticsWrapper episode statistics (madrl_environments/__init__.py:314-369): rew [T][E][A],
  * done uint8 [T][E]; carry float64 [E][A+3] (zero-initialised by the caller, kept between calls);
  * outputs at the steps where an episode closes (ep_end[t][e] = 1; zeros elsewhere):

@@ -158,6 +158,8 @@ def _signatures():
         "madrl_standardize_bf16": (i32, [i32, sz, vp, vp, vp, f64, f64, i32, f64, i32, vp]),
         "madrl_standardize_obs_terminal_f32": (i32, [i32, i32, sz] + [vp] * 5 + [f64, f64, vp]),
         "madrl_standardize_obs_terminal_bf16": (i32, [i32, i32, sz] + [vp] * 5 + [f64, f64, vp]),
+        "madrl_obs_wrap_step_f32": (i32, [i32] * 4 + [vp] * 7 + [f64, f64, vp]),
+        "madrl_obs_wrap_step_bf16": (i32, [i32] * 4 + [vp] * 7 + [f64, f64, vp]),
         "madrl_episode_stats_f32": (i32, [i32, i32, i32, vp, vp, f64, i32, vp, vp, vp, vp, vp, vp]),
         # moments and advantage centring
         "madrl_moments_f32": (i32, [sz, vp, vp, vp, vp, vp]),

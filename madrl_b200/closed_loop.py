@@ -9,6 +9,9 @@ architecture: MLP, GRU, LSTM, conv), and the env kernels stay policy-free.
 
 The outputs are the tensors ``postproc.process_samples_recurrent`` / ``process_samples_concurrent`` and
 ``rltools_sampler.process_samples`` take, with ``obs_before = obs0``.
+
+With ``frame_stack=B`` and / or ``standardizer=`` the policy reads observations wrapped as the reference's
+``StandardizedEnv`` inside ``ObservationBuffer`` wrap them, one fused kernel per step (madrl_obs_wrap_step_*).
 """
 import collections
 import contextlib
@@ -16,8 +19,9 @@ import contextlib
 import torch
 
 from . import _lib
+from ._lib import _ptr
 
-Rollout = collections.namedtuple("Rollout", "actions obs rew done info extras state")
+Rollout = collections.namedtuple("Rollout", "actions obs rew done info extras state policy_obs")
 
 
 def _map_state(fn, state):
@@ -85,22 +89,89 @@ class PolicyRollout(object):
     generator assigns the graph's random kernels one block of Philox offsets and moves its offset past that block
     at each replay, whereas the eager loop advances it kernel by kernel.
 
-    ``__call__(obs0, state0=None)`` returns a ``Rollout`` (actions, obs, rew, done, info, extras, state) of VIEWS
-    of the rollout's buffers: the next call overwrites them, so clone what must outlive it.
+    Observation wrappers (the reference's runners wrap the env as ``ObservationBuffer(StandardizedEnv(env),
+    buffer_size)``):
+    * ``standardizer``: a ``postproc.Standardizer`` of the engine's (E, A, D) on its device.  With
+      ``enable_obsnorm`` the policy reads observations standardised by the per-env running estimates, updated at
+      every step in the reference's order (at a done step the terminal observation first, then the reset one); the
+      Standardizer's float64 state is updated in place, so it carries over between calls and to open-loop use.
+      Its reward side (``enable_rewnorm``, ``scale_reward``) feeds no policy input and is applied to ``rew`` once
+      after the T steps (``Standardizer.rew``, inside the graph), which equals per-step application.
+    * ``frame_stack=B`` (1..8): the policy reads the last B observations as ``[E, A, D, B]`` (the newest in slot
+      B-1; after a reset every slot holds the reset observation).  ``obs.reshape(E, A, D * B)`` is the reference's
+      ``buffer.flatten()``.  ``obs0`` is then ``[E, A, D, B]``.
+    Either option runs one fused kernel after each step's launch (policy -> env launch -> wrapper kernel ->
+    recurrent-state reset).  ``obs`` then holds the standardised observations (with obsnorm) and
+    ``policy_obs[t]`` the wrapped observation step t returned: a new [T, E, A, D, B] buffer with B > 1 (at C2,
+    T = 256, B = 4: 17.9 GB in float32, 8.9 GB in bfloat16), ``obs`` itself with B = 1.  The sample-processing
+    passes take ``policy_obs.view(T, E, A, D * B)`` with ``obs_before = obs0.view(E, A, D * B)``.  Obsnorm needs
+    the terminal observations: the ``set_terminal_obs`` tensor when the caller has one, otherwise a private
+    one-step buffer, set for the loop and unset afterwards.  The start of a run::
+
+        o = engine.reset()
+        std.obs(o)                                           # the reset observation updates the estimate
+        obs0 = postproc.FrameStack(E, A, D, B, dev, engine.obs_dtype).reset(o)   # or o itself with B = 1
+
+    and each later call takes the previous call's ``policy_obs[-1]``.  The wrappers need float32 or bfloat16
+    observations, ``auto_reset`` and, for Pursuit, ``flatten=True`` (ObservationBuffer takes 1-D observations).
+
+    ``__call__(obs0, state0=None)`` returns a ``Rollout`` (actions, obs, rew, done, info, extras, state, policy_obs)
+    of VIEWS of the rollout's buffers: the next call overwrites them, so clone what must outlive it.
     """
 
-    def __init__(self, engine, policy, T, auto_reset=True, record=None, graph=True, obs_cache=None):
+    def __init__(self, engine, policy, T, auto_reset=True, record=None, graph=True, obs_cache=None, frame_stack=1,
+                 standardizer=None):
         self.engine, self.policy, self.T = engine, policy, T
         self.auto_reset, self.record, self.graph, self.obs_cache = auto_reset, record, graph, obs_cache
+        self.frame_stack, self.standardizer = frame_stack, standardizer
         self._key = None
         self._graph = None
+        self._check_wrappers()
+
+    def _check_wrappers(self):
+        """Raise for wrapper options the kernels or the reference do not support."""
+        B, std, eng = self.frame_stack, self.standardizer, self.engine
+        if not isinstance(B, int) or not 1 <= B <= 8:
+            raise ValueError("frame_stack must be an int in [1, 8], got %r" % (B,))
+        if B == 1 and std is None:
+            return
+        opt = "frame_stack" if std is None else "standardizer"
+        if not self.auto_reset:
+            raise ValueError("%s needs auto_reset=True (the wrappers restart at each env's reset)" % opt)
+        if eng.obs_dtype not in (torch.float32, torch.bfloat16):
+            raise TypeError("%s needs float32 or bfloat16 observations, the engine's are %s" % (opt, eng.obs_dtype))
+        if getattr(eng, "flatten", True) is False:
+            raise ValueError("%s needs a Pursuit engine with flatten=True (ObservationBuffer takes 1-D observations)"
+                             % opt)
+        if std is not None:
+            from .postproc import Standardizer
+            if not isinstance(std, Standardizer):
+                raise TypeError("standardizer must be a postproc.Standardizer, got %r" % type(std))
+            shape = (eng.n_envs, eng._n_acting, eng.obs_dim)
+            for t, n in ((std.obs_mean, "obs_mean"), (std.obs_var, "obs_var")):
+                _lib.require_tensor(t, "standardizer." + n, torch.float64, shape, eng.device)
+            for t, n in ((std.rew_mean, "rew_mean"), (std.rew_var, "rew_var")):
+                _lib.require_tensor(t, "standardizer." + n, torch.float64, shape[:2], eng.device)
+
+    def _wrapped(self):
+        """The fused wrapper kernel runs after every step."""
+        std = self.standardizer
+        return self.frame_stack > 1 or (std is not None and bool(std.enable_obsnorm))
+
+    def _obs0_shape(self):
+        eng = self.engine
+        return (eng.n_envs, eng._n_acting, eng.obs_dim) + ((self.frame_stack,) if self.frame_stack > 1 else ())
 
     def _settings(self, state0):
-        eng = self.engine
+        eng, std = self.engine, self.standardizer
         term = eng._term_obs if self.auto_reset else None
+        wrap = None if std is None else (
+            id(std), tuple(t.data_ptr() for t in (std.obs_mean, std.obs_var, std.rew_mean, std.rew_var)),
+            float(std.obs_alpha), float(std.rew_alpha), float(std.eps), bool(std.enable_obsnorm),
+            bool(std.enable_rewnorm), float(std.scale_reward))
         return (self.T, id(eng), eng.obs_dtype, None if term is None else (term.data_ptr(), tuple(term.shape)),
                 eng.launch_settings, self.auto_reset, self.graph, self._obs_cache(), self.record,
-                tuple((tuple(s.shape), s.dtype) for s in _flat(state0)), state0 is None)
+                tuple((tuple(s.shape), s.dtype) for s in _flat(state0)), state0 is None, self.frame_stack, wrap)
 
     def _obs_cache(self):
         if self.obs_cache is not None:
@@ -114,13 +185,43 @@ class PolicyRollout(object):
         E, A, dev = eng.n_envs, eng._n_acting, eng.device
         self._act = torch.zeros((T, E, A) + eng._act_tail, dtype=eng._act_dtype, device=dev)
         self._traj = tuple(torch.zeros(s, dtype=dt, device=dev) for dt, s in eng._trajectory_shapes(T))
-        self._obs0 = torch.zeros((E, A, eng.obs_dim), dtype=eng.obs_dtype, device=dev)
+        self._obs0 = torch.zeros(self._obs0_shape(), dtype=eng.obs_dtype, device=dev)
         self._state0 = _map_state(torch.clone, state0)
         self._term = eng._term_obs if self.auto_reset else None
         if self._term is not None:
             _lib.require_tensor(self._term, "the set_terminal_obs tensor", eng.obs_dtype, (T, E, A, eng.obs_dim), dev)
+        self._check_wrappers()
+        std = self.standardizer
+        obsnorm = std is not None and bool(std.enable_obsnorm)
+        # the terminal observations obsnorm reads: a private one-step buffer when the caller keeps none
+        self._term1 = None
+        if obsnorm and self._term is None:
+            self._term1 = torch.zeros((1, E, A, eng.obs_dim), dtype=eng.obs_dtype, device=dev)
+        self._stats = (std.obs_mean, std.obs_var) if obsnorm else None
+        self._policy_obs = self._traj[0]
+        if self.frame_stack > 1:
+            self._policy_obs = torch.zeros((T,) + self._obs0_shape(), dtype=eng.obs_dtype, device=dev)
         self._extras = None   # allocated at the first policy call: shapes and dtypes are the policy's
         self._graph = None
+
+    def _wrap_step(self, t):
+        """madrl_obs_wrap_step_* of step t: standardise obs[t] (and term[t]) in place, stack into policy_obs[t]."""
+        eng, B = self.engine, self.frame_stack
+        obs, _, done, _ = self._traj
+        E, A, D = eng.n_envs, eng._n_acting, eng.obs_dim
+        term = None
+        if self._stats is not None:
+            term = self._term1[0] if self._term1 is not None else self._term[t]
+        prev = out = None
+        if B > 1:
+            prev = self._obs0 if t == 0 else self._policy_obs[t - 1]
+            out = self._policy_obs[t]
+        mean, var = self._stats if self._stats is not None else (None, None)
+        std = self.standardizer
+        fn = getattr(_lib.lib(), "madrl_obs_wrap_step_%s" % ("bf16" if eng.obs_dtype == torch.bfloat16 else "f32"))
+        _lib.check(fn(E, A, D, B, _ptr(obs[t]), _ptr(term), _ptr(done[t]), _ptr(prev), _ptr(out), _ptr(mean),
+                      _ptr(var), float(std.obs_alpha) if std is not None else 0.0,
+                      float(std.eps) if std is not None else 0.0, _lib.stream(eng.device)))
 
     def _record_buffers(self, extras):
         keys = extras.keys() if self.record is None else self.record
@@ -133,6 +234,7 @@ class PolicyRollout(object):
         obs, rew, done, info = self._traj
         state = self._state0
         prev = self._obs0
+        wrapped = self._wrapped()
         for t in range(self.T):
             a, extras, state = self.policy(prev, state)
             if self._extras is None:
@@ -144,22 +246,29 @@ class PolicyRollout(object):
                 eng.set_terminal_obs(self._term[t:t + 1])
             eng.rollout(self._act[t:t + 1], auto_reset=self.auto_reset,
                         out=(obs[t:t + 1], rew[t:t + 1], done[t:t + 1], info[t:t + 1]))
+            if wrapped:
+                self._wrap_step(t)
             state = reset_state(state, done[t])
-            prev = obs[t]
+            prev = self._policy_obs[t]
+        if self.standardizer is not None:
+            self.standardizer.rew(rew)
         return state
 
     @contextlib.contextmanager
     def _engine_settings(self):
-        """The engine with our obs cache mode (set before any capture begins, so a refused mode raises there);
-        its own mode and terminal-observation tensor are restored after."""
+        """The engine with our obs cache mode (set before any capture begins, so a refused mode raises there) and
+        our private terminal-observation buffer, if any; its own mode and terminal-observation tensor are restored
+        after."""
         eng = self.engine
         keep_mode, keep_term = eng.obs_cache, eng._term_obs
         eng.set_obs_cache(self._obs_cache())
         try:
+            if self._term1 is not None:
+                eng.set_terminal_obs(self._term1)
             yield
         finally:
             eng.set_obs_cache(keep_mode)
-            if self._term is not None:
+            if self._term is not None or self._term1 is not None:
                 eng.set_terminal_obs(keep_term)
 
     def _capture(self):
@@ -177,8 +286,7 @@ class PolicyRollout(object):
 
     def __call__(self, obs0, state0=None):
         eng = self.engine
-        _lib.require_tensor(obs0, "obs0", eng.obs_dtype, (eng.n_envs, eng._n_acting, eng.obs_dim), eng.device,
-                            contiguous=False)
+        _lib.require_tensor(obs0, "obs0", eng.obs_dtype, self._obs0_shape(), eng.device, contiguous=False)
         with torch.cuda.device(eng.device):
             key = self._settings(state0)
             if key != self._key:
@@ -196,7 +304,7 @@ class PolicyRollout(object):
                 with self._engine_settings():
                     state = self._loop()
         obs, rew, done, info = self._traj
-        return Rollout(self._act, obs, rew, done, info, dict(self._extras), state)
+        return Rollout(self._act, obs, rew, done, info, dict(self._extras), state, self._policy_obs)
 
 
 def _flat(state):

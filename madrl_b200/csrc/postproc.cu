@@ -92,6 +92,23 @@ __device__ __forceinline__ double inv_std(double v, double eps) {
   return r;
 }
 
+// One element's running-estimate update (__init__.py:258-262), shared by every standardiser kernel so that the
+// whole-rollout passes and the closed loop's per-step pass give the same bits.  The fused multiply-adds are
+// spelled out: left to contraction, nvcc fused `(1-a) m + a x` as fma(m, 1-a, a x) in one kernel and as
+// fma(x, a, (1-a) m) in another, so the running estimates drifted apart in their last bits.  These are the forms
+// the whole-rollout kernels were compiled to before.
+__device__ __forceinline__ void running_update(double x, double& m, double& v, double alpha) {
+  m = fma(m, 1.0 - alpha, alpha * x);
+  const double d = x - m;
+  v = fma(v, 1.0 - alpha, alpha * d * d);
+}
+
+// The update, then x standardised by the updated estimate (observations: centred).
+__device__ __forceinline__ double standardize_obs_one(double x, double& m, double& v, double alpha, double eps) {
+  running_update(x, m, v, alpha);
+  return (x - m) * inv_std(v, eps);
+}
+
 template <typename O>
 __global__ void standardize_kernel(int T, size_t n, O* __restrict__ x, double* __restrict__ mean,
                                    double* __restrict__ var, double alpha, double eps, int center,
@@ -104,9 +121,7 @@ __global__ void standardize_kernel(int T, size_t n, O* __restrict__ x, double* _
     const double xv = (double)obs_widen<float>(x[k]);
     double o = xv;
     if (enable) {
-      m = (1.0 - alpha) * m + alpha * xv;
-      const double d = xv - m;
-      v = (1.0 - alpha) * v + alpha * d * d;
+      running_update(xv, m, v, alpha);
       o = (center ? (xv - m) : xv) * inv_std(v, eps);
     }
     x[k] = obs_cvt<O>((float)(scale * o));
@@ -128,21 +143,46 @@ __global__ void standardize_terminal_kernel(int T, int E, size_t per_env, O* __r
   double m = mean[i], v = var[i];
   for (int t = 0; t < T; ++t) {
     const size_t k = (size_t)t * n + i;
-    if (done[(size_t)t * E + e]) {                 // step(): the terminal observation comes first
-      const double tv = (double)obs_widen<float>(term[k]);
-      m = (1.0 - alpha) * m + alpha * tv;
-      const double d = tv - m;
-      v = (1.0 - alpha) * v + alpha * d * d;
-      term[k] = obs_cvt<O>((float)((tv - m) * inv_std(v, eps)));
-    }
-    const double xv = (double)obs_widen<float>(x[k]);
-    m = (1.0 - alpha) * m + alpha * xv;
-    const double d = xv - m;
-    v = (1.0 - alpha) * v + alpha * d * d;
-    x[k] = obs_cvt<O>((float)((xv - m) * inv_std(v, eps)));
+    if (done[(size_t)t * E + e])                   // step(): the terminal observation comes first
+      term[k] = obs_cvt<O>((float)standardize_obs_one((double)obs_widen<float>(term[k]), m, v, alpha, eps));
+    x[k] = obs_cvt<O>((float)standardize_obs_one((double)obs_widen<float>(x[k]), m, v, alpha, eps));
   }
   mean[i] = m;
   var[i] = v;
+}
+
+// One closed-loop step of StandardizedEnv inside ObservationBuffer (PolicyRollout with a Standardizer and / or
+// frame_stack > 1), right after the engine's one-step launch: the same values as standardize_terminal_kernel then
+// frame_stack_kernel at T = 1, in one pass.  With mean / var (obsnorm): where done[e] is set the estimate is first
+// updated with term (written back standardised), then with obs (written back standardised, in place).  Then the
+// stack: out = the new value in every slot where done is set, else prev shifted left by one with the new value in
+// slot B-1.  B = 1 needs no prev; out may be NULL there.  mean / var and prev are read once per step (evict-first);
+// obs was just written by the launch and out is read by the policy next, so both keep normal L2 priority.
+template <int B, typename O>
+__global__ void obs_wrap_step_kernel(size_t n /* E*A*D */, size_t per_env, O* __restrict__ obs,
+                                     O* __restrict__ term, const uint8_t* __restrict__ done,
+                                     const O* __restrict__ prev, O* __restrict__ out, double* __restrict__ mean,
+                                     double* __restrict__ var, double alpha, double eps) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const bool reset = done[i / per_env] != 0;
+  O x = obs[i];
+  if (mean) {
+    double m = __ldcs(mean + i), v = __ldcs(var + i);
+    if (reset)
+      term[i] = obs_cvt<O>((float)standardize_obs_one((double)obs_widen<float>(term[i]), m, v, alpha, eps));
+    x = obs_cvt<O>((float)standardize_obs_one((double)obs_widen<float>(x), m, v, alpha, eps));
+    obs[i] = x;
+    __stcs(mean + i, m);
+    __stcs(var + i, v);
+  }
+  if (!out) return;
+  O buf[B];
+#pragma unroll
+  for (int b = 0; b < B - 1; ++b) buf[b] = reset ? x : __ldcs(prev + i * B + b + 1);
+  buf[B - 1] = x;
+#pragma unroll
+  for (int b = 0; b < B; ++b) out[i * B + b] = buf[b];
 }
 
 // DiagnosticsWrapper episode statistics (madrl_environments/__init__.py:314-369): per env, walk the
@@ -813,6 +853,41 @@ extern "C" int madrl_standardize_obs_terminal_bf16(int T, int E, size_t per_env,
                                                    double alpha, double eps, void* stream) {
   return standardize_obs_terminal(T, E, per_env, (uint16_t*)x_dev, (uint16_t*)term_dev, done_dev, mean_dev, var_dev,
                                   alpha, eps, stream);
+}
+
+template <typename O>
+static int obs_wrap_step(int E, int A, int D, int B, O* obs_dev, O* term_dev, const uint8_t* done_dev,
+                         const O* prev_dev, O* out_dev, double* mean_dev, double* var_dev, double alpha, double eps,
+                         void* stream) {
+  MADRL_REQUIRE(E >= 1 && A >= 1 && D >= 1, "bad sizes");
+  MADRL_REQUIRE(B >= 1 && B <= 8, "buffer_size must be in [1,8], got %d", B);
+  MADRL_REQUIRE(obs_dev && done_dev, "NULL buffer");
+  MADRL_REQUIRE(!mean_dev == !var_dev, "mean and var must both be given (obsnorm) or both be NULL");
+  MADRL_REQUIRE(!mean_dev || term_dev, "obsnorm needs the terminal observations");
+  MADRL_REQUIRE(B == 1 || (prev_dev && out_dev), "buffer_size > 1 needs prev and out");
+  const size_t per_env = (size_t)A * D, n = (size_t)E * per_env;
+  const unsigned grid = (unsigned)((n + 255) / 256);
+  cudaStream_t s = (cudaStream_t)stream;
+#define MADRL_WS(BB) case BB: MADRL_LAUNCH((obs_wrap_step_kernel<BB, O>), grid, 256, 0, s, n, per_env, obs_dev, term_dev, done_dev, prev_dev, out_dev, mean_dev, var_dev, alpha, eps); break
+  switch (B) { MADRL_WS(1); MADRL_WS(2); MADRL_WS(3); MADRL_WS(4); MADRL_WS(5); MADRL_WS(6); MADRL_WS(7); MADRL_WS(8); }
+#undef MADRL_WS
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_obs_wrap_step_f32(int E, int A, int D, int B, float* obs_dev, float* term_dev,
+                                       const uint8_t* done_dev, const float* prev_dev, float* out_dev,
+                                       double* mean_dev, double* var_dev, double alpha, double eps, void* stream) {
+  return obs_wrap_step(E, A, D, B, obs_dev, term_dev, done_dev, prev_dev, out_dev, mean_dev, var_dev, alpha, eps,
+                       stream);
+}
+
+extern "C" int madrl_obs_wrap_step_bf16(int E, int A, int D, int B, void* obs_dev, void* term_dev,
+                                        const uint8_t* done_dev, const void* prev_dev, void* out_dev,
+                                        double* mean_dev, double* var_dev, double alpha, double eps, void* stream) {
+  return obs_wrap_step(E, A, D, B, (uint16_t*)obs_dev, (uint16_t*)term_dev, done_dev, (const uint16_t*)prev_dev,
+                       (uint16_t*)out_dev, mean_dev, var_dev, alpha, eps, stream);
 }
 
 template <typename O>
