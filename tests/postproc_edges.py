@@ -377,3 +377,135 @@ def plan_paths(n_ep, ep_rec, T, A):
             s, L, term = ep_rec[e, j]
             out += [(e, a, bool(term), e * T * A + s * A + a * L, L, e * T + s) for a in range(A)]
     return out
+
+
+def path_records(done, A, agent_major=False):
+    """int32 [P, 4] (env, agent, start, length) of the paths of done [T, E] (cut at done and at the end of the
+    rollout), in (env, episode, agent) order, or (agent, env, episode) with agent_major: the padded-path table."""
+    T, E = done.shape
+    eps = []
+    for e in range(E):
+        s = 0
+        for t in range(T):
+            if done[t, e] or t == T - 1:
+                eps.append((e, s, t + 1 - s))
+                s = t + 1
+    recs = [(e, a, s, n) for a in range(A) for e, s, n in eps] if agent_major else \
+        [(e, a, s, n) for e, s, n in eps for a in range(A)]
+    return np.array(recs, np.int32).reshape(-1, 4)
+
+
+def sequential_sum(x):
+    """float64 sum of x from left to right, one rounding per term (Python >= 3.12's sum() of floats compensates)."""
+    acc = 0.0
+    for v in np.asarray(x, np.float64).ravel():
+        acc += float(v)
+    return acc
+
+
+# ---------------------------------------------------------------- rltools' sample processing
+
+def slice_rows(S):
+    """Rows per group around a kernel's S row slices: one row, every slice empty but one or holding one row, and
+    the 8-warp stride of a slice."""
+    return tuple(sorted({r for r in (1, S - 1, S, S + 1, 8 * S - 1, 8 * S + 1) if r >= 1}))
+
+
+def mixed_scale(rs, *shape):
+    """float32 values whose magnitudes span 1e-3 .. 1e3 (so that an absolute error bound is not trivially loose)."""
+    return (rs.randn(*shape) * 10.0 ** rs.randint(-3, 4, size=shape) + 0.25).astype(np.float32)
+
+
+def check_column_sums(got, rows):
+    """got [G, 2, D]: per group g the float64 column sums of x and x^2 over rows[:, g] (rows [n, G, D], widened
+    float32, so every square is exact in float64), each within n 2^-52 sum|.| of NumPy's float64 sum."""
+    n = rows.shape[0]
+    for j, v in enumerate((rows, rows * rows)):
+        err = np.abs(got[:, j] - v.sum(0))
+        assert np.all(err <= n * 2.0 ** -52 * np.abs(v).sum(0)), (j, err.max())
+
+
+def time_index(done, t0=None):
+    """(idx, path) [T, E]: the time index of every (t, e) -- its position in its path plus t0[e] on env e's first
+    path, the baseline's lfb_index -- and its path's number, paths numbered env by env in time order."""
+    T, E = done.shape
+    idx, path = np.zeros((T, E), np.int64), np.zeros((T, E), np.int64)
+    p = 0
+    for e in range(E):
+        s = 0
+        for t in range(T):
+            idx[t, e] = t - s + (t0[e] if (t0 is not None and s == 0) else 0)
+            path[t, e] = p
+            if done[t, e] or t == T - 1:
+                s, p = t + 1, p + 1
+    return idx, path
+
+
+def time_baseline_case(T, E, A, L, seed):
+    """q [T,E,A], done [T,E] and t0 whose largest time index is L - 1: env 0 runs the whole horizon, env 1 ends a
+    path on every step, the others at random.  L == T: no t0; L > T: env 0's t0 = L - T carries the index past T
+    (the other envs' t0 stay below it)."""
+    assert 1 <= T <= L
+    rs = np.random.RandomState(seed)
+    done = (rs.rand(T, E) < 0.2).astype(np.uint8)
+    done[:, 0] = 0
+    if E > 1:
+        done[:, 1] = 1
+    t0 = None
+    if L > T:
+        t0 = rs.randint(0, L - T + 1, size=E).astype(np.int32)
+        t0[0] = L - T
+    return mixed_scale(rs, T, E, A), done, t0
+
+
+def check_time_baseline(simplev, bin_sum, bin_cnt, q, done, t0, per_agent):
+    """Counts exact; sums within n 2^-52 sum|q| of NumPy's; simplev the returned bins' float64 quotient rounded to
+    float32, bit for bit; and that quotient within float32 rounding of NumPy's nanmean over the NaN-padded paths
+    (Sampler.process's simplev)."""
+    T, E, A = q.shape
+    idx, path = time_index(done, t0)
+    G, L = (A if per_agent else 1), int(idx.max()) + 1
+    assert bin_sum.shape == (G, L) and bin_cnt.shape == (G, L)
+    q64 = q.astype(np.float64)
+    s, c, mag = np.zeros((G, L)), np.zeros((G, L), np.int64), np.zeros((G, L))
+    for a in range(A):
+        g = a if per_agent else 0
+        np.add.at(s[g], idx, q64[..., a])
+        np.add.at(c[g], idx, 1)
+        np.add.at(mag[g], idx, np.abs(q64[..., a]))
+    assert np.array_equal(bin_cnt, c)
+    tol = c * 2.0 ** -52 * mag
+    assert np.all(np.abs(bin_sum - s) <= tol), np.abs(bin_sum - s).max()
+    grp = np.arange(A) if per_agent else np.zeros(A, np.int64)
+    got_bin = bin_sum[grp[None, None, :], idx[..., None]] / bin_cnt[grp[None, None, :], idx[..., None]]
+    assert np.array_equal(simplev, got_bin.astype(np.float32))
+    P = int(path.max()) + 1
+    for g in range(G):
+        agents = [g] if per_agent else list(range(A))
+        pad = np.full((P * len(agents), L), np.nan)
+        for k, a in enumerate(agents):
+            pad[path * len(agents) + k, idx] = q64[..., a]
+        m = c[g] > 0                     # a bin no row reaches (below a t0) is never read
+        want = np.nanmean(pad[:, m], axis=0)
+        got = bin_sum[g, m] / bin_cnt[g, m]
+        assert np.all(np.abs(got - want) <= 4 * np.spacing(np.abs(want)) + tol[g, m] / c[g, m]), g
+
+
+def lfbr_single_row_obs(D, k, bf16, rs):
+    """D finite observation values for rltools' unclipped feature map: 0, +-1, +-1e30, +-2^-130 (subnormal in
+    float32 and bfloat16), +-3e4, rotated by k so that every position sees each of them, the rest random."""
+    special = [0.0, 1.0, -1.0, 1e30, -1e30, 2.0 ** -130, -2.0 ** -130, 3e4, -3e4]
+    o = (rs.randn(D) * 8).astype(np.float32)
+    for i in range(0, D, 2):
+        o[i] = special[(k + i // 2) % len(special)]
+    return bf16_bits(o)[1] if bf16 else o
+
+
+def lfbr_features(seen, idx, norm):
+    """rltools' features [(o - mu) / s, a, a * a, 1] (Df = D + 3) in float64 of rows seen [..., D] (widened
+    float32), time indices idx [...] (a = idx / 100, one rounding) and norm [..., 2, D] = (mu, s) or None."""
+    o = np.asarray(seen, np.float64)
+    if norm is not None:
+        o = (o - norm[..., 0, :]) / norm[..., 1, :]
+    a = np.asarray(idx, np.float64)[..., None] / 100.0
+    return np.concatenate([o, a, a * a, np.ones_like(a)], axis=-1)
