@@ -145,11 +145,23 @@ int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream);
  * (= one env); `warps_per_block` is range-checked ([0,4]) for ABI stability and otherwise ignored.  The same
  * holds for madrl_pursuit_set_launch and madrl_hostage_set_launch, whose default is as many as fit. */
 int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm);
-/* The library default's cap on resident blocks per SM for an open-loop rollout of T steps of this handle
+/* The library default's cap on resident env warps per SM for an open-loop rollout of T steps of this handle
  * (madrl_ww_rollout / _step / _rollout_host*): 16 for some float32-observation batches (DESIGN §4.3), else 0
- * = as many as fit.  Resets, heuristic-policy and peer-exchange rollouts always use as many as fit.
+ * = as many as fit.  Where it caps, the writer-warp kernel runs if it can (madrl_ww_set_obs_writer), else
+ * one-warp blocks.  Resets, heuristic-policy and peer-exchange rollouts always use as many as fit.
  * Negative on error. */
 int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T);
+/* Observation write path of Waterworld's float32 open-loop rollouts (madrl_ww_rollout / _step / _rollout_host*).
+ * The writer-warp kernel runs blocks of 8 warps that step 8 adjacent envs and stage each step's rows in shared
+ * memory, plus one warp that copies those rows to the observation tensor (DESIGN §4.1).  It needs at most 32
+ * objects, the env-step's rows to be staged whole (as for C2) and a 16-byte-aligned obs pointer and step stride (n_envs * n_pursuers *
+ * obs_dim a multiple of 4).  AUTO (the default): it replaces the launches madrl_ww_default_blocks_per_sm caps,
+ * whose cap then counts env warps per SM, unless madrl_ww_set_launch set a geometry.  ON: wherever it can run.
+ * OFF: never.  Every value written is the same on either path.  MADRL_EINVAL for an unknown mode. */
+#define MADRL_WW_OBS_WRITER_AUTO 0
+#define MADRL_WW_OBS_WRITER_OFF 1
+#define MADRL_WW_OBS_WRITER_ON 2
+int madrl_ww_set_obs_writer(madrl_ww* h, int mode);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
  * terminal one.  After this call every `*_rollout` (device pointers) with auto_reset first copies the rows

@@ -21,6 +21,8 @@ class EngineError(RuntimeError):
 OBS_NATIVE, OBS_BF16 = 0, 1
 # L2 policy of the rollouts' observation stores (madrl_*_set_obs_cache)
 OBS_CACHE_STREAM, OBS_CACHE_KEEP = 0, 1
+# Waterworld's observation write path (madrl_ww_set_obs_writer)
+WW_OBS_WRITER_AUTO, WW_OBS_WRITER_OFF, WW_OBS_WRITER_ON = 0, 1, 2
 
 
 class WWConfig(C.Structure):
@@ -143,6 +145,7 @@ def _signatures():
             ("rollout_host2", (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32]))))
     sig.update({
         "madrl_ww_default_blocks_per_sm": (i32, [vp, i32]),
+        "madrl_ww_set_obs_writer": (i32, [vp, i32]),
         "madrl_ww_set_peers": (i32, [vp, i32, i32, i32, P(vp), P(vp), P(vp)]),
         "madrl_ww_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
         "madrl_pursuit_set_params": (i32, [vp, f64, f64]),

@@ -199,6 +199,32 @@ __device__ __forceinline__ void bulk_wait_read_all_but_1() { asm volatile("cp.as
 __device__ __forceinline__ void bulk_wait_all() {
   asm volatile("cp.async.bulk.wait_group 0;\n\tfence.proxy.async.global;" ::: "memory");
 }
+// mbarriers in shared memory (Waterworld's writer-warp ring): init with the number of arrivals that complete a
+// phase; arrive (release, CTA scope) `count` of them; wait until the phase of parity `parity` has completed
+// (acquire).  A barrier in its first phase counts the phase before it, parity 1, as completed.
+__device__ __forceinline__ void mbar_init(uint32_t a, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(a), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t a, uint32_t count) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t a, uint32_t parity) {
+  asm volatile("{ .reg .pred p;\n\t"
+               "WAIT:\n\t"
+               "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+               "@!p bra WAIT; }" ::"r"(a), "r"(parity) : "memory");
+}
+// The writer warp's reads of Waterworld's writer-warp ring, which the ring's mbarriers order after the env warps'
+// staging: 16 bytes, one float, or a 16-byte-aligned run as one evict-first bulk store (bulk_store_stream).  And
+// 16 bytes to global memory evict-first (bits moved unchanged).
+__device__ __forceinline__ float4 ring_lds_f32x4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ float ring_lds_f32(uint32_t a) { return lds_f32(a); }
+__device__ __forceinline__ void ring_bulk_store(void* dst, uint32_t src, uint32_t bytes) { bulk_store_stream(dst, src, bytes); }
+__device__ __forceinline__ void stcs_f32x4(void* p, float4 v) { __stcs(reinterpret_cast<float4*>(p), v); }
 // bfloat16 bits of v, rounded to nearest even (cvt.rn), as a plain uint16_t: no cuda_bf16.h type enters the
 // kernels.  The pair form packs `lo` into bits 0-15 (the lower address) and `hi` into bits 16-31.
 __device__ __forceinline__ uint16_t bf16_rn(float v) {
@@ -238,6 +264,65 @@ static inline void bulk_store_keep(void* dst, uint32_t src, uint32_t bytes) { bu
 static inline void bulk_wait_read_all() {}
 static inline void bulk_wait_read_all_but_1() {}
 static inline void bulk_wait_all() {}
+// mbarriers, on the emulator's warp rendezvous alone.  A barrier's state is its 8 bytes of shared memory: the
+// arrivals still pending in the current phase, and the init count with the parity of the current phase in bit 31.
+// Arrivals and waits are not plain accesses, so the hazard checker does not see them.  A wait is made by all
+// lanes of a warp (as the kernels do): they poll together through warp_exchange, which hands the fiber schedule
+// to the other warps, and leave together once every lane has seen the phase complete.  Polling long after the
+// last arrival anywhere means a phase that never completes, i.e. a missing arrival: reported, then abort.
+static long g_emu_mbar_arrivals = 0;
+static inline void mbar_init(uint32_t a, uint32_t count) {
+  const uint32_t st[2] = {count, count};
+  memcpy(emu_at(a), st, 8);
+}
+static inline void mbar_arrive(uint32_t a, uint32_t count) {
+  uint32_t st[2];
+  memcpy(st, emu_at(a), 8);
+  if (count == 0 || count > st[0]) {
+    fprintf(stderr, "madrl_emu: mbarrier at offset %u: %u arrivals, %u pending in the phase\n", a, count, st[0]);
+    abort();
+  }
+  st[0] -= count;
+  if (st[0] == 0) { st[1] ^= 1u << 31; st[0] = st[1] & 0x7fffffffu; }   // phase complete: the next one starts
+  memcpy(emu_at(a), st, 8);
+  ++g_emu_mbar_arrivals;
+}
+static inline void mbar_wait(uint32_t a, uint32_t parity) {
+  long seen = g_emu_mbar_arrivals, idle = 0;
+  while (true) {
+    uint32_t st[2];
+    memcpy(st, emu_at(a), 8);
+    const bool done = (st[1] >> 31) != (parity & 1u);   // the phase of that parity is no longer the current one
+    const uint64_t* all = madrl_emu::warp_exchange(done ? 1u : 0u);
+    bool every = true;
+    for (int l = 0; l < 32; ++l) every = every && (all[l] & 1u);
+    if (every) return;
+    if (g_emu_mbar_arrivals != seen) { seen = g_emu_mbar_arrivals; idle = 0; }
+    else if (++idle > (1L << 20)) {
+      fprintf(stderr, "madrl_emu: mbarrier at offset %u never completes its phase of parity %u (block %u): a missing arrival\n",
+              a, parity & 1u, blockIdx.x);
+      abort();
+    }
+  }
+}
+// The writer warp's reads of the ring are ordered by the mbarriers, which the hazard checker (per-lane counts of
+// __syncwarp / __syncthreads) cannot follow across warps, so they are not recorded; the env warps' accesses are.
+static inline float4 ring_lds_f32x4(uint32_t a) { float4 v; memcpy(&v, emu_at(a), 16); return v; }
+static inline float ring_lds_f32(uint32_t a) { float v; memcpy(&v, emu_at(a), 4); return v; }
+static inline void ring_bulk_store(void* dst, uint32_t src, uint32_t bytes) {
+  if (((uintptr_t)dst | src | bytes) & 15u) {
+    fprintf(stderr, "madrl_emu: misaligned bulk store dst=%p src=%u bytes=%u\n", dst, src, bytes);
+    abort();
+  }
+  memcpy(dst, emu_at(src), bytes);
+}
+static inline void stcs_f32x4(void* p, float4 v) {
+  if ((uintptr_t)p & 15u) {
+    fprintf(stderr, "madrl_emu: misaligned 16-byte store %p\n", p);
+    abort();
+  }
+  memcpy(p, &v, 16);
+}
 // Round-to-nearest-even on the bit pattern, as cvt.rn.bf16.f32 rounds finite values and infinities.  A NaN
 // maps to some NaN here; which one the hardware returns is not modelled (observations are never NaN).
 static inline uint16_t bf16_rn(float v) {
@@ -309,6 +394,12 @@ __device__ __forceinline__ void keep_terminal_rows(const T* src, T* dst, int n, 
   __syncwarp();                                   // the rows were stored by other lanes of this warp
   for (int i = lane; i < n; i += 32) dst[i] = __ldcg(src + i);
   __syncwarp();                                   // ... and the reset pass overwrites them next
+}
+// The same from rows still staged in shared memory at `src` (the caller has synced the warp after staging them).
+template <typename O>
+__device__ __forceinline__ void keep_terminal_rows_staged(uint32_t src, O* dst, int n, int lane) {
+  for (int i = lane; i < n; i += 32) dst[i] = lds_obs<O>(src + (uint32_t)(i * sizeof(O)));
+  __syncwarp();                                   // the reset pass overwrites them next
 }
 
 template <typename real>

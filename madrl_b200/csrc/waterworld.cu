@@ -6,7 +6,8 @@
 //   * One WARP owns one env for the WHOLE T-step rollout.  The env's state lives in REGISTERS:
 //     lane l holds objects l, l+32, ... (position + velocity); objects are ordered pursuers,
 //     evaders, poisons.  There is no block barrier anywhere (blocks are one warp, and shared memory
-//     is the warp's own): warps are completely independent, so the SM's schedulers overlap the
+//     is the warp's own; the WRITER instantiation's blocks add a warp that writes 8 env warps'
+//     observations, see ww_obs_writer): warps are completely independent, so the SM's schedulers overlap the
 //     phases of different envs.  HBM sees the state once per launch (a coalesced per-env record)
 //     and, per step, only actions in and obs / reward / done / info out.
 //   * Per step and pursuer, lanes act first as OBJECTS (relative position, squared distance,
@@ -22,6 +23,7 @@
 #include <math.h>
 #include <cmath>
 #include <new>
+#include <type_traits>
 
 #include "common.cuh"
 #include "engine.cuh"
@@ -126,6 +128,46 @@ __host__ __device__ __forceinline__ uint32_t obs_stage_bytes(int n, int real_byt
 // the H100's 227 KB of shared memory per SM.
 constexpr size_t kStepStageMaxBytes = 6 * 1024;
 
+// Writer-warp staging (ww_kernel's WRITER instantiations, DESIGN §4.1): a block of kWrEnvs env warps, which
+// step adjacent envs, and one writer warp.  Every env-step's rows go into the env warp's part of a ring
+// slot of the block's shared memory; the writer warp copies each full slot, one step of kWrEnvs adjacent envs
+// and so one contiguous run of the [T][E][Np][D] tensor, to HBM.  The env warps then never wait on a store or
+// issue one; they only fence their rows into the async proxy before handing a slot over.  The defaults are the
+// fastest of scripts/ww_write_path.py's sweep (DESIGN §4.3); the macros exist for that sweep.
+#ifndef MADRL_WW_WRITER_SLOTS
+#define MADRL_WW_WRITER_SLOTS 2        // S: steps of the group in flight between the env warps and the writer
+#endif
+#ifndef MADRL_WW_WRITER_ENVS
+#define MADRL_WW_WRITER_ENVS 8         // env warps (= adjacent envs) per block
+#endif
+#ifndef MADRL_WW_WRITER_WARPS_PER_SM
+#define MADRL_WW_WRITER_WARPS_PER_SM 16   // resident env warps per SM
+#endif
+#ifndef MADRL_WW_WRITER_BULK
+#define MADRL_WW_WRITER_BULK 1         // 0: the writer copies a slot with 16-byte stores instead of one cp.async.bulk
+#endif
+constexpr int kWrSlots = MADRL_WW_WRITER_SLOTS, kWrEnvs = MADRL_WW_WRITER_ENVS;
+constexpr int kWrBlocksPerSm = MADRL_WW_WRITER_WARPS_PER_SM / MADRL_WW_WRITER_ENVS;
+constexpr bool kWrBulk = MADRL_WW_WRITER_BULK != 0;
+// A group's rows start 16-byte aligned in every step whenever the tensor's base and step stride are.
+static_assert(kWrEnvs % 4 == 0 && kWrSlots >= 2 && kWrBlocksPerSm >= 1, "writer-warp geometry");
+constexpr int kWrThreads = 32 * (kWrEnvs + 1);
+// Shared memory of a writer block: the full / empty mbarriers of the S slots, each env warp's candidate slots,
+// then the ring (slots of `slot` bytes).
+__host__ __device__ __forceinline__ uint32_t wr_slot_bytes(int env_step_bytes) {
+  return ((uint32_t)(kWrEnvs * env_step_bytes) + 15u) & ~15u;
+}
+constexpr uint32_t kWrBarBytes = (2 * 8 * kWrSlots + 15) & ~15;
+// An env warp's view of the ring: the mbarriers (full s at bar + 8 s, empty s at bar + 8 (S + s)), the ring, the
+// slot size, this warp's rows within a slot, and the slot s and phase parity of the current step.
+struct WrRing {
+  uint32_t bar, ring, slot, rows, phase;
+  int s;
+  __device__ __forceinline__ uint32_t empty() const { return bar + 8u * (uint32_t)(kWrSlots + s); }
+  __device__ __forceinline__ uint32_t step_rows() const { return ring + (uint32_t)s * slot + rows; }
+};
+struct NoWrRing {};
+
 // Shared address of element 0 of `row` (a row of the env-step starting at `obs_t`), after waiting for
 // the bulk store that last read that memory: the previous step's (whole-step staging, first row of
 // the step) or the one two rows ago (ring slot `slot_off`).
@@ -164,6 +206,59 @@ __device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int 
   }
 }
 
+// WRITER: shared address of element 0 of `row` in this env warp's part of the step's ring slot (`rows`), after
+// waiting, at the step's first row, until the writer warp has released the slot (`empty`, completed phase
+// parity `phase ^ 1`: the copy of what the slot held S steps ago; the first S steps find the slot free).
+template <typename O>
+__device__ __forceinline__ uint32_t wr_row_stage(uint32_t empty, uint32_t phase, uint32_t rows, const O* obs_t, const O* row) {
+  if (row == obs_t) mbar_wait(empty, phase ^ 1u);
+  return rows + (uint32_t)((row - obs_t) * sizeof(O));
+}
+
+// The writer warp of a WRITER block: for every step of every env group of the block, wait until the group's
+// env warps have staged the step in ring slot s ("full" mbarrier s), copy the slot to the group's contiguous run
+// of the observation tensor (16-aligned: the host only selects WRITER when the base and step stride are), and
+// release the slot ("empty" mbarrier s).  The copy is one cp.async.bulk (evict-first), and a slot is released
+// once the next one's bulk store is issued and the slot's own has read its source.  Without kWrBulk it is
+// 16-byte shared loads and evict-first global stores instead: the generic proxy, so the env warps need no
+// proxy fence, but the writer issues two instructions per 16 bytes.  The <= 3 elements after the last
+// 16-byte boundary of a partial last group are stored one per lane.
+template <typename real, typename O>
+__device__ __forceinline__ void ww_obs_writer(const WWParams<real, O>& p, uint32_t bar, uint32_t ring, uint32_t slot_bytes,
+                                              uint32_t env_bytes, int lane) {
+  static_assert(sizeof(O) == sizeof(float), "the writer warp stores float32 observations");
+  int s = 0;
+  [[maybe_unused]] int prev = -1;   // kWrBulk: the slot whose bulk store was issued last
+  uint32_t phase = 0u;
+  const size_t step_bytes = p.obs_step * sizeof(O);
+  for (int g0 = (int)blockIdx.x * kWrEnvs; g0 < p.E; g0 += (int)gridDim.x * kWrEnvs) {
+    const uint32_t n = (uint32_t)min(kWrEnvs, p.E - g0) * env_bytes, n16 = n & ~15u;
+    char* dst = reinterpret_cast<char*>(p.obs + (size_t)g0 * p.Np * p.D);
+    for (int t = 0; t < p.T; ++t, dst += step_bytes) {
+      const uint32_t src = ring + (uint32_t)s * slot_bytes;
+      mbar_wait(bar + 8u * s, phase);
+      if constexpr (kWrBulk) {
+        if (lane == 0) ring_bulk_store(dst, src, n16);
+      } else {
+#pragma unroll 4
+        for (uint32_t i = 16u * (uint32_t)lane; i < n16; i += 512u) stcs_f32x4(dst + i, ring_lds_f32x4(src + i));
+      }
+      const uint32_t tail = n16 + (uint32_t)lane * (uint32_t)sizeof(O);
+      if (tail < n) store_stream(reinterpret_cast<float*>(dst + tail), ring_lds_f32(src + tail));
+      __syncwarp();   // every lane has read the slot before it is released
+      if constexpr (kWrBulk) {
+        if (lane == 0 && prev >= 0) { bulk_wait_read_all_but_1(); mbar_arrive(bar + 8u * (kWrSlots + prev), 1u); }
+        prev = s;
+      } else {
+        if (lane == 0) mbar_arrive(bar + 8u * (kWrSlots + s), 1u);
+      }
+      if (++s == kWrSlots) { s = 0; phase ^= 1u; }
+    }
+  }
+  if constexpr (kWrBulk)
+    if (lane == 0) bulk_wait_all();   // the last bulk store has read its source before the block exits
+}
+
 // OPL = objects per lane (ceil(n_obj / 32)); KCH = sensors per lane (ceil(K / 32));
 // KC = compile-time sensor count (0 = runtime p.K): with KC known the 7 feature-row stores of a
 // pursuer use immediate offsets from one shared address.
@@ -172,17 +267,22 @@ __device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int 
 // POLICY = the actions come from the in-kernel heuristic policy instead of the action tensor (again a
 // separate instantiation: the open-loop kernel carries none of its instructions).
 // KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
-template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false, bool KEEP = false>
-__global__ void __launch_bounds__(32, (OPL <= 4 ? 28 : 16))
+// WRITER = writer-warp staging (kWrEnvs env warps + 1 writer warp per block; whole-step staging, 16-byte-aligned
+// observation base and step stride, open loop, no PEER / POLICY / KEEP).
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false, bool KEEP = false,
+          bool WRITER = false>
+__global__ void __launch_bounds__(WRITER ? kWrThreads : 32, WRITER ? kWrBlocksPerSm : (OPL <= 4 ? 28 : 16))
 ww_kernel(const __grid_constant__ WWParams<real, O> p) {
   const real INF = real_inf<real>();
   const int K = KC > 0 ? KC : p.K;
   // 32-thread blocks: the env index derives from blockIdx alone, so ptxas can prove every loop and
   // branch on it warp-uniform -- no BRA.DIV guards in front of the warp collectives, loop bookkeeping
   // on the uniform datapath, fewer registers.
-  const int lane = threadIdx.x;
-  const int warp_global = blockIdx.x;
-  const int warp_stride = gridDim.x;
+  const int lane = WRITER ? (int)(threadIdx.x & 31u) : (int)threadIdx.x;
+  // WRITER: env warp 0 .. kWrEnvs-1, or the writer; broadcast from lane 0 so that ptxas knows it is warp-uniform
+  const int wr_warp = WRITER ? __shfl_sync(FULL_MASK, (int)(threadIdx.x >> 5), 0) : 0;
+  const int warp_global = WRITER ? (int)blockIdx.x * kWrEnvs + wr_warp : (int)blockIdx.x;
+  const int warp_stride = WRITER ? (int)gridDim.x * kWrEnvs : (int)gridDim.x;
   const int eLo = p.Np, eHi = p.Np + p.Ne, Nall = p.Nall;
   constexpr bool SMEM = OPL >= 2;
   const unsigned lt_mask = lanemask_lt();
@@ -190,6 +290,26 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
   // this warp's candidate slots (OPL >= 2), then its observation staging (32-bit shared address)
   uint32_t slots = smem_addr(ww_smem);
   asm volatile("" : "+r"(slots));   // keep it in a register: ptxas otherwise re-derives it from SR_CgaCtaId at every use
+  // WRITER: the ring (an empty type otherwise, so that the other instantiations compile as they did without it)
+  typename std::conditional<WRITER, WrRing, NoWrRing>::type wr;
+  if constexpr (WRITER) {
+    const uint32_t env_bytes = (uint32_t)(p.Np * p.D) * (uint32_t)sizeof(O);
+    const uint32_t cand = SMEM ? (uint32_t)Nall * CandSlot<real>::kStride : 0u;
+    wr.bar = slots;
+    wr.slot = wr_slot_bytes((int)env_bytes);
+    wr.ring = wr.bar + kWrBarBytes + kWrEnvs * cand;
+    wr.rows = (uint32_t)wr_warp * env_bytes;
+    wr.s = 0;
+    wr.phase = 0u;
+    if (threadIdx.x == 0)
+      for (int s = 0; s < kWrSlots; ++s) { mbar_init(wr.bar + 8u * s, kWrEnvs); mbar_init(wr.bar + 8u * (kWrSlots + s), 1u); }
+    __syncthreads();
+    if (wr_warp == kWrEnvs) {
+      ww_obs_writer(p, wr.bar, wr.ring, wr.slot, env_bytes, lane);
+      return;
+    }
+    slots = wr.bar + kWrBarBytes + (uint32_t)wr_warp * cand;
+  }
 
   // ---- per-lane constants: this lane as OBJECT (classes, thresholds) and as SENSOR -----------
   real cull2_l[OPL], coll2_l[OPL];
@@ -420,7 +540,9 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             MADRL_WW_SCAN(endU, endE, bE, aE)
             MADRL_WW_SCAN(endE, endP, bP, aP)
 #undef MADRL_WW_SCAN
-            const uint32_t srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
+            uint32_t srow;
+            if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), obs_t, obs_row);
+            else srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
             for (int kc = 0; kc < KCH; ++kc) {
               const real sx = sx_l[kc], sy = sy_l[kc];
@@ -490,7 +612,9 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
 #undef MADRL_WW_SCAN
             }
           }
-          const uint32_t srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
+          uint32_t srow;
+          if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), obs_t, obs_row);
+          else srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
           for (int kc = 0; kc < KCH; ++kc) {
             const real sx = sx_l[kc], sy = sy_l[kc];
@@ -542,7 +666,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             }
           }
           }
-          if (!p.stage_step) {
+          if (!WRITER && !p.stage_step) {
             obs_row_store<KEEP>(stage + slot_off, obs_row, n_feat * K, lane);
             slot_off = slot_bytes - slot_off;
           }
@@ -585,8 +709,10 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
         if (lane < p.Np) {
           const real vE = (real)((whoEnc >> lane) & 1u), vP = (real)((whoP >> lane) & 1u), id = (real)(lane + 1);
           const int i = lane * p.D + n_feat * K;
-          if (p.stage_step) {
-            const uint32_t a = stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)(i * sizeof(O));
+          if (WRITER || p.stage_step) {
+            uint32_t a;
+            if constexpr (WRITER) a = wr.step_rows() + (uint32_t)(i * sizeof(O));
+            else a = stage + ((uint32_t)(uintptr_t)obs_t & 15u) + (uint32_t)(i * sizeof(O));
             stage_obs<O>(a, vE);
             stage_obs<O>(a + (uint32_t)sizeof(O), vP);
             if (p.addid) stage_obs<O>(a + 2 * (uint32_t)sizeof(O), id);
@@ -596,7 +722,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             if (p.addid) store_obs<KEEP>(obs_t + i + 2, obs_cvt<O>(id));
           }
         }
-        if (p.stage_step) obs_row_store<KEEP>(stage, obs_t, p.Np * p.D, lane);
+        if (!WRITER && p.stage_step) obs_row_store<KEEP>(stage, obs_t, p.Np * p.D, lane);
         if (!pass && lane < p.Np) {
           real r = pen;
           if (p.reward_global) {
@@ -655,14 +781,24 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
           // reset observation (rllab/sandbox/rocky/tf/envs/vec_env_executor.py:24-27)
           need_reset = done && p.auto_reset;
           if (need_reset) {   // the rows' bulk stores must land before they are read back or rewritten by the reset pass
-            if (lane == 0) bulk_wait_all();
+            if (!WRITER && lane == 0) bulk_wait_all();
             __syncwarp();
           }
-          if (need_reset && p.term_obs != nullptr)
-            keep_terminal_rows(obs_t, p.term_obs + (obs_t - p.obs), p.Np * p.D, lane);
+          if (need_reset && p.term_obs != nullptr) {
+            // WRITER: the terminal rows are still in the slot, which the reset pass overwrites before the writer
+            // warp sees it, so HBM gets the reset rows once
+            if constexpr (WRITER) keep_terminal_rows_staged<O>(wr.step_rows(), p.term_obs + (obs_t - p.obs), p.Np * p.D, lane);
+            else keep_terminal_rows(obs_t, p.term_obs + (obs_t - p.obs), p.Np * p.D, lane);
+          }
         }
         pass = need_reset ? 1 : 0;
       } while (need_reset);
+      if constexpr (WRITER) {   // hand the slot to the writer warp; the last env of a partial group also arrives for the absent ones
+        if constexpr (kWrBulk) fence_async_shared();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(wr.bar + 8u * wr.s, e + 1 == p.E ? (uint32_t)(kWrEnvs - wr_warp) : 1u);
+        if (++wr.s == kWrSlots) { wr.s = 0; wr.phase ^= 1u; }
+      }
       obs_t += p.obs_step;
       act_t += p.agent_step;
       rew_t += p.agent_step;
@@ -683,7 +819,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
       p.timestep[e] = tt; p.path_len[e] = ts; p.ctr[e] = ctr;
     }
   }
-  if (lane == 0) bulk_wait_all();   // the last bulk store has read its source before the block exits
+  if (!WRITER && lane == 0) bulk_wait_all();   // the last bulk store has read its source before the block exits
 }
 
 }  // namespace madrl
@@ -701,6 +837,7 @@ struct madrl_ww : EngineCore {
   void* peer_rew[8];
   void* peer_done[8];
   void* peer_info[8];
+  int obs_writer = MADRL_WW_OBS_WRITER_AUTO;   // set_obs_writer
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Np = cfg.n_pursuers, rb = lay.real_bytes;
@@ -786,11 +923,20 @@ extern "C" int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
+extern "C" int madrl_ww_set_obs_writer(madrl_ww* h, int mode) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(mode == MADRL_WW_OBS_WRITER_AUTO || mode == MADRL_WW_OBS_WRITER_OFF || mode == MADRL_WW_OBS_WRITER_ON,
+                "unknown observation writer mode %d", mode);
+  h->obs_writer = mode;
+  return MADRL_OK;
+}
+
 template <typename real>
 static size_t ww_cand_bytes(int opl, int n_obj) { return opl >= 2 ? (size_t)n_obj * CandSlot<real>::kStride : 0; }
 
-// The library's default cap on resident one-warp blocks per SM for an open-loop rollout of T steps with
-// float32 observations (0 = as many as fit; set_launch overrides it).  See DESIGN §4.3 for the numbers
+// The library's default cap on resident env warps per SM for an open-loop rollout of T steps with float32
+// observations (0 = as many as fit; set_launch overrides it).  Where it caps, the writer-warp kernel runs if it
+// can (ww_use_writer), with that many env warps per SM; else one-warp blocks.  See DESIGN §4.3 for the numbers
 // behind each condition, measured on C2 (5 pursuers, 4096 envs: 2.17 -> 2.02 ms per 256-step launch):
 //   * whole-step staging only: the C2 kernel computes about as fast with 16 warps per SM, each stepping two
 //     envs in turn, as with 31, but its observation stores overlap the sensing better.  The ring staging of
@@ -822,6 +968,36 @@ static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, int cap, cud
   return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY, KEEP>, smem, p.E, stream, p, cap);
 }
 
+// Whether a plain open-loop float32 rollout (no policy, peers or KEEP) of at most 32 objects runs on the writer-warp
+// kernel.  It needs whole-step staging, and a 16-byte-aligned observation base and step stride, so that every group's rows start on a
+// 16-byte boundary; otherwise, or with set_obs_writer(OFF), the one-warp kernel runs.  By default (AUTO) it replaces
+// the launches ww_default_blocks_per_sm caps, unless set_launch chose a geometry; ON takes it wherever it can run.
+static bool ww_use_writer(const madrl_ww* h, const WWParams<float, float>& p) {
+  if (h->obs_writer == MADRL_WW_OBS_WRITER_OFF || p.mode != 0 || !p.stage_step) return false;
+  if (((uintptr_t)p.obs | (uintptr_t)(p.obs_step * sizeof(float))) & 15u) return false;
+  return h->obs_writer == MADRL_WW_OBS_WRITER_ON || (h->blocks_per_sm == 0 && ww_default_blocks_per_sm(h, p.T) > 0);
+}
+
+// The writer-warp kernel: kWrThreads-thread blocks, kWrBlocksPerSm of them per SM (fewer if they do not fit), each
+// looping over groups of kWrEnvs adjacent envs.
+template <int OPL, int KCH, int KC>
+static int ww_launch_writer(madrl_ww* h, const WWParams<float, float>& p, cudaStream_t stream) {
+  auto kfn = ww_kernel<float, float, OPL, KCH, KC, false, false, false, true>;
+  const size_t smem = kWrBarBytes + kWrEnvs * ww_cand_bytes<float>(OPL, p.Nall) +
+                      kWrSlots * (size_t)wr_slot_bytes(p.Np * p.D * (int)sizeof(float));
+  MADRL_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int resident = 0;
+  MADRL_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&resident, kfn, kWrThreads, smem));
+  MADRL_REQUIRE(resident >= 1, "the writer-warp kernel does not fit an SM (%zu bytes of shared memory)", smem);
+  const int per_sm = resident < kWrBlocksPerSm ? resident : kWrBlocksPerSm;
+  const int groups = (p.E + kWrEnvs - 1) / kWrEnvs;
+  const int grid = groups < h->sms * per_sm ? groups : h->sms * per_sm;
+  MADRL_LAUNCH(kfn, grid, kWrThreads, smem, stream, p);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
 // The fused peer exchange is instantiated for native observations only (bf16 rollouts with peers are
 // rejected in ww_launch): it adds nothing to the observation path.
 template <typename real, typename O, int OPL, int KCH, int KC>
@@ -834,6 +1010,9 @@ static int ww_launch_inst(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t 
   if constexpr (sizeof(real) == 4)   // set_obs_cache refuses KEEP on fp64 handles
     if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
       return ww_launch_inst2<real, O, OPL, KCH, KC, false, false, true>(h, p, cap, stream);
+  // (with more than 32 objects, the writer instantiations spill registers at 2 blocks of 288 threads per SM)
+  if constexpr (sizeof(real) == 4 && sizeof(O) == 4 && OPL == 1)
+    if (ww_use_writer(h, p)) return ww_launch_writer<OPL, KCH, KC>(h, p, stream);
   return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, cap, stream);
 }
 

@@ -125,6 +125,12 @@ class BatchedMAWaterWorld(BatchedEngine):
         _lib.check(self._L.madrl_ww_set_peers(self._h, 0, 0, 0, None, None, None))
         self._launch_settings_changed()
 
+    def set_obs_writer(self, mode):
+        """Observation write path of float32 open-loop rollouts (madrl_ww_set_obs_writer): _lib.WW_OBS_WRITER_AUTO
+        (the default), _OFF or _ON.  The values written are the same either way."""
+        _lib.check(self._L.madrl_ww_set_obs_writer(self._h, int(mode)))
+        self._launch_settings_changed()
+
     def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, actions_out=None):
         """T lockstep steps in one launch with the reference's hand-written policy
         (heuristics/waterworld.py:11-53) evaluated inside the kernel: closed loop, no action tensor,

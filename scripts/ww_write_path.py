@@ -1,6 +1,7 @@
 """Waterworld observation write path against the card's streaming-write rate (one GPU command).
 
     python scripts/ww_write_path.py [--lib NAME=PATH ...] [--rounds R] [--blocks-per-sm N ...]
+                                    [--obs-writer MODE ...] [--envs E1,E2,...]
 
 Prints the card (name, power limit, SM clock), then times with CUDA events
   * `fill_` of a float32 tensor the size of one headline launch's observations ([256, 4096, 5, 213]):
@@ -12,7 +13,12 @@ through MADRL_B200_LIB, e.g. one made by scripts/build_variant.py from another c
 child process of its own, the builds alternating for R rounds, and the median and min-max spread over
 the rounds are printed per build.  Each `--blocks-per-sm N` times every build once more with the
 persistent wave capped at N one-warp blocks per SM (engine.set_launch): at N = 16 each warp steps about
-two envs in turn, which shows how much of a warp's time the other resident warps can absorb.
+two envs in turn, which shows how much of a warp's time the other resident warps can absorb.  Each
+`--obs-writer on|off` times every build once more with that Waterworld observation write path
+(set_obs_writer; builds without the entry point are timed as they are).  `--envs` times C2 at these batch sizes
+instead of 4096 only (the sizes scripts/ww_launch_cap.py uses: 2200,2640,3000,4096,6000,8192).  The writer-warp
+kernel's geometry is compiled in (MADRL_WW_WRITER_* in csrc/waterworld.cu): its sweep is a list of `--lib` builds
+made with scripts/build_variant.py NAME -DMADRL_WW_WRITER_SLOTS=3 ...
 """
 import argparse
 import json
@@ -23,6 +29,16 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SHAPES = {"c2": dict(cfg=dict(n_pursuers=5, n_evaders=5, n_poison=10, n_sensors=30), E=4096, T=256),
           "c4": dict(cfg=dict(n_pursuers=20, n_evaders=50, n_poison=50, n_sensors=30), E=4096, T=64)}
+WRITER_MODES = {"auto": 0, "off": 1, "on": 2}   # MADRL_WW_OBS_WRITER_*
+
+
+def shapes(envs):
+    """The timed shapes: C2 at each batch size of `envs` (named c2 at 4096, c2@E otherwise), then C4."""
+    out = {}
+    for E in envs:
+        out["c2" if E == 4096 else "c2@%d" % E] = dict(SHAPES["c2"], E=E)
+    out["c4"] = SHAPES["c4"]
+    return out
 
 
 def card():
@@ -61,14 +77,15 @@ def fill_rate(reps):
     return {"bytes": nbytes, "ms": ms, "gbs": nbytes / (ms * 1e-3) / 1e9}
 
 
-def rollout_rate(name, reps, bps):
+def rollout_rate(s, reps, bps, writer):
     import torch
     sys.path.insert(0, ROOT)
-    from madrl_b200 import BatchedMAWaterWorld
-    s = SHAPES[name]
+    from madrl_b200 import BatchedMAWaterWorld, _lib
     E, T, Np = s["E"], s["T"], s["cfg"]["n_pursuers"]
     eng = BatchedMAWaterWorld(E, device="cuda", seed=0, **s["cfg"])
     eng.set_launch(blocks_per_sm=bps)
+    if writer != "auto" and hasattr(_lib.lib(), "madrl_ww_set_obs_writer"):
+        eng.set_obs_writer(WRITER_MODES[writer])
     eng.reset()
     g = torch.Generator(device="cuda")
     g.manual_seed(1234)
@@ -81,8 +98,8 @@ def rollout_rate(name, reps, bps):
             "agent_steps_per_sec": E * Np * T / (ms * 1e-3)}
 
 
-def child(reps, bps):
-    print(json.dumps({n: rollout_rate(n, reps, bps) for n in SHAPES}), flush=True)
+def child(reps, bps, writer, envs):
+    print(json.dumps({n: rollout_rate(s, reps, bps, writer) for n, s in shapes(envs).items()}), flush=True)
 
 
 def main():
@@ -93,42 +110,50 @@ def main():
     ap.add_argument("--reps", type=int, default=10, help="timed launches per shape and round")
     ap.add_argument("--blocks-per-sm", type=int, action="append", default=[], metavar="N",
                     help="also time with at most N resident blocks per SM (0 = the library default)")
+    ap.add_argument("--obs-writer", action="append", default=[], choices=["on", "off"],
+                    help="also time with this Waterworld observation write path (set_obs_writer)")
+    ap.add_argument("--envs", default="4096", help="C2 batch sizes")
     ap.add_argument("--child", action="store_true", help=argparse.SUPPRESS)
     ap.add_argument("--bps", type=int, default=0, help=argparse.SUPPRESS)
+    ap.add_argument("--writer", default="auto", help=argparse.SUPPRESS)
     a = ap.parse_args()
+    envs = [int(x) for x in a.envs.split(",")]
     if a.child:
-        return child(a.reps, a.bps)
+        return child(a.reps, a.bps, a.writer, envs)
     import torch
     if not torch.cuda.is_available():
         raise SystemExit("ww_write_path.py needs a CUDA device")
     libs = [tuple(s.split("=", 1)) for s in a.lib] or [("default", os.environ.get("MADRL_B200_LIB", ""))]
-    # one timed build per (library, blocks per SM); bps 0 = the default launch, named by the library alone
-    libs = [(n if b == 0 else "%s@%d" % (n, b), path, b) for b in [0] + a.blocks_per_sm for n, path in libs]
+    # one timed build per (library, blocks per SM, write path); bps 0 and "auto" = the default launch, named by the
+    # library alone
+    libs = [(n + ("" if b == 0 else "@%d" % b) + ("" if w == "auto" else "/" + w), path, b, w)
+            for w in ["auto"] + a.obs_writer for b in [0] + a.blocks_per_sm for n, path in libs]
+    timed = shapes(envs)
     print("card:", json.dumps(card()))
     fill = fill_rate(20)
     print("fill_ float32 %.2f GB: %.3f ms, %.1f GB/s (streaming-write rate)" % (fill["bytes"] / 1e9, fill["ms"], fill["gbs"]))
-    res = {n: {s: [] for s in SHAPES} for n, _, _ in libs}
+    res = {n: {s: [] for s in timed} for n, _, _, _ in libs}
     for r in range(a.rounds):
-        for n, path, bps in libs:
+        for n, path, bps, w in libs:
             env = dict(os.environ)
             env.pop("MADRL_B200_LIB", None)
             if path:
                 env["MADRL_B200_LIB"] = os.path.abspath(path)
             p = subprocess.run([sys.executable, os.path.abspath(__file__), "--child", "--reps", str(a.reps),
-                                "--bps", str(bps)],
+                                "--bps", str(bps), "--writer", w, "--envs", a.envs],
                                env=env, cwd=ROOT, capture_output=True, text=True)
             if p.returncode:
                 sys.stderr.write(p.stdout + p.stderr)
                 raise SystemExit("round %d, build %s failed" % (r, n))
             rec = json.loads(p.stdout.strip().splitlines()[-1])
-            for s in SHAPES:
+            for s in timed:
                 res[n][s].append(rec[s])
                 print("round %d %-11s %s: %.3f ms/launch, obs %.1f GB/s (%.1f%% of fill), %.3g agent-steps/s"
                       % (r, n, s, rec[s]["ms"], rec[s]["obs_gbs"], 100 * rec[s]["obs_gbs"] / fill["gbs"],
                          rec[s]["agent_steps_per_sec"]), flush=True)
     print("summary (median over %d rounds; spread = (max - min) / median of the launch time):" % a.rounds)
-    for n, _, _ in libs:
-        for s in SHAPES:
+    for n, _, _, _ in libs:
+        for s in timed:
             ms = sorted(x["ms"] for x in res[n][s])
             med = ms[len(ms) // 2]
             gbs = res[n][s][0]["obs_bytes"] / (med * 1e-3) / 1e9
