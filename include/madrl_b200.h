@@ -630,6 +630,43 @@ int madrl_lfbr_predict_agents_bf16(int T, int E, int A, int D, const void* obs_d
     const int32_t* seg_start_dev, const int32_t* t0_dev, const double* norm_dev, const double* coef_dev,
     float* values_dev, void* stream);
 
+/* rllab's DDPG replay pool (rllab/rllab/algos/ddpg.py:85-145 MAReplayPool), decentralized mode, in device memory
+ * (csrc/replay.cu).  The pool of M = max_pool_size slots: pool_obs / pool_next [M][D] (float32 or bfloat16 bits),
+ * pool_act float32 [M][Ad], pool_rew float32 [M], pool_term uint8 [M]; ctl int64 [4] = top, bottom, size and the
+ * sampler's draw counter, all read and written on the device only.
+ *   madrl_replay_add_*     inserts the transitions of one rollout as DDPG.train adds them (:285-353): (t, e, a) order;
+ *                          observation obs[t-1] (obs_before [E][A][D] at t = 0), action act[t] (float32 [T][E][A][Ad]),
+ *                          reward float32(double(rew[t]) * scale_reward), next observation term[t] where done[t]
+ *                          else obs[t], terminal done[t].  Paths continue from path_len0 / timestep0 (int32 [E], the
+ *                          engine's counters before the launch); a done step with path length >= max_path_length
+ *                          (> 0) and timestep < timestep_limit is a horizon cut, dropped unless include_horizon.
+ *                          When K kept transitions exceed M only the last M land; ctl moves as K add_sample calls.
+ *                          ws: madrl_replay_workspace_size(T, E) bytes, 16-byte aligned.  Three launches.
+ *   madrl_replay_sample_*  n x B draws with replacement, uniform over slots [0, size - 1) (the set random_batch's
+ *                          rejection loop accepts): slot of draw c = mulhi64(Philox4x32-10 words 1:0 of counter
+ *                          (c, 0, 0, 2) under key seed, max(size - 1, 1)), c = ctl[3] + row; ctl[3] += n * B.
+ *                          Writes idx int64 [n*B] and the rows of obs / next observations / actions / rewards /
+ *                          terminals.  Two launches. */
+int madrl_replay_workspace_size(int T, int E, size_t* bytes);
+int madrl_replay_add_f32(int T, int E, int A, int D, int Ad, size_t M, const float* obs_dev, const float* act_dev,
+    const float* rew_dev, const uint8_t* done_dev, const float* obs_before_dev, const float* term_dev,
+    const int32_t* path_len0_dev, const int32_t* timestep0_dev, int max_path_length, int timestep_limit,
+    int include_horizon, double scale_reward, float* pool_obs_dev, float* pool_next_dev, float* pool_act_dev,
+    float* pool_rew_dev, uint8_t* pool_term_dev, int64_t* ctl_dev, void* ws_dev, void* stream);
+int madrl_replay_add_bf16(int T, int E, int A, int D, int Ad, size_t M, const void* obs_dev, const float* act_dev,
+    const float* rew_dev, const uint8_t* done_dev, const void* obs_before_dev, const void* term_dev,
+    const int32_t* path_len0_dev, const int32_t* timestep0_dev, int max_path_length, int timestep_limit,
+    int include_horizon, double scale_reward, void* pool_obs_dev, void* pool_next_dev, float* pool_act_dev,
+    float* pool_rew_dev, uint8_t* pool_term_dev, int64_t* ctl_dev, void* ws_dev, void* stream);
+int madrl_replay_sample_f32(int n, int B, int D, int Ad, size_t M, uint64_t seed, const float* pool_obs_dev,
+    const float* pool_next_dev, const float* pool_act_dev, const float* pool_rew_dev, const uint8_t* pool_term_dev,
+    int64_t* ctl_dev, int64_t* idx_dev, float* obs_out_dev, float* next_out_dev, float* act_out_dev,
+    float* rew_out_dev, uint8_t* term_out_dev, void* stream);
+int madrl_replay_sample_bf16(int n, int B, int D, int Ad, size_t M, uint64_t seed, const void* pool_obs_dev,
+    const void* pool_next_dev, const float* pool_act_dev, const float* pool_rew_dev, const uint8_t* pool_term_dev,
+    int64_t* ctl_dev, int64_t* idx_dev, void* obs_out_dev, void* next_out_dev, float* act_out_dev,
+    float* rew_out_dev, uint8_t* term_out_dev, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

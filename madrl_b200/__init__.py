@@ -13,9 +13,11 @@ from .waterworld import BatchedMAWaterWorld, MAWaterWorld, Archea  # noqa: F401
 from .pursuit import BatchedPursuitEvade, PursuitEvade, DiscreteAgent  # noqa: F401
 from .hostage import BatchedHostageWorld, ContinuousHostageWorld, CircAgent  # noqa: F401
 from .closed_loop import PolicyRollout  # noqa: F401
+from .replay import ReplayPool  # noqa: F401
 
 __all__ = [
     "EngineError", "launch_count", "Agent", "AbstractMAEnv", "EzPickle", "Box", "Discrete",
     "BatchedMAWaterWorld", "MAWaterWorld", "Archea", "BatchedPursuitEvade", "PursuitEvade",
     "DiscreteAgent", "BatchedHostageWorld", "ContinuousHostageWorld", "CircAgent", "PolicyRollout",
+    "ReplayPool",
 ]

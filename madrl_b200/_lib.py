@@ -196,6 +196,12 @@ def _signatures():
         # rltools' linear feature baseline
         "madrl_lfbr_workspace_size": (i32, [i32, P(sz)]),
         "madrl_lfbr_agents_workspace_size": (i32, [i32, i32, P(sz)]),
+        # rllab's DDPG replay pool
+        "madrl_replay_workspace_size": (i32, [i32, i32, P(sz)]),
+        "madrl_replay_add_f32": (i32, [i32] * 5 + [sz] + [vp] * 8 + [i32] * 3 + [f64] + [vp] * 8),
+        "madrl_replay_add_bf16": (i32, [i32] * 5 + [sz] + [vp] * 8 + [i32] * 3 + [f64] + [vp] * 8),
+        "madrl_replay_sample_f32": (i32, [i32] * 4 + [sz, u64] + [vp] * 13),
+        "madrl_replay_sample_bf16": (i32, [i32] * 4 + [sz, u64] + [vp] * 13),
     })
     for ag in ("", "_agents"):
         for dt in ("f32", "bf16"):
