@@ -162,6 +162,13 @@ int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T);
 #define MADRL_WW_OBS_WRITER_OFF 1
 #define MADRL_WW_OBS_WRITER_ON 2
 int madrl_ww_set_obs_writer(madrl_ww* h, int mode);
+/* Norm of madrl_ww_rollout_heuristic's actions.  AGENT (the default): each pursuer's action is divided by its own
+ * norm, as the reference's Visualizer calls the policy (one agent per call).  ENV: all Np actions of an env are
+ * divided by one Frobenius norm, as rltools' decrollout calls it (heuristics/waterworld.py:47-51 on the env's
+ * Np x 2 batch; all zero when that norm is 0).  MADRL_EINVAL for an unknown value. */
+#define MADRL_HEURISTIC_NORM_AGENT 0
+#define MADRL_HEURISTIC_NORM_ENV 1
+int madrl_ww_set_heuristic_norm(madrl_ww* h, int norm);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
  * terminal one.  After this call every `*_rollout` (device pointers) with auto_reset first copies the rows
@@ -198,7 +205,8 @@ int madrl_ww_rollout(madrl_ww* h, int T, const void* actions_dev, void* obs_dev,
  * obs0_dev real [E][Np][obs_dim]: the observation the first action is computed from (the reset
  * observation, or the last observation of the previous rollout); actions_out_dev real [T][E][Np][2]
  * receives the actions taken (NULL = not recorded).  Needs speed_features (the 7K layout the policy
- * indexes).  Each agent row is normalised by its own norm (the reference is called per agent, B = 1).
+ * indexes).  Each agent row is normalised by its own norm (the reference is called per agent, B = 1), or, after
+ * madrl_ww_set_heuristic_norm(h, MADRL_HEURISTIC_NORM_ENV), all of an env's rows by one norm.
  * Other arguments as madrl_ww_rollout. */
 int madrl_ww_rollout_heuristic(madrl_ww* h, int T, const void* obs0_dev, void* actions_out_dev,
                                void* obs_dev, void* rew_dev, uint8_t* done_dev, int32_t* info_dev,
@@ -451,6 +459,25 @@ int madrl_obs_wrap_step_bf16(int E, int A, int D, int B, void* obs_dev, void* te
 int madrl_episode_stats_f32(int T, int E, int A, const float* rew_dev, const uint8_t* done_dev,
                             double discount, int max_traj_len, double* carry_dev, float* ep_reward_dev,
                             float* ep_disc_dev, int32_t* ep_len_dev, uint8_t* ep_end_dev, void* stream);
+/* Whole-episode records of an evaluation (rltools/rltools/util.py:141-231 evaluate_policy), over a rollout cut into
+ * launches of any length: rew real [T][E][A] (float32 or float64), done uint8 [T][E], info int32 [T][E][C]
+ * (0 <= C <= MADRL_EVAL_INFO_MAX; NULL with C = 0).  carry: MADRL_EVAL_CARRY_WORDS 8-byte words per (e, a), zeroed by
+ * the caller when the evaluation starts and kept between calls, so any cut gives the same bits.  The k-th episode
+ * env e completes (k < K) goes to record k * E + e; later ones are not recorded:
+ *   ret  float64 [K*E][A]  sum of the episode's rewards in time order;
+ *   qsum float64 [K*E][A]  sum over its steps t of the discounted reward-to-go q_t, accumulated forward as
+ *                          sum_s r_s * G_s with G_s = sum_{j<=s} discount^j (no fused multiply-adds);
+ *   len  int32 [K*E]       its length;
+ *   info_sum int64 [K*E][C] its info sums (rltools/rltools/trajutil.py:105-108).
+ * One thread per (e, a), no atomics, no host synchronisation. */
+#define MADRL_EVAL_CARRY_WORDS 8
+#define MADRL_EVAL_INFO_MAX 2
+int madrl_eval_episodes_f32(int T, int E, int A, int C, const float* rew_dev, const uint8_t* done_dev,
+                            const int32_t* info_dev, double discount, int K, void* carry_dev, double* ret_dev,
+                            double* qsum_dev, int32_t* len_dev, int64_t* info_sum_dev, void* stream);
+int madrl_eval_episodes_f64(int T, int E, int A, int C, const double* rew_dev, const uint8_t* done_dev,
+                            const int32_t* info_dev, double discount, int K, void* carry_dev, double* ret_dev,
+                            double* qsum_dev, int32_t* len_dev, int64_t* info_sum_dev, void* stream);
 
 /* Whole-batch moments, deterministic (fixed grid, fixed combination order), float64 accumulation,
  * NumPy's two-pass population variance.  Series s0 = a, s1 = b, s2 = b - a (b may be NULL):

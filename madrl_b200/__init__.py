@@ -14,10 +14,11 @@ from .pursuit import BatchedPursuitEvade, PursuitEvade, DiscreteAgent  # noqa: F
 from .hostage import BatchedHostageWorld, ContinuousHostageWorld, CircAgent  # noqa: F401
 from .closed_loop import PolicyRollout  # noqa: F401
 from .replay import ReplayPool  # noqa: F401
+from .evaluate import evaluate_heuristic, evaluate_policy  # noqa: F401
 
 __all__ = [
     "EngineError", "launch_count", "Agent", "AbstractMAEnv", "EzPickle", "Box", "Discrete",
     "BatchedMAWaterWorld", "MAWaterWorld", "Archea", "BatchedPursuitEvade", "PursuitEvade",
     "DiscreteAgent", "BatchedHostageWorld", "ContinuousHostageWorld", "CircAgent", "PolicyRollout",
-    "ReplayPool",
+    "ReplayPool", "evaluate_policy", "evaluate_heuristic",
 ]

@@ -23,6 +23,10 @@ OBS_NATIVE, OBS_BF16 = 0, 1
 OBS_CACHE_STREAM, OBS_CACHE_KEEP = 0, 1
 # Waterworld's observation write path (madrl_ww_set_obs_writer)
 WW_OBS_WRITER_AUTO, WW_OBS_WRITER_OFF, WW_OBS_WRITER_ON = 0, 1, 2
+# norm of Waterworld's in-kernel heuristic actions (madrl_ww_set_heuristic_norm)
+HEURISTIC_NORM_AGENT, HEURISTIC_NORM_ENV = 0, 1
+# evaluation records (madrl_eval_episodes_*): 8-byte carry words per (env, agent), most info columns
+EVAL_CARRY_WORDS, EVAL_INFO_MAX = 8, 2
 
 
 class WWConfig(C.Structure):
@@ -146,6 +150,7 @@ def _signatures():
     sig.update({
         "madrl_ww_default_blocks_per_sm": (i32, [vp, i32]),
         "madrl_ww_set_obs_writer": (i32, [vp, i32]),
+        "madrl_ww_set_heuristic_norm": (i32, [vp, i32]),
         "madrl_ww_set_peers": (i32, [vp, i32, i32, i32, P(vp), P(vp), P(vp)]),
         "madrl_ww_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
         "madrl_pursuit_set_params": (i32, [vp, f64, f64]),
@@ -164,6 +169,8 @@ def _signatures():
         "madrl_obs_wrap_step_f32": (i32, [i32] * 4 + [vp] * 7 + [f64, f64, vp]),
         "madrl_obs_wrap_step_bf16": (i32, [i32] * 4 + [vp] * 7 + [f64, f64, vp]),
         "madrl_episode_stats_f32": (i32, [i32, i32, i32, vp, vp, f64, i32, vp, vp, vp, vp, vp, vp]),
+        "madrl_eval_episodes_f32": (i32, [i32] * 4 + [vp] * 3 + [f64, i32] + [vp] * 6),
+        "madrl_eval_episodes_f64": (i32, [i32] * 4 + [vp] * 3 + [f64, i32] + [vp] * 6),
         # moments and advantage centring
         "madrl_moments_f32": (i32, [sz, vp, vp, vp, vp, vp]),
         "madrl_center_advantages_f32": (i32, [sz, vp, i32, i32, vp, vp, vp]),

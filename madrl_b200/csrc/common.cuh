@@ -73,6 +73,14 @@ __device__ __forceinline__ real warp_allreduce_sum(real v) {
   return v;
 }
 
+// The same for the maximum (of non-NaN values).
+template <typename real>
+__device__ __forceinline__ real warp_allreduce_max(real v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(FULL_MASK, v, o));
+  return v;
+}
+
 // The warp-per-env kernels are launched as 32-thread blocks (one env per block; see engine_launch in
 // engine.cuh).  The env index then derives from blockIdx alone, so ptxas can prove the persistent loop
 // and every branch on warp-uniform values uniform: the BRA.DIV guards in front of the warp collectives

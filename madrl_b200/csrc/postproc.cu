@@ -225,6 +225,69 @@ __global__ void episode_stats_kernel(int T, int E, int A, const float* __restric
   c[A] = len; c[A + 1] = disc; c[A + 2] = pw;
 }
 
+// Whole-episode records of an evaluation (rltools/rltools/util.py:141-231): one thread per (env, agent) column walks
+// the time axis.  carry [E][A][MADRL_EVAL_CARRY_WORDS] 8-byte words: ret, qsum, G, discount^len (doubles), len,
+// episodes completed, the C info sums (int64; only agent 0's column sums the env's info); zeroed = a fresh start.
+// G_s = sum_{j<=s} discount^j is carried forward, so sum_t q_t = sum_s r_s G_s needs no future reward.  Every
+// float64 operation is rounded on its own (__dadd_rn / __dmul_rn): a contraction into fma would change the bits
+// between builds and against the NumPy oracle.
+template <typename R>
+__global__ void eval_episodes_kernel(int T, int E, int A, int C, const R* __restrict__ rew,
+                                     const uint8_t* __restrict__ done, const int32_t* __restrict__ info,
+                                     double discount, int K, void* __restrict__ carry, double* __restrict__ ret_out,
+                                     double* __restrict__ qsum_out, int32_t* __restrict__ len_out,
+                                     int64_t* __restrict__ info_out) {
+  const size_t n = (size_t)E * A;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int e = (int)(i / A), a = (int)(i - (size_t)e * A);
+  double* cd = (double*)carry + i * MADRL_EVAL_CARRY_WORDS;
+  int64_t* ci = (int64_t*)carry + i * MADRL_EVAL_CARRY_WORDS;
+  double ret = cd[0], qsum = cd[1], G = cd[2];
+  int64_t len = ci[4], k = ci[5];
+  double pw = len == 0 ? 1.0 : cd[3];
+  int64_t isum[MADRL_EVAL_INFO_MAX];
+#pragma unroll
+  for (int j = 0; j < MADRL_EVAL_INFO_MAX; ++j) isum[j] = ci[6 + j];
+  for (int t = 0; t < T; ++t) {
+    const size_t te = (size_t)t * E + e;
+    const double r = (double)rew[te * A + a];
+    ret = __dadd_rn(ret, r);
+    G = __dadd_rn(G, pw);
+    qsum = __dadd_rn(qsum, __dmul_rn(r, G));
+    pw = __dmul_rn(pw, discount);
+    ++len;
+    if (a == 0) {
+#pragma unroll
+      for (int j = 0; j < MADRL_EVAL_INFO_MAX; ++j)
+        if (j < C) isum[j] += info[te * C + j];
+    }
+    if (done[te]) {
+      if (k < K) {
+        const size_t rec = (size_t)k * E + e;
+        ret_out[rec * A + a] = ret;
+        qsum_out[rec * A + a] = qsum;
+        if (a == 0) {
+          len_out[rec] = (int32_t)len;
+#pragma unroll
+          for (int j = 0; j < MADRL_EVAL_INFO_MAX; ++j)
+            if (j < C) info_out[rec * C + j] = isum[j];
+        }
+      }
+      ++k;
+      ret = qsum = G = 0.0;
+      pw = 1.0;
+      len = 0;
+#pragma unroll
+      for (int j = 0; j < MADRL_EVAL_INFO_MAX; ++j) isum[j] = 0;
+    }
+  }
+  cd[0] = ret; cd[1] = qsum; cd[2] = G; cd[3] = pw;
+  ci[4] = len; ci[5] = k;
+#pragma unroll
+  for (int j = 0; j < MADRL_EVAL_INFO_MAX; ++j) ci[6 + j] = isum[j];
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // Whole-batch moments for advantage centring (rllab/rllab/algos/util.py:7-12, applied at
@@ -623,6 +686,40 @@ extern "C" int madrl_episode_stats_f32(int T, int E, int A, const float* rew_dev
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;
+}
+
+template <typename R>
+static int eval_episodes(int T, int E, int A, int C, const R* rew_dev, const uint8_t* done_dev, const int32_t* info_dev,
+                         double discount, int K, void* carry_dev, double* ret_dev, double* qsum_dev, int32_t* len_dev,
+                         int64_t* info_sum_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && K >= 1, "bad sizes");
+  MADRL_REQUIRE(C >= 0 && C <= MADRL_EVAL_INFO_MAX, "info columns must be in [0, %d], got %d", MADRL_EVAL_INFO_MAX, C);
+  MADRL_REQUIRE((size_t)K * E * A < ((size_t)1 << 31), "K*E*A must be < 2^31");
+  MADRL_REQUIRE(discount >= 0.0 && discount <= 1.0, "discount must be in [0, 1], got %g", discount);
+  MADRL_REQUIRE(rew_dev && done_dev && carry_dev && ret_dev && qsum_dev && len_dev, "NULL buffer");
+  MADRL_REQUIRE(C == 0 || (info_dev && info_sum_dev), "NULL info buffer with %d info columns", C);
+  const size_t n = (size_t)E * A;
+  MADRL_LAUNCH(eval_episodes_kernel<R>, (unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream, T, E, A, C, rew_dev,
+               done_dev, info_dev, discount, K, carry_dev, ret_dev, qsum_dev, len_dev, info_sum_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_eval_episodes_f32(int T, int E, int A, int C, const float* rew_dev, const uint8_t* done_dev,
+                                       const int32_t* info_dev, double discount, int K, void* carry_dev,
+                                       double* ret_dev, double* qsum_dev, int32_t* len_dev, int64_t* info_sum_dev,
+                                       void* stream) {
+  return eval_episodes(T, E, A, C, rew_dev, done_dev, info_dev, discount, K, carry_dev, ret_dev, qsum_dev, len_dev,
+                       info_sum_dev, stream);
+}
+
+extern "C" int madrl_eval_episodes_f64(int T, int E, int A, int C, const double* rew_dev, const uint8_t* done_dev,
+                                       const int32_t* info_dev, double discount, int K, void* carry_dev,
+                                       double* ret_dev, double* qsum_dev, int32_t* len_dev, int64_t* info_sum_dev,
+                                       void* stream) {
+  return eval_episodes(T, E, A, C, rew_dev, done_dev, info_dev, discount, K, carry_dev, ret_dev, qsum_dev, len_dev,
+                       info_sum_dev, stream);
 }
 
 extern "C" int madrl_gae_f32(int T, int E, int A, const float* rew_dev, const float* value_dev,

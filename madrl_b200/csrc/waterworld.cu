@@ -265,11 +265,13 @@ __device__ __forceinline__ void ww_obs_writer(const WWParams<real, O>& p, uint32
 // PEER = compile the fused multi-GPU exchange in (a separate instantiation, so the single-GPU kernel
 // carries none of its registers).
 // POLICY = the actions come from the in-kernel heuristic policy instead of the action tensor (again a
-// separate instantiation: the open-loop kernel carries none of its instructions).
+// separate instantiation: the open-loop kernel carries none of its instructions): kWwPolicyAgent divides each
+// pursuer's action by its own norm, kWwPolicyEnv all of an env's actions by one norm (madrl_ww_set_heuristic_norm).
 // KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
 // WRITER = writer-warp staging (kWrEnvs env warps + 1 writer warp per block; whole-step staging, 16-byte-aligned
 // observation base and step stride, open loop, no PEER / POLICY / KEEP).
-template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY = false, bool KEEP = false,
+constexpr int kWwPolicyAgent = 1, kWwPolicyEnv = 2;
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY = 0, bool KEEP = false,
           bool WRITER = false>
 __global__ void __launch_bounds__(WRITER ? kWrThreads : 32, WRITER ? kWrBlocksPerSm : (OPL <= 4 ? 28 : 16))
 ww_kernel(const __grid_constant__ WWParams<real, O> p) {
@@ -407,7 +409,18 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
     for (int t = 0; t < p.T; ++t) {
       V2 act;
       act.x = 0; act.y = 0;
-      if constexpr (POLICY) {
+      if constexpr (POLICY == kWwPolicyEnv) {
+        // heuristics/waterworld.py:47-51 on the env's Np x 2 batch: every action divided by the batch's Frobenius
+        // norm, all zero when it is 0; scaled by the largest |component| first, as below
+        const real m = warp_allreduce_max(lane < p.Np ? fmax(fabs(pax), fabs(pay)) : (real)0);
+        const real ux = m > (real)0 ? pax / m : (real)0, uy = m > (real)0 ? pay / m : (real)0;
+        const real n = sqrt(warp_allreduce_sum(lane < p.Np ? ux * ux + uy * uy : (real)0));
+        if (lane < p.Np) {
+          if (m > (real)0) { act.x = ux / n; act.y = uy / n; }
+          if (p.actions_out != nullptr)
+            reinterpret_cast<V2*>(p.actions_out)[(size_t)t * p.agent_step + (size_t)e * p.Np + lane] = act;
+        }
+      } else if constexpr (POLICY) {
         if (lane < p.Np) {   // heuristics/waterworld.py:44-50: unit vector, or zero when nothing is sensed
           // scaled by the larger component first: the squares of a tiny sum (cancellation leaves ~1e-21) would be
           // denormal in float32 and the "unit" vector off by 1e-4
@@ -838,6 +851,7 @@ struct madrl_ww : EngineCore {
   void* peer_done[8];
   void* peer_info[8];
   int obs_writer = MADRL_WW_OBS_WRITER_AUTO;   // set_obs_writer
+  int heuristic_norm = MADRL_HEURISTIC_NORM_AGENT;   // set_heuristic_norm
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Np = cfg.n_pursuers, rb = lay.real_bytes;
@@ -931,6 +945,14 @@ extern "C" int madrl_ww_set_obs_writer(madrl_ww* h, int mode) {
   return MADRL_OK;
 }
 
+extern "C" int madrl_ww_set_heuristic_norm(madrl_ww* h, int norm) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(norm == MADRL_HEURISTIC_NORM_AGENT || norm == MADRL_HEURISTIC_NORM_ENV,
+                "unknown heuristic norm %d", norm);
+  h->heuristic_norm = norm;
+  return MADRL_OK;
+}
+
 template <typename real>
 static size_t ww_cand_bytes(int opl, int n_obj) { return opl >= 2 ? (size_t)n_obj * CandSlot<real>::kStride : 0; }
 
@@ -961,7 +983,7 @@ extern "C" int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T) {
   return ww_default_blocks_per_sm(h, T);
 }
 
-template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, bool POLICY, bool KEEP = false>
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY, bool KEEP = false>
 static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, int cap, cudaStream_t stream) {
   const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(O))
                                                                         : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(O)));
@@ -982,7 +1004,7 @@ static bool ww_use_writer(const madrl_ww* h, const WWParams<float, float>& p) {
 // looping over groups of kWrEnvs adjacent envs.
 template <int OPL, int KCH, int KC>
 static int ww_launch_writer(madrl_ww* h, const WWParams<float, float>& p, cudaStream_t stream) {
-  auto kfn = ww_kernel<float, float, OPL, KCH, KC, false, false, false, true>;
+  auto kfn = ww_kernel<float, float, OPL, KCH, KC, false, 0, false, true>;
   const size_t smem = kWrBarBytes + kWrEnvs * ww_cand_bytes<float>(OPL, p.Nall) +
                       kWrSlots * (size_t)wr_slot_bytes(p.Np * p.D * (int)sizeof(float));
   MADRL_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1002,18 +1024,21 @@ static int ww_launch_writer(madrl_ww* h, const WWParams<float, float>& p, cudaSt
 // rejected in ww_launch): it adds nothing to the observation path.
 template <typename real, typename O, int OPL, int KCH, int KC>
 static int ww_launch_inst(madrl_ww* h, const WWParams<real, O>& p, cudaStream_t stream) {
-  if (p.policy_obs0 != nullptr) return ww_launch_inst2<real, O, OPL, KCH, KC, false, true>(h, p, 0, stream);
+  if (p.policy_obs0 != nullptr)
+    return h->heuristic_norm == MADRL_HEURISTIC_NORM_ENV
+               ? ww_launch_inst2<real, O, OPL, KCH, KC, false, kWwPolicyEnv>(h, p, 0, stream)
+               : ww_launch_inst2<real, O, OPL, KCH, KC, false, kWwPolicyAgent>(h, p, 0, stream);
   if constexpr (sizeof(O) == sizeof(real))
-    if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, false>(h, p, 0, stream);
+    if (p.n_peers > 0) return ww_launch_inst2<real, O, OPL, KCH, KC, true, 0>(h, p, 0, stream);
   // only the plain open-loop rollout was measured with the default cap
   const int cap = p.mode == 0 ? ww_default_blocks_per_sm(h, p.T) : 0;
   if constexpr (sizeof(real) == 4)   // set_obs_cache refuses KEEP on fp64 handles
     if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
-      return ww_launch_inst2<real, O, OPL, KCH, KC, false, false, true>(h, p, cap, stream);
+      return ww_launch_inst2<real, O, OPL, KCH, KC, false, 0, true>(h, p, cap, stream);
   // (with more than 32 objects, the writer instantiations spill registers at 2 blocks of 288 threads per SM)
   if constexpr (sizeof(real) == 4 && sizeof(O) == 4 && OPL == 1)
     if (ww_use_writer(h, p)) return ww_launch_writer<OPL, KCH, KC>(h, p, stream);
-  return ww_launch_inst2<real, O, OPL, KCH, KC, false, false>(h, p, cap, stream);
+  return ww_launch_inst2<real, O, OPL, KCH, KC, false, 0>(h, p, cap, stream);
 }
 
 template <typename real, typename O>

@@ -131,12 +131,25 @@ class BatchedMAWaterWorld(BatchedEngine):
         _lib.check(self._L.madrl_ww_set_obs_writer(self._h, int(mode)))
         self._launch_settings_changed()
 
-    def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, actions_out=None):
+    _heuristic_norms = {"agent": _lib.HEURISTIC_NORM_AGENT, "env": _lib.HEURISTIC_NORM_ENV}
+    _heuristic_norm = _lib.HEURISTIC_NORM_AGENT
+
+    def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, actions_out=None,
+                          norm="agent"):
         """T lockstep steps in one launch with the reference's hand-written policy
         (heuristics/waterworld.py:11-53) evaluated inside the kernel: closed loop, no action tensor,
         no per-step launch.  obs0 [E, Np, D] = the observation the first action is computed from
-        (`reset()`'s, or `obs[-1]` of the previous rollout).  Returns
-        (actions [T,E,Np,2] or None, obs, rew, done, info)."""
+        (`reset()`'s, or `obs[-1]` of the previous rollout).  `norm`: "agent" divides each pursuer's action
+        by its own norm (the reference's Visualizer calls the policy per agent); "env" divides all of an env's
+        actions by one norm, as rltools' decrollout calls it with the env's Np observations as one batch
+        (madrl_ww_set_heuristic_norm).  Returns (actions [T,E,Np,2] or None, obs, rew, done, info)."""
+        if norm not in self._heuristic_norms:
+            raise ValueError("norm must be 'agent' or 'env', got %r" % (norm,))
+        code = self._heuristic_norms[norm]
+        if code != self._heuristic_norm:
+            _lib.check(self._L.madrl_ww_set_heuristic_norm(self._h, code))
+            self._heuristic_norm = code
+            self._launch_settings_changed()
         return self._rollout_heuristic(T, obs0, auto_reset, out, record_actions, actions_out)
 
 
