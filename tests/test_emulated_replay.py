@@ -3,7 +3,8 @@ by the warp emulator of tests/emu and compared, through the C ABI, with oracle/r
 rows in every word width the kernels pick (16, 8, 4 and 2 bytes), odd D, A = 1, T = 1, no done step, every step
 done, nothing kept, more kept transitions than the pool holds, a wrap in the middle of an add, and [T, E] off the
 block and warp sizes.  Every output sits in a canary-guarded buffer, and the pool starts filled with random bytes,
-so a slot an add must not touch and still does, or a write outside a buffer, fails."""
+so a slot an add must not touch and still does, or a write outside a buffer, fails.  The launch-geometry edges of
+tests/test_replay_edges_gpu.py (tests/replay_eval_edges.py) run here too, at the emulator's two SMs."""
 import ctypes as C
 import os
 import subprocess
@@ -15,6 +16,7 @@ from emu import build_emu, driver
 from emu.driver import Guarded
 from emu.driver import ptr as _p
 from oracle import replay_oracle as ro
+import replay_eval_edges as RE
 
 pytestmark = driver.needs_cxx
 
@@ -74,7 +76,7 @@ def rollout(rs, T, E, A, D, Ad, w, mpl, limit, p_done, pl0, ts0):
 class EmuPool(object):
     """The pool's buffers in guarded host memory, pre-filled like the oracle's with random bytes."""
 
-    def __init__(self, lib, M, D, Ad, w, include, rs):
+    def __init__(self, lib, M, D, Ad, w, include, rs, start=None):
         self.lib, self.M, self.D, self.Ad, self.w = lib, M, D, Ad, w
         self.sfx = "bf16" if w == np.uint16 else "f32"
         self.oracle = ro.ReplayOracle(M, D, Ad, obs_dtype=w, scale_reward=SCALE,
@@ -89,6 +91,10 @@ class EmuPool(object):
             getattr(self.oracle, name)[...] = g.arr
             self.bufs[name] = g
         self.ctl = Guarded((4,), np.int64, 0)
+        if start is not None:      # (top, bottom, size, draws) of a pool part-way through its life
+            o = self.oracle
+            o.top, o.bottom, o.size, o.draws = start
+            self.ctl.arr[...] = start
 
     def add(self, r, pl0, ts0, mpl, limit):
         T, E, A, D = r["obs"].shape
@@ -206,3 +212,68 @@ def test_argument_errors(lib):
         args = list(s)
         args[k] = bad
         assert lib.madrl_replay_sample_f32(*args, None) != 0, k
+
+
+# ------------------------------------------------------------------ the edge cases of tests/test_replay_edges_gpu.py
+# at the emulator's geometry: two SMs, so the insert grid G is 128 warps; the scan block is kScanThreads as on the
+# device, reached here with one warp of envs (T = cells)
+
+@pytest.mark.parametrize("which", range(4), ids=["G-1", "G", "G+1", "2G+1"])
+def test_insert_grid_edges(lib, which):
+    rows = RE.insert_grid_rows(2)[which]
+    T, E, A = RE.grid_shape(rows)
+    rs = np.random.RandomState(100 + which)
+    pl, ts = RE.start_counters(rs, E, 5)
+    r, _, _ = RE.rollout(rs, T, E, A, 3, 2, np.float32, 5, 10 ** 6, 0.05, pl, ts)
+    K = int(ro.keep_flags(r["done"], pl, ts, 5, 10 ** 6, False).sum()) * A
+    M = K + 37
+    pool = EmuPool(lib, M, 3, 2, np.float32, False, rs, start=(M - 20, 0, M - 20, 0))
+    assert pool.add(r, pl, ts, 5, 10 ** 6) == K > 0
+    if which != 2:
+        return
+    # G + 1 rows and K >> M: the grid-stride loop starts at a step past 0
+    M = max(K // 7, 1) + 1
+    assert RE.landing_step(r["done"], pl, ts, 5, 10 ** 6, False, A, K - M) > 0
+    EmuPool(lib, M, 3, 2, np.float32, False, rs).add(r, pl, ts, 5, 10 ** 6)
+
+
+@pytest.mark.parametrize("cut", RE.CUTS)
+@pytest.mark.parametrize("which", range(4), ids=["S-1", "S", "S+1", "2S+1"])
+def test_scan_cuts(lib, which, cut):
+    T, E, A, mpl = RE.scan_cells()[which], 20, 3, 6
+    rs = np.random.RandomState(1000 * which + RE.CUTS.index(cut))
+    pl, ts = RE.start_counters(rs, E, mpl)
+    r, _, _ = RE.rollout(rs, T, E, A, 2, 1, np.float32, mpl, 10 ** 6, 0.02, pl, ts)
+    M, first, K = RE.cut_pool_size(cut, r["done"], pl, ts, mpl, 10 ** 6, False, A)
+    top = int(rs.randint(0, M))
+    pool = EmuPool(lib, M, 2, 1, np.float32, False, rs, start=(top, top, M, 0) if first % 2 else (top, 0, top, 0))
+    assert pool.add(r, pl, ts, mpl, 10 ** 6) == K
+
+
+@pytest.mark.parametrize("E", RE.PLAN_ENVS)
+def test_plan_warps(lib, E):
+    T, A, mpl = 7, 2, 3
+    rs = np.random.RandomState(E)
+    z = np.zeros(E, np.int32)
+    pool = EmuPool(lib, 5 * T * E * A, 5, 2, np.float32, False, rs)
+    r, _, _ = RE.rollout(rs, T, E, A, 5, 2, np.float32, mpl, 10 ** 6, 0.0, z, z)
+    pool.add(r, z, z, mpl, 10 ** 6)
+    pl, ts = RE.start_counters(rs, E, mpl)
+    r, _, _ = RE.rollout(rs, T, E, A, 5, 2, np.float32, mpl, 10 ** 6, 0.1, pl, ts)
+    pool.add(r, pl, ts, mpl, 10 ** 6)
+    pool.sample(E, 1, 3 * E)
+
+
+@pytest.mark.parametrize("row", RE.WORD_ROWS, ids=["%s_D%d_%dB" % ("bf16" if w == np.uint16 else "f32", D, b)
+                                                   for w, D, b in RE.WORD_ROWS])
+def test_word_widths_and_sample_rows(lib, row):
+    w, D, _ = row
+    rs = np.random.RandomState(D)
+    pool = EmuPool(lib, 500, D, 33, w, True, rs)
+    pl, ts = RE.start_counters(rs, 45, 3)
+    for _ in range(2):
+        r, pl1, ts1 = RE.rollout(rs, 5, 45, 3, D, 33, w, 3, 9, 0.1, pl, ts)
+        pool.add(r, pl, ts, 3, 9)
+        pl, ts = pl1, ts1
+    for n, B in RE.SAMPLE_ROWS:
+        pool.sample(5 + B, n, B)

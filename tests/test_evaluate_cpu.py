@@ -13,6 +13,7 @@ import types
 import numpy as np
 import pytest
 
+import replay_eval_edges as RE
 from emu.driver import Guarded, needs_cxx, ptr
 from madrl_b200 import evaluate as ev
 from madrl_b200 import _lib
@@ -85,6 +86,35 @@ def test_emulated_eval_episodes_equal_the_oracle_for_every_cut(name):
         assert np.array_equal(carry, want_carry), (name, step)
         o_recs, o_carry = run_oracle(rew, done, info, disc, K, cuts)
         assert all(np.array_equal(a, b) for a, b in zip(o_recs, want)) and np.array_equal(o_carry, want_carry)
+
+
+@needs_cxx
+@pytest.mark.parametrize("C", [0, 1, 2])
+@pytest.mark.parametrize("run", range(len(RE.RECORD_RUNS)),
+                         ids=["T%d_K%d_g%s" % (r[0], r[1], r[2]) for r in RE.RECORD_RUNS])
+@pytest.mark.parametrize("shape", RE.RECORD_SHAPES[:3] + RE.RECORD_SHAPES[4:6] + RE.RECORD_SHAPES[7:9],
+                         ids=lambda s: "E%d_A%d" % s)
+def test_emulated_records_at_the_edge_cases(shape, run, C):
+    """The cases of tests/test_evaluate_edges_gpu.py (tests/replay_eval_edges.py): records filled with sentinels
+    first, carry and records bit for bit after every launch."""
+    from emu.driver import load
+    lib = load()
+    E, A = shape
+    T, K, disc, launch_len = RE.RECORD_RUNS[run]
+    f64 = (RE.RECORD_SHAPES.index(shape) + C + run) % 2 == 1
+    rew, done, info, cuts = RE.record_case(T, E, A, C, K, 17 * E + A + run, f64, launch_len)
+    carry = Guarded((E, A, _lib.EVAL_CARRY_WORDS), np.int64, 0)
+    recs = [Guarded(x.shape, x.dtype, 0) for x in RE.record_sentinels(E, A, C, K)]
+    for g, x in zip(recs, RE.record_sentinels(E, A, C, K)):
+        g.arr[...] = x
+    fn = lib.madrl_eval_episodes_f64 if f64 else lib.madrl_eval_episodes_f32
+    want = RE.record_sentinels(E, A, C, K)
+    for t0, t1, w_carry, w_recs in RE.run_records_oracle(rew, done, info, disc, K, cuts, want):
+        r, d, i = (np.ascontiguousarray(x[t0:t1]) for x in (rew, done, info))
+        assert fn(t1 - t0, E, A, C, ptr(r), ptr(d), ptr(i) if C else None, disc, K, ptr(carry.arr),
+                  *[ptr(x.arr) for x in recs[:3]], ptr(recs[3].arr) if C else None, None) == 0
+        assert np.array_equal(carry.check("carry"), w_carry), (t0, t1)
+        assert RE.records_equal([x.check("record") for x in recs], w_recs), (t0, t1)
 
 
 def episodes_of(rew, done, info, K):

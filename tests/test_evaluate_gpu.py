@@ -122,12 +122,8 @@ def test_kernel_matches_the_oracle_at_product_shapes(shape):
     eo.eval_episodes(r, d, i, disc, K, carry, want)
     assert np.array_equal(got[2], want[2]) and np.array_equal(got[3], want[3])
     assert (want[2] > 0).all(), "every env must complete K episodes"
-    # bounds of any summation order: sum |r| and sum |r| G over each record's steps
-    absr = eo.new_records(E, A, C, K)
-    eo.eval_episodes(np.abs(r), d, i, disc, K, eo.new_carry(E, A), absr)
-    assert np.all(np.abs(got[0] - want[0]) <= 1e-12 * absr[0])
-    assert np.all(np.abs(got[1] - want[1]) <= 1e-12 * absr[1])
-    print(shape, "records bit-identical:", np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1]))
+    # every float64 operation is rounded on its own, in the oracle's order: the records are its bits
+    assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
 
 
 class Linear(object):
