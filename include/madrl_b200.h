@@ -505,6 +505,17 @@ int madrl_moments_agents_f32(size_t rows, int A, const float* a_dev, const float
                              double* workspace_dev, void* stream);
 int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
                                        double* stats_dev, double* workspace_dev, void* stream);
+/* The two passes of madrl_moments_agents_f32 one at a time, for statistics pooled over the shards of a batch
+ * (the same kernels, grid and combination order; A = 1 is the whole batch).  pass 0 writes the SUMS of the three
+ * series to stats[.][0..2] and their minima to stats[.][6..8]; pass 1 reads means from stats[.][0..2] and writes
+ * the SUMS of squared deviations about them to stats[.][3..5].  Dividing by the rows gives madrl_moments_*'s
+ * bits.  madrl_center_apply_f32: the centring / shifting of madrl_center_advantages_* with the given stats
+ * [A][MADRL_MOMENTS_STATS] (mean [0], variance [3], minimum [6]).  MADRL_EINVAL as madrl_moments_agents_f32, or
+ * for a pass other than 0 and 1. */
+int madrl_moments_pass_f32(size_t rows, int A, const float* a_dev, const float* b_dev, int pass, double* stats_dev,
+                           double* workspace_dev, void* stream);
+int madrl_center_apply_f32(size_t rows, int A, float* adv_dev, const double* stats_dev, int center, int positive,
+                           void* stream);
 
 /* Path packing: time-major rollout tensors -> rllab's per-(env, episode, agent) paths
  * (rllab/rllab/sampler/ma_sampler.py:52-100 `dec_rollout`, episodes cut at `done` as
@@ -623,6 +634,15 @@ int madrl_time_baseline_f32(int T, int E, int A, int per_agent, int L, const flo
                             const int32_t* seg_start_dev, const int32_t* n_ep_dev, const int32_t* ep_rec_dev,
                             const int32_t* t0_dev, double* bin_sum_dev, int32_t* bin_count_dev, float* simplev_dev,
                             void* ws_dev, void* stream);
+/* madrl_time_baseline_f32 in two calls, so that the bins of the shards of a batch can be summed in between:
+ * _bins writes bin_sum / bin_count (ws as for madrl_time_baseline_f32), _apply writes simplev from the bins it is
+ * given.  Same kernels; _bins then _apply on the same arguments give madrl_time_baseline_f32's bits. */
+int madrl_time_baseline_bins_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
+                                 const int32_t* n_ep_dev, const int32_t* ep_rec_dev, const int32_t* t0_dev,
+                                 double* bin_sum_dev, int32_t* bin_count_dev, void* ws_dev, void* stream);
+int madrl_time_baseline_apply_f32(int T, int E, int A, int per_agent, int L, const int32_t* seg_start_dev,
+                                  const int32_t* t0_dev, const double* bin_sum_dev, const int32_t* bin_count_dev,
+                                  float* simplev_dev, void* stream);
 
 /* rltools' LinearFeatureBaseline (rltools/rltools/baselines/linear.py): the madrl_lfb_* kernels with rltools'
  * feature map, Df = D + 3: [(o - mu) / s, i/100, (i/100)^2, 1] with o widened to float64 and not clipped.

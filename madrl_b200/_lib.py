@@ -176,6 +176,8 @@ def _signatures():
         "madrl_center_advantages_f32": (i32, [sz, vp, i32, i32, vp, vp, vp]),
         "madrl_moments_agents_f32": (i32, [sz, i32, vp, vp, vp, vp, vp]),
         "madrl_center_advantages_agents_f32": (i32, [sz, i32, vp, i32, i32, vp, vp, vp]),
+        "madrl_moments_pass_f32": (i32, [sz, i32, vp, vp, i32, vp, vp, vp]),
+        "madrl_center_apply_f32": (i32, [sz, i32, vp, vp, i32, i32, vp]),
         # path packing and padding
         "madrl_paths_plan": (i32, [i32, i32, i32] + [vp] * 6),
         "madrl_paths_pack_u32": (i32, [i32] * 4 + [vp] * 6),
@@ -200,6 +202,8 @@ def _signatures():
         "madrl_running_moments_bf16": (i32, [sz, i32, i32, sz] + [vp] * 5),
         "madrl_time_baseline_workspace_size": (i32, [i32, i32, P(sz)]),
         "madrl_time_baseline_f32": (i32, [i32] * 5 + [vp] * 10),
+        "madrl_time_baseline_bins_f32": (i32, [i32] * 5 + [vp] * 8),
+        "madrl_time_baseline_apply_f32": (i32, [i32] * 5 + [vp] * 6),
         # rltools' linear feature baseline
         "madrl_lfbr_workspace_size": (i32, [i32, P(sz)]),
         "madrl_lfbr_agents_workspace_size": (i32, [i32, i32, P(sz)]),

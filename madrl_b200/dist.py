@@ -81,6 +81,63 @@ def gather_trajectories(tensors, env_dim=1, group=None, dst=None, equal_shards=T
     return tuple(out)
 
 
+def _world(group):
+    return dist.get_world_size(group) if dist.is_initialized() else 1
+
+
+def _gather_parts(t, group):
+    """[W, *t.shape]: every rank's `t` in rank order.  A gloo group exchanges through host memory (the partials
+    are small); the result lives on t's device."""
+    t = t.contiguous()
+    src = t.cpu() if dist.get_backend(group) == "gloo" else t
+    buf = torch.empty((_world(group) * t.numel(),), dtype=t.dtype, device=src.device)
+    dist.all_gather_into_tensor(buf, src.reshape(-1), group=group)
+    return buf.view((_world(group),) + tuple(t.shape)).to(t.device)
+
+
+def _pool(t, group, combine):
+    if t.dtype not in (torch.float64, torch.int64):
+        raise ValueError("pooled partials must be float64 or int64, got %s" % t.dtype)
+    if _world(group) == 1:
+        return t
+    parts = _gather_parts(t, group)
+    out = parts[0].clone()
+    for r in range(1, parts.shape[0]):          # ascending rank order: the same bits on every rank
+        out = combine(out, parts[r])
+    return out
+
+
+def pool_sum(t, group):
+    """The sum over `group`'s ranks of each rank's float64 or int64 partial `t` (the same shape on every rank),
+    added in ascending rank order by an explicit loop, not by the collective's own reduction: every rank gets the
+    same bits whatever the NCCL algorithm or topology.  A one-rank group returns `t` itself."""
+    return _pool(t, group, torch.add)
+
+
+def pool_max(t, group):
+    """The elementwise maximum of every rank's partial (as `pool_sum`)."""
+    return _pool(t, group, torch.maximum)
+
+
+def pool_min(t, group):
+    """The elementwise minimum of every rank's partial (as `pool_sum`)."""
+    return _pool(t, group, torch.minimum)
+
+
+def pool_cat(t, group):
+    """Every rank's `t` concatenated along its last axis in rank order (the other axes equal on every rank, the
+    last may differ): per-path values of env-contiguous shards come out in the unsharded batch's path order.  A
+    one-rank group returns `t` itself."""
+    if _world(group) == 1:
+        return t
+    n = t.shape[-1]
+    sizes = [int(v) for v in _gather_parts(torch.tensor([n], dtype=torch.int64, device=t.device), group)[:, 0]]
+    padded = torch.zeros(tuple(t.shape[:-1]) + (max(sizes),), dtype=t.dtype, device=t.device)
+    padded[..., :n] = t
+    parts = _gather_parts(padded, group)
+    return torch.cat([parts[r][..., :s] for r, s in enumerate(sizes)], dim=-1)
+
+
 def _align(n, a=16):
     return (n + a - 1) // a * a
 

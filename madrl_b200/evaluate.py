@@ -16,7 +16,15 @@ Each env of the engine runs episodes back to back from ``engine.reset()``; an ep
 K * max_path_length steps, so every env completes at least K episodes, and the first K of env e are records
 k * E + e; the statistics take records 0 .. n_trajs - 1.  The rollout runs in launches of ``chunk`` steps;
 ``madrl_eval_episodes_*`` folds each launch into the records on the device, and the records are read to the host
-once, at the end.  Differences from the reference (DESIGN §8): exactly ``n_trajs`` episodes (its workers also
+once, at the end.
+
+With ``group`` (a ``torch.distributed`` group whose ranks each hold one shard of the env batch, built by
+``dist.make_sharded``) E is the global batch: K = ceil(n_trajs / E_global), each rank records its own envs' episodes,
+and the reading gathers every rank's records into the unsharded order k * E_global + global env id.  The env
+kernels key their random streams by the global env id and do the same work per env whatever the shard, so the
+result equals the unsharded evaluation's, on every rank.
+
+Differences from the reference (DESIGN §8): exactly ``n_trajs`` episodes (its workers also
 return the episodes still running when the n_trajs-th arrives); each env's first K episodes (not the first
 n_trajs to finish anywhere, which over-represents short episodes); Philox streams instead of one
 ``np.random.seed`` per trajectory; q stays finite where discount^t underflows.
@@ -30,7 +38,18 @@ from ._lib import _ptr
 MODES = ("centralized", "decentralized", "concurrent")
 
 
-def _plan(engine, n_trajs, discount, mode, chunk):
+def _global_envs(engine, group):
+    """The envs of the whole batch: the engine's own, or with a group of several ranks its shard's global size."""
+    from .dist import _world
+    if group is None or _world(group) == 1:
+        return engine.n_envs
+    shard = getattr(engine, "shard", None)
+    if shard is None:
+        raise ValueError("an evaluation over several ranks needs an engine built by dist.make_sharded")
+    return int(shard[2])
+
+
+def _plan(engine, n_trajs, discount, mode, chunk, group=None):
     """(max_traj_len, K) of an evaluation; raises ValueError for arguments the evaluation cannot run."""
     if mode not in MODES:
         raise ValueError("mode must be one of %s, got %r" % (", ".join(MODES), mode))
@@ -43,7 +62,7 @@ def _plan(engine, n_trajs, discount, mode, chunk):
     mpl = int(engine.cfg.max_path_length)
     if mpl < 1:
         raise ValueError("evaluation needs an engine built with max_path_length > 0 (the reference's max_traj_len)")
-    return mpl, -(-int(n_trajs) // engine.n_envs)
+    return mpl, -(-int(n_trajs) // _global_envs(engine, group))
 
 
 class EpisodeRecords(object):
@@ -78,12 +97,24 @@ class EpisodeRecords(object):
             _lib.check(fn(T, E, A, C, _ptr(rew), _ptr(done), _ptr(info), self.discount, self.K, _ptr(self.carry),
                           _ptr(self.ret), _ptr(self.qsum), _ptr(self.len), _ptr(self.info_sum), _lib.stream(dev)))
 
-    def read(self, n):
-        buf = self._buf.cpu().numpy()
-        o1, o2, o3 = (8 * sum(self._words[:i]) for i in (1, 2, 3))
-        N, A, C = self.K * self.E, self.A, self.C
-        return (buf[:o1].view(np.float64).reshape(N, A)[:n], buf[o1:o2].view(np.float64).reshape(N, A)[:n],
-                buf[o3:].view(np.int32)[:n], buf[o2:o3].view(np.int64).reshape(N, C)[:n])
+    def read(self, n, group=None):
+        """Records 0 .. n-1.  ``group``: those of the whole batch, from every rank's records gathered in one
+        exchange (`dist.pool_cat` over env-contiguous shards), in the order k * E_global + global env id."""
+        if group is None:
+            buf = self._buf.cpu().numpy()
+            o1, o2, o3 = (8 * sum(self._words[:i]) for i in (1, 2, 3))
+            N, A, C = self.K * self.E, self.A, self.C
+            return (buf[:o1].view(np.float64).reshape(N, A)[:n], buf[o1:o2].view(np.float64).reshape(N, A)[:n],
+                    buf[o3:].view(np.int32)[:n], buf[o2:o3].view(np.int64).reshape(N, C)[:n])
+        from .dist import pool_cat
+        K, E, A, C = self.K, self.E, self.A, self.C
+        fields = (self.ret, self.qsum, self.info_sum, self.len.view(-1, 1))
+        rec = torch.cat([f.view(K, E, -1).view(torch.uint8) for f in fields], dim=2)      # [K, E, bytes per record]
+        rec = pool_cat(rec.transpose(1, 2).contiguous(), group).transpose(1, 2).reshape(-1, rec.shape[2])[:n]
+        rec = rec.cpu().numpy()
+        o1, o2, o3 = 8 * A, 16 * A, 16 * A + 8 * C
+        return (rec[:, :o1].copy().view(np.float64), rec[:, o1:o2].copy().view(np.float64),
+                rec[:, o3:].copy().view(np.int32)[:, 0], rec[:, o2:o3].copy().view(np.int64))
 
 
 def statistics(ret, qsum, length, info_sum, mode, info_keys):
@@ -102,17 +133,18 @@ def statistics(ret, qsum, length, info_sum, mode, info_keys):
 
 
 def evaluate_policy(engine, policy, n_trajs, discount, mode, chunk=64, state0=None, frame_stack=1, standardizer=None,
-                    graph=True):
+                    graph=True, group=None):
     """rltools' evaluate_policy for a PyTorch `policy` (the ``PolicyRollout`` interface: ``policy(obs, state) ->
     (actions, extras, state)``), run as ``PolicyRollout`` launches of `chunk` steps (one more of the remaining
     steps).  `state0`: the policy's initial recurrent state (zeroed again at every episode start by the loop).
     `frame_stack` / `standardizer`: the observation wrappers of ``PolicyRollout``, started as its docstring
     describes (the reset observation updates the standardiser, then fills the stack); the standardiser's state
     is updated in place.  The rewards recorded are the ones the rollout returns (after the standardiser's reward
-    side, if enabled).  The engine is reset first; it is left where the evaluation ended."""
+    side, if enabled).  The engine is reset first; it is left where the evaluation ended.  ``group``: evaluate over
+    the env shards of its ranks (see the module docstring); every rank gets the whole batch's dict."""
     from .closed_loop import PolicyRollout
     from .postproc import FrameStack
-    mpl, K = _plan(engine, n_trajs, discount, mode, chunk)
+    mpl, K = _plan(engine, n_trajs, discount, mode, chunk, group)
     rec = EpisodeRecords(engine, K, discount)
     steps = K * mpl
     with torch.cuda.device(engine.device):
@@ -131,10 +163,10 @@ def evaluate_policy(engine, policy, n_trajs, discount, mode, chunk=64, state0=No
                 r = loop(obs0, state)
                 rec.add(r.rew, r.done, r.info)
                 obs0, state = r.policy_obs[-1], r.state
-    return statistics(*rec.read(int(n_trajs)), mode, engine._info_keys)
+    return statistics(*rec.read(int(n_trajs), group), mode, engine._info_keys)
 
 
-def evaluate_heuristic(engine, n_trajs, discount, mode, chunk=64, norm="env", py2_division=True):
+def evaluate_heuristic(engine, n_trajs, discount, mode, chunk=64, norm="env", py2_division=True, group=None):
     """rltools' evaluate_policy for the reference's hand-written policy of the engine's family, evaluated inside
     the rollout kernels (``rollout_heuristic``) in launches of `chunk` steps:
 
@@ -143,13 +175,13 @@ def evaluate_heuristic(engine, n_trajs, discount, mode, chunk=64, norm="env", py
     * Pursuit: the per-agent policy of heuristics/pursuit.py; `py2_division` as in ``rollout_heuristic``.
     * Hostage: the reference has no heuristic; raises ValueError.
 
-    The engine is reset first; it is left where the evaluation ended."""
+    The engine is reset first; it is left where the evaluation ended.  ``group`` as for `evaluate_policy`."""
     fam = engine._abi
     if fam == "hostage":
         raise ValueError("the reference has no Hostage heuristic policy")
     if fam == "ww" and norm not in ("agent", "env"):
         raise ValueError("norm must be 'agent' or 'env', got %r" % (norm,))
-    mpl, K = _plan(engine, n_trajs, discount, mode, chunk)
+    mpl, K = _plan(engine, n_trajs, discount, mode, chunk, group)
     rec = EpisodeRecords(engine, K, discount)
     steps = K * mpl
     kw = dict(norm=norm) if fam == "ww" else dict(py2_division=py2_division)
@@ -164,4 +196,4 @@ def evaluate_heuristic(engine, n_trajs, discount, mode, chunk=64, norm="env", py
             rec.add(rew, done, info)
             obs0.copy_(obs[T - 1])
             t += T
-    return statistics(*rec.read(int(n_trajs)), mode, engine._info_keys)
+    return statistics(*rec.read(int(n_trajs), group), mode, engine._info_keys)

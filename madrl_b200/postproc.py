@@ -103,17 +103,50 @@ def _agent_columns(t, name):
     return t.numel() // A, A
 
 
-def center_advantages(adv, center=True, positive=False, inplace=False, per_agent=False):
+def _pooled_moments(a, b, A, group):
+    """float64 [A, 9] moments of the columns of a, b [rows, A] over every rank of a ``torch.distributed`` group:
+    the sums and row counts pooled give the means, the sums of squared deviations about those means pooled give
+    the population variances (NumPy's two passes over the union of the shards), the minima pool by their
+    minimum.  `dist.pool_sum` combines in rank order, so every rank gets the same bits; one rank gets
+    `moments_agents`'s (the division by the rows happens once, on the pooled sums)."""
+    from .dist import pool_min, pool_sum
+    rows, dev = a.numel() // A, a.device
+    stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=dev)
+    ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=dev)
+    fn = _lib.lib().madrl_moments_pass_f32
+    with torch.cuda.device(dev):
+        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 0, _ptr(stats), _ptr(ws), _lib.stream(dev)))
+    count = torch.full((A, 1), float(rows), dtype=torch.float64, device=dev)
+    sums = pool_sum(torch.cat([stats[:, 0:3], count], dim=1), group)
+    stats[:, 6:9] = pool_min(stats[:, 6:9].contiguous(), group)
+    n = sums[:, 3:4]
+    stats[:, 0:3] = sums[:, 0:3] / n
+    with torch.cuda.device(dev):
+        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 1, _ptr(stats), _ptr(ws), _lib.stream(dev)))
+    stats[:, 3:6] = pool_sum(stats[:, 3:6].contiguous(), group) / n
+    return stats
+
+
+def center_advantages(adv, center=True, positive=False, inplace=False, per_agent=False, group=None):
     """``util.center_advantages`` / ``util.shift_advantages_to_positive`` over every sample of the
     batch (base.py:82-86 applies them to the concatenation of all paths): float64 mean / population
     std / min computed on the device, deterministic.  Returns the processed tensor (same shape).
     ``per_agent=True``: the last axis of ``adv`` (e.g. [T,E,A]) is the agent, and each agent's samples are
     centred with their own statistics, as the concurrent sampler does per agent
-    (batch_ma_sampler.py:102-106)."""
+    (batch_ma_sampler.py:102-106).  ``group``: a ``torch.distributed`` group whose ranks hold the shards of one
+    batch: the statistics are the whole batch's (`moments` with ``group``), the same on every rank."""
     if per_agent:
         rows, A = _agent_columns(adv, "adv")
     _lib.require_tensor(adv, "adv", torch.float32, (...,), "cuda", contiguous=False)
     out = adv.contiguous() if inplace else adv.contiguous().clone()
+    if group is not None:
+        if not per_agent:
+            rows, A = out.numel(), 1
+        stats = _pooled_moments(out, None, A, group)
+        with torch.cuda.device(out.device):
+            _lib.check(_lib.lib().madrl_center_apply_f32(rows, A, _ptr(out), _ptr(stats), int(bool(center)),
+                                                         int(bool(positive)), _lib.stream(out.device)))
+        return out
     if per_agent:
         stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=out.device)
         ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=out.device)
@@ -130,14 +163,18 @@ def center_advantages(adv, center=True, positive=False, inplace=False, per_agent
     return out
 
 
-def moments(a, b=None):
+def moments(a, b=None, group=None):
     """float64 [9] cuda tensor: means, population variances and minima of the series a, b, b - a
-    (b of a's shape) taken over every element (NumPy's two-pass ``var``)."""
+    (b of a's shape) taken over every element (NumPy's two-pass ``var``).  ``group``: a ``torch.distributed``
+    group whose ranks hold the shards of one batch: the moments of the whole batch, the same bits on every rank
+    (a one-rank group gives ``group=None``'s bits)."""
     _lib.require_tensor(a, "a", torch.float32, (...,), None, contiguous=False)
     _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
     _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
     a = a.contiguous()
     b = b.contiguous() if b is not None else None
+    if group is not None:
+        return _pooled_moments(a, b, 1, group)[0]
     stats, ws = _moments_buffers(a.device)
     with torch.cuda.device(a.device):
         _lib.check(_lib.lib().madrl_moments_f32(a.numel(), _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
@@ -145,14 +182,16 @@ def moments(a, b=None):
     return stats
 
 
-def moments_agents(a, b=None):
+def moments_agents(a, b=None, group=None):
     """float64 [A, 9] cuda tensor: ``moments`` of each agent's samples, the agent being the last axis of
-    a (and b), e.g. [T,E,A]."""
+    a (and b), e.g. [T,E,A].  ``group`` as for `moments`."""
     rows, A = _agent_columns(a, "a")
     _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
     _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
     a = a.contiguous()
     b = b.contiguous() if b is not None else None
+    if group is not None:
+        return _pooled_moments(a, b, A, group)
     stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=a.device)
     ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=a.device)
     with torch.cuda.device(a.device):
@@ -168,13 +207,14 @@ def _explained_variance_1d(st):
     return 1 - var_res / (vary + 1e-8)
 
 
-def explained_variance(ypred, y, per_agent=False):
+def explained_variance(ypred, y, per_agent=False, group=None):
     """``special.explained_variance_1d`` (special.py:51-59) of baseline predictions against returns,
     over every sample of the batch; one 72-byte device->host read.  ``per_agent=True``: one value per
-    agent (the last axis), over that agent's samples -- a list of A floats."""
+    agent (the last axis), over that agent's samples -- a list of A floats.  ``group`` as for `moments`."""
+    kw = {} if group is None else dict(group=group)
     if per_agent:
-        return [_explained_variance_1d(st) for st in moments_agents(ypred, y).cpu().numpy()]
-    return _explained_variance_1d(moments(ypred, y).cpu().numpy())
+        return [_explained_variance_1d(st) for st in moments_agents(ypred, y, **kw).cpu().numpy()]
+    return _explained_variance_1d(moments(ypred, y, **kw).cpu().numpy())
 
 
 class FrameStack(object):
@@ -501,7 +541,9 @@ def process_samples_concurrent(baseline, obs, done, rew, discount, gae_lambda, o
     -- the returns do not depend on the values -- and then predicts.
 
     obs [T,E,A,D], done [T,E] uint8, rew [T,E,A] float32 (cuda) -> (values, advantages, returns) [T,E,A] and the
-    A explained variances (a list of floats)."""
+    A explained variances (a list of floats).  ``group``: a ``torch.distributed`` group whose ranks hold the env
+    shards of one batch: the fit's normal equations are summed over its ranks, and the explained variances and
+    the centring statistics are the whole batch's (`moments_agents` with ``group``)."""
     if not isinstance(baseline, LinearFeatureBaseline) or baseline.n_agents is None:
         raise ValueError("process_samples_concurrent needs a LinearFeatureBaseline built with n_agents")
     T, E, A, _ = _lib.require_tensor(obs, "obs", _OBS_DTYPES, (None, None, baseline.n_agents, baseline.obs_dim),
@@ -526,9 +568,10 @@ def _sampler_core(baseline, obs, done, rew, discount, gae_lambda, obs_before, t0
     else:
         values = baseline.predict(obs, done, obs_before, t0)
         adv, ret = gae(rew, values, done, discount, gae_lambda)
-    ev = explained_variance(values, ret, per_agent=per_agent)
+    kw = {} if group is None else dict(group=group)
+    ev = explained_variance(values, ret, per_agent=per_agent, **kw)
     if center or positive:
-        adv = center_advantages(adv, center, positive, inplace=True, per_agent=per_agent)
+        adv = center_advantages(adv, center, positive, inplace=True, per_agent=per_agent, **kw)
     return values, adv, ret, ev
 
 
@@ -793,6 +836,16 @@ def _statistics(sums, first_ret):
     return out if sums.dim() == 2 else out[0]
 
 
+def _pooled_statistics(sums, first_ret, group):
+    """`_statistics` over the paths of every rank of `group` (None: this rank's): each rank's per-path values,
+    8 bytes each, gathered in rank order (`dist.pool_cat`) -- for env-contiguous shards the unsharded batch's
+    path order, so the statistics are the unsharded ones bit for bit, and those of one rank its own."""
+    if group is not None:
+        from .dist import pool_cat
+        sums, first_ret = pool_cat(torch.stack([sums, first_ret]), group).unbind(0)
+    return _statistics(sums, first_ret)
+
+
 def path_returns(rew, ret, done, per_agent=False):
     """Per path (episodes cut at ``done``): the undiscounted return ``sum(path["rewards"])`` (float64, in time
     order) and the first return ``path["returns"][0]`` -- float64 tensors [P] in (env, episode, agent) order, or
@@ -807,14 +860,16 @@ def path_returns(rew, ret, done, per_agent=False):
     return _PathTable(done, A, per_agent).sums(rew, ret)
 
 
-def path_statistics(rew, ret, done, per_agent=False):
+def path_statistics(rew, ret, done, per_agent=False, group=None):
     """The return statistics both branches of ``process_samples`` log (base.py:144-147, :170-180):
     ``AverageDiscountedReturn`` (mean of the paths' first returns), ``AverageReturn``, ``StdReturn`` (population),
     ``MaxReturn``, ``MinReturn`` (over the paths' undiscounted returns) and ``NumTrajs``, as Python numbers in a
     dict; ``per_agent=True`` (concurrent control): a list of A dicts, agent a's over its own paths.  Arguments as
     `path_returns`.  Unlike `EpisodeStats` every path counts, including the unfinished one at the end of the
-    rollout, and nothing is averaged over agents."""
-    return _statistics(*path_returns(rew, ret, done, per_agent))
+    rollout, and nothing is averaged over agents.  ``group``: a ``torch.distributed`` group whose ranks hold the env
+    shards of one batch: the statistics are over the paths of every rank, the same on every rank and equal to the
+    unsharded batch's (`_pooled_statistics`)."""
+    return _pooled_statistics(*path_returns(rew, ret, done, per_agent), group)
 
 
 def process_samples_recurrent(baseline, obs, actions, rew, done, discount, gae_lambda, mode, obs_before=None,
@@ -828,8 +883,10 @@ def process_samples_recurrent(baseline, obs, actions, rew, done, discount, gae_l
     (concurrent; ``shared=True`` is fitted first, as in `process_samples_concurrent`), pooled with
     ``obs_dim = A*D`` (centralized).  obs [T,E,A,D] float32 or bfloat16, actions [T,E,A,...], rew [T,E,A] float32,
     done [T,E] uint8; ``obs_before``, ``t0`` as for the baseline, ``infos``, ``agent_infos`` as for `pad_paths`.
-    ``group``: a ``torch.distributed`` group the baseline's normal equations are summed over; the statistics stay
-    per rank.
+    ``group``: a ``torch.distributed`` group whose ranks hold the env shards of one batch: the baseline's normal
+    equations are summed over its ranks, the explained variance and the centring use the whole batch's moments,
+    and the return statistics are over every rank's paths (`path_statistics` with ``group``).  Padding stays per
+    rank: each rank's batch holds its own paths.
 
     Two quirks of the reference are kept: the branch has no ``positive_adv`` (rllab ignores the flag there), and
     centring always divides by ``std + 1e-8``.  Centring is over every sample (per agent for concurrent control)
@@ -856,7 +913,7 @@ def process_samples_recurrent(baseline, obs, actions, rew, done, discount, gae_l
     table = _PathTable(done, obs.shape[2], concurrent)
     data = _pad_all(table, obs, actions, rew, infos, obs_before, agent_infos)
     data.update(advantages=table.pad(adv), returns=table.pad(ret))
-    stats = _statistics(*table.sums(rew, ret))
+    stats = _pooled_statistics(*table.sums(rew, ret), group)
     if not baseline.shared:
         baseline.fit(obs, done, ret, obs_before, t0, group)
     out = dict(data, paths=PaddedPaths(mode=mode, **data, **table.records()), values=values, ExplainedVariance=ev)

@@ -23,6 +23,7 @@ import torch
 
 from . import _lib, postproc
 from ._lib import _ptr
+from .dist import pool_cat, pool_max, pool_sum
 from .postproc import _OBS_DTYPES, AGENTS_MAX, _check_mode, _paths_plan
 
 
@@ -113,24 +114,35 @@ class RunningStandardizer(object):
         new_meansq = ((a.unsqueeze(-1) * meansq).double() + b.unsqueeze(-1) * (sums[..., 1, :] / n)).float()
         return count + n, new_mean, new_meansq
 
-    def update(self, x, obs_before=None):
-        """x [..., D] (every row; [..., A, D] with n_agents: agent a's rows update standardiser a); rows of a
-        rollout [T, E, A, D] with ``obs_before`` are the observations the actions were taken in."""
-        groups = 1 if self.n_agents is None else self.n_agents
+    def _pooled_sums(self, x, obs_before, groups, group):
+        """`_sums`, summed over the ranks of a ``torch.distributed`` ``group`` (`dist.pool_sum`) if one is given."""
         sums, n = self._sums(x, obs_before, groups)
+        if group is not None:
+            sums = pool_sum(sums, group)
+            n = int(pool_sum(torch.tensor([n], dtype=torch.int64, device=sums.device), group)[0])
+        return sums, n
+
+    def update(self, x, obs_before=None, group=None):
+        """x [..., D] (every row; [..., A, D] with n_agents: agent a's rows update standardiser a); rows of a
+        rollout [T, E, A, D] with ``obs_before`` are the observations the actions were taken in.  ``group``: a
+        ``torch.distributed`` group whose ranks hold the shards of one batch: the column sums and the row count
+        are pooled over its ranks before the mix, so every rank holds the same state (the whole batch's update)."""
+        groups = 1 if self.n_agents is None else self.n_agents
+        sums, n = self._pooled_sums(x, obs_before, groups, group)
         if self.n_agents is None:
             sums = sums[0]
         self.count, self.mean, self.meansq = self._mix(self.count, self.mean, self.meansq, sums, n)
         self._refresh()
 
-    def update_per_agent(self, x, obs_before=None):
+    def update_per_agent(self, x, obs_before=None, group=None):
         """One update per agent, in agent order, with agent a's rows of x [..., A, D]: rltools' concurrent optimizer
-        updates its single reward normaliser this way (algos/policyopt.py:221-231).  Needs n_agents=None."""
+        updates its single reward normaliser this way (algos/policyopt.py:221-231).  Needs n_agents=None.
+        ``group`` as for `update`."""
         if self.n_agents is not None:
             raise ValueError("update_per_agent updates one standardiser A times: it needs n_agents=None")
         if x.dim() < 2 or not 1 <= x.shape[-2] <= AGENTS_MAX:
             raise ValueError("x must be [..., A, D] with A in [1, %d], got shape %s" % (AGENTS_MAX, tuple(x.shape)))
-        sums, n = self._sums(x, obs_before, int(x.shape[-2]))
+        sums, n = self._pooled_sums(x, obs_before, int(x.shape[-2]), group)
         count, mean, meansq = self.count, self.mean, self.meansq
         for a in range(sums.shape[0]):
             count, mean, meansq = self._mix(count, mean, meansq, sums[a], n)
@@ -196,10 +208,11 @@ class LinearFeatureBaseline(postproc.LinearFeatureBaseline):
         if norm is not None:
             self.obsnorm.set_param_values(*norm)
 
-    def update_obsnorm(self, obs, obs_before=None):
-        """The baseline's obsnorm update from a batch's observation rows (a no-op without obsnorm)."""
+    def update_obsnorm(self, obs, obs_before=None, group=None):
+        """The baseline's obsnorm update from a batch's observation rows (a no-op without obsnorm); ``group`` as
+        for `RunningStandardizer.update`."""
         if self.obsnorm is not None:
-            self.obsnorm.update(obs, obs_before)
+            self.obsnorm.update(obs, obs_before, group)
 
     def solve(self, G):
         """Coefficients from normal equations G ([Df+1, Df+1] or [A, Df+1, Df+1]): one (batched) Cholesky; raises
@@ -224,13 +237,15 @@ def _check_rollout(q_like, name, done, t0):
     return T, E, A
 
 
-def time_baseline(q, done, t0=None, per_agent=False):
+def time_baseline(q, done, t0=None, per_agent=False, group=None):
     """The time-dependent baseline of ``Sampler.process`` (samplers/__init__.py:46-52): for each time index i (a
     row's position in its path, plus ``t0[e]`` on env e's first path -- the baseline's own index), the mean of q
     over the paths that reach i.  q [T,E,A] float32, done [T,E] uint8 (cuda).  Returns ``simplev`` [T,E,A] float32
     (each row's bin mean), the float64 bin sums and the int32 counts [G, L] (G = A with ``per_agent``, one set of
     bins per agent; else 1 over every agent's rows; L = the largest index + 1).  Deterministic; one 4-byte
-    device->host read (L)."""
+    device->host read (L).  ``group``: a ``torch.distributed`` group whose ranks hold the env shards of one batch:
+    L is the largest over the ranks and the bins are summed over them (`dist.pool_sum`) before ``simplev`` is
+    written, so every rank uses the whole batch's bins."""
     T, E, A = _check_rollout(q, "q", done, t0)
     G = A if per_agent else 1
     if G > AGENTS_MAX:
@@ -240,6 +255,8 @@ def time_baseline(q, done, t0=None, per_agent=False):
     last = ep_rec[:, :, 1].max()
     if t0 is not None:
         last = torch.maximum(last, (t0.to(torch.int32) + ep_rec[:, 0, 1]).max())
+    if group is not None:
+        last = pool_max(last.to(torch.int64).reshape(1), group)[0]
     L = int(last)
     if L < 1:
         raise ValueError("t0 must be >= 0")
@@ -251,6 +268,17 @@ def time_baseline(q, done, t0=None, per_agent=False):
     bin_sum = torch.empty((G, L), dtype=torch.float64, device=dev)
     bin_cnt = torch.empty((G, L), dtype=torch.int32, device=dev)
     simplev = torch.empty_like(q)
+    if group is not None:
+        with torch.cuda.device(dev):
+            _lib.check(lib.madrl_time_baseline_bins_f32(T, E, A, int(bool(per_agent)), L, _ptr(q), _ptr(n_ep),
+                                                        _ptr(ep_rec), _ptr(t0), _ptr(bin_sum), _ptr(bin_cnt), _ptr(ws),
+                                                        _lib.stream(dev)))
+        bin_sum = pool_sum(bin_sum, group).contiguous()
+        bin_cnt = pool_sum(bin_cnt.to(torch.int64), group).to(torch.int32).contiguous()
+        with torch.cuda.device(dev):
+            _lib.check(lib.madrl_time_baseline_apply_f32(T, E, A, int(bool(per_agent)), L, _ptr(seg_s), _ptr(t0),
+                                                         _ptr(bin_sum), _ptr(bin_cnt), _ptr(simplev), _lib.stream(dev)))
+        return simplev, bin_sum, bin_cnt
     with torch.cuda.device(dev):
         _lib.check(lib.madrl_time_baseline_f32(T, E, A, int(bool(per_agent)), L, _ptr(q), _ptr(seg_s), _ptr(n_ep),
                                                _ptr(ep_rec), _ptr(t0), _ptr(bin_sum), _ptr(bin_cnt), _ptr(simplev),
@@ -296,6 +324,11 @@ def process_samples(baseline, obs, done, rew, discount, gae_lambda, rewnorm=None
     7. GAE(γ, λ) with r' and the values chosen, bootstrap 0 at each path's end;
     8. ``baseline.fit`` to q (summed over a ``torch.distributed`` ``group``'s ranks if given).
 
+    With a ``group`` whose ranks hold the env shards of one batch, steps 3 and 5 pool over its ranks
+    (`time_baseline` and `postproc.moments` with ``group``), so ``v_r``, ``tv_r`` and ``fallback`` are the whole
+    batch's and the same on every rank; ``rewnorm`` and the baseline's obsnorm are the caller's to update with the
+    same ``group``.
+
     obs [T,E,A,D] float32 or bfloat16, done [T,E] uint8, rew [T,E,A] float32 (cuda); ``obs_before``, ``t0`` as for
     the baseline.  ``baseline``: `LinearFeatureBaseline` with ``obs_dim = D`` (decentralized), ``n_agents = A``
     (concurrent), ``obs_dim = A*D`` (centralized).  Returns a dict: ``advantages``, ``q`` and ``values`` (the values
@@ -318,9 +351,12 @@ def process_samples(baseline, obs, done, rew, discount, gae_lambda, rewnorm=None
     else:
         values = baseline.predict(obs, done, obs_before, t0)
     adv, q = postproc.gae(rew_n, values, done, discount, gae_lambda)
-    simplev = time_baseline(q, done, t0, per_agent)[0]
+    simplev = time_baseline(q, done, t0, per_agent, group)[0]
     mom = postproc.moments_agents if per_agent else postproc.moments
-    st = torch.stack([mom(q, values), mom(q, simplev)]).cpu().numpy()
+    if group is None:
+        st = torch.stack([mom(q, values), mom(q, simplev)]).cpu().numpy()
+    else:
+        st = torch.stack([mom(q, values, group=group), mom(q, simplev, group=group)]).cpu().numpy()
     v_r, tv_r = _explained(st[0]), _explained(st[1])
     fallback = v_r < 0
     if np.any(fallback):
@@ -336,12 +372,15 @@ def process_samples(baseline, obs, done, rew, discount, gae_lambda, rewnorm=None
     return dict(advantages=adv, q=q, values=values, v_r=v_r, tv_r=tv_r, fallback=fallback)
 
 
-def sample_fields(rew, done, mode="decentralized"):
+def sample_fields(rew, done, mode="decentralized", group=None):
     """The fields rltools' ``sample()`` logs (samplers/serial.py:36-47, :75-85, :114-130) from a rollout's raw
     rewards: ``ret`` (mean over paths of the undiscounted reward sums), ``batch`` (paths), ``avglen`` (int of the
     mean length), ``maxlen``, ``minlen`` and ``ravg`` (mean reward per step).  Concurrent control averages ``ret``,
     ``batch`` and ``ravg`` over the agents (their paths share the cuts, so the lengths are every agent's);
-    centralized control counts one path per episode with agent 0's reward.  rew [T,E,A] float32, done [T,E] uint8."""
+    centralized control counts one path per episode with agent 0's reward.  rew [T,E,A] float32, done [T,E] uint8.
+    ``group``: a ``torch.distributed`` group whose ranks hold the env shards of one batch: the fields are over the
+    paths of every rank (each path's sum and length gathered in rank order, `dist.pool_cat`), the same on every
+    rank and equal to the unsharded batch's."""
     _check_mode(mode)
     _check_rollout(rew, "rew", done, None)
     if mode == "centralized":
@@ -350,6 +389,8 @@ def sample_fields(rew, done, mode="decentralized"):
     table = postproc._PathTable(done, rew.shape[2], per_agent)
     sums, _ = table.sums(rew, rew)
     lens = table.rec[:, 3].view(table.lead).double()
+    if group is not None:
+        sums, lens = pool_cat(torch.stack([sums, lens]), group).unbind(0)
     steps = lens.sum(-1)
     vals = torch.stack([sums.mean(-1), sums.sum(-1) / steps, lens.mean(-1), lens.max(-1).values,
                         lens.min(-1).values], dim=-1).reshape(-1, 5).cpu().numpy()

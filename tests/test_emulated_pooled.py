@@ -1,0 +1,208 @@
+"""The entry points that split a statistic where the shards of a batch are pooled, executed on the CPU by the warp
+emulator of tests/emu through the C ABI: madrl_time_baseline_bins_f32 + madrl_time_baseline_apply_f32 against the
+fused madrl_time_baseline_f32, madrl_moments_pass_f32 against madrl_moments_f32 / madrl_moments_agents_f32 and
+madrl_center_apply_f32 against madrl_center_advantages_*.  On the same arguments the split calls give the fused
+calls' bits; the bins of two env halves, summed, give the whole batch's counts exactly and its simplev within one
+float32 ulp.  Outputs sit in canary-guarded buffers; the argument checks (MADRL_EINVAL, no launch) are exercised."""
+import ctypes as C
+
+import numpy as np
+import pytest
+
+import postproc_edges as pe
+from emu import build_emu, driver
+from emu.driver import Guarded
+from emu.driver import ptr as _p
+
+pytestmark = driver.needs_cxx
+
+EMU_MOM_BLOCKS = build_emu.GRID["MADRL_MOM_BLOCKS"]
+# (T, E, done probability): slices of one and several envs, L off and past the 128-thread bin block
+TB_SHAPES = ((5, 2, 0.3), (9, 7, 0.2), (140, 4, 0.0), (33, 11, 0.1))
+
+
+@pytest.fixture(scope="module")
+def lib():
+    return driver.load(())
+
+
+def _ws(lib, G, L):
+    nbytes = C.c_size_t()
+    assert lib.madrl_time_baseline_workspace_size(G, L, C.byref(nbytes)) == 0
+    return np.zeros(nbytes.value, np.uint8)
+
+
+def _fused(lib, q, done, t0, per_agent, L):
+    T, E, A = q.shape
+    G = A if per_agent else 1
+    seg_s, _, n_ep, ep_rec = driver.paths_plan(lib, done, A)
+    s, c, v = np.full((G, L), np.nan), np.full((G, L), -1, np.int32), np.full((T, E, A), np.nan, np.float32)
+    assert lib.madrl_time_baseline_f32(T, E, A, per_agent, L, _p(q), _p(seg_s), _p(n_ep), _p(ep_rec), _p(t0), _p(s),
+                                       _p(c), _p(v), _p(_ws(lib, G, L)), None) == 0
+    return s, c, v
+
+
+def _bins(lib, q, done, t0, per_agent, L):
+    T, E, A = q.shape
+    G = A if per_agent else 1
+    _, _, n_ep, ep_rec = driver.paths_plan(lib, done, A)
+    s, c = Guarded((G, L), np.float64, np.nan), Guarded((G, L), np.int32, -1)
+    assert lib.madrl_time_baseline_bins_f32(T, E, A, per_agent, L, _p(q), _p(n_ep), _p(ep_rec), _p(t0), _p(s.arr),
+                                            _p(c.arr), _p(_ws(lib, G, L)), None) == 0, lib.madrl_last_error()
+    return s.check("sums").copy(), c.check("counts").copy()
+
+
+def _apply(lib, done, t0, per_agent, A, L, s, c):
+    T, E = done.shape
+    seg_s = driver.paths_plan(lib, done, A)[0]
+    v = Guarded((T, E, A), np.float32, np.nan)
+    assert lib.madrl_time_baseline_apply_f32(T, E, A, per_agent, L, _p(seg_s), _p(t0), _p(s), _p(c), _p(v.arr),
+                                             None) == 0, lib.madrl_last_error()
+    return v.check("simplev").copy()
+
+
+def _case(A, k):
+    T, E, p = TB_SHAPES[k]
+    rs = np.random.RandomState(100 * A + k)
+    done = (rs.rand(T, E) < p).astype(np.uint8)
+    if T > 2:
+        done[0, 0] = done[T - 1, E - 1] = 1
+    q = rs.randn(T, E, A).astype(np.float32)
+    return q, done, (None, rs.randint(0, 6, E).astype(np.int32))
+
+
+def _last_index(done, t0):
+    """The largest time index of a rollout's rows (lfb_index), + 1."""
+    T, E = done.shape
+    L = 0
+    for e in range(E):
+        s = 0
+        for t in range(T):
+            L = max(L, t - s + (t0[e] if (t0 is not None and s == 0) else 0) + 1)
+            if done[t, e]:
+                s = t + 1
+    return L
+
+
+@pytest.mark.parametrize("A", (1, 2, 3, 5))
+def test_time_baseline_bins_then_apply_equal_the_fused_call(lib, A):
+    for k in range(len(TB_SHAPES)):
+        q, done, t0s = _case(A, k)
+        for t0 in t0s:
+            L = _last_index(done, t0)
+            for per_agent in (0, 1):
+                s, c, v = _fused(lib, q, done, t0, per_agent, L)
+                bs, bc = _bins(lib, q, done, t0, per_agent, L)
+                assert np.array_equal(bs, s) and np.array_equal(bc, c)
+                got = _apply(lib, done, t0, per_agent, A, L, bs, bc)
+                assert np.array_equal(got.view(np.uint32), v.view(np.uint32)), (k, per_agent)
+
+
+@pytest.mark.parametrize("A", (1, 3))
+def test_time_baseline_bins_of_two_env_halves_pool_to_the_whole_batch(lib, A):
+    """Each half's bins over the pooled L (a larger L than the half's own: zero bins past its paths), summed: the
+    whole batch's counts exactly, its sums to rounding, and each half's simplev within one float32 ulp of the
+    whole batch's rows."""
+    for k in range(len(TB_SHAPES)):
+        q, done, t0s = _case(A, k)
+        E = done.shape[1]
+        if E < 2:
+            continue
+        h = E // 2
+        for t0 in t0s:
+            L = _last_index(done, t0)
+            halves = [(slice(0, h), None if t0 is None else t0[:h].copy()),
+                      (slice(h, E), None if t0 is None else t0[h:].copy())]
+            for per_agent in (0, 1):
+                s, c, v = _fused(lib, q, done, t0, per_agent, L)
+                parts = [_bins(lib, np.ascontiguousarray(q[:, sl]), np.ascontiguousarray(done[:, sl]), t, per_agent,
+                               L) for sl, t in halves]
+                ps, pc = parts[0][0] + parts[1][0], parts[0][1] + parts[1][1]
+                assert np.array_equal(pc, c)
+                np.testing.assert_allclose(ps, s, rtol=1e-13, atol=1e-13)
+                for sl, t in halves:
+                    got = _apply(lib, np.ascontiguousarray(done[:, sl]), t, per_agent, A, L, ps, pc)
+                    d = np.abs(got.view(np.int32).astype(np.int64) - v[:, sl].view(np.int32).astype(np.int64))
+                    assert d.max() <= 1
+
+
+def _passes(lib, rows, A, a, b):
+    """madrl_moments_pass_f32's two passes, the means formed between them as the pooled host code forms them."""
+    st = Guarded((A, 9), np.float64, np.nan)
+    ws = np.empty((A, 4096))
+    assert lib.madrl_moments_pass_f32(rows, A, _p(a), _p(b), 0, _p(st.arr), _p(ws), None) == 0
+    sums = st.arr[:, 0:3].copy()
+    st.arr[:, 0:3] = sums / float(rows)
+    assert lib.madrl_moments_pass_f32(rows, A, _p(a), _p(b), 1, _p(st.arr), _p(ws), None) == 0
+    out = st.check("stats").copy()
+    return sums, out[:, 3:6].copy(), out[:, 6:9].copy(), out
+
+
+@pytest.mark.parametrize("A", (1, 2, 3))
+def test_moment_passes_equal_the_fused_moments_bitwise(lib, A):
+    """Sums over rows give madrl_moments_*'s means, the second pass about those means over rows its variances, and
+    the minima are its minima, bit for bit, at the grid-stride edges and with and without b."""
+    for rows in pe.stride_sizes(EMU_MOM_BLOCKS):
+        x, y = pe.agent_columns(rows, A, A)
+        for b in (y, None):
+            want, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
+            if A == 1:
+                assert lib.madrl_moments_f32(rows, _p(x), _p(b), _p(want), _p(ws), None) == 0
+            else:
+                assert lib.madrl_moments_agents_f32(rows, A, _p(x), _p(b), _p(want), _p(ws), None) == 0
+            sums, sq, mins, got = _passes(lib, rows, A, x, b)
+            cols = slice(0, 3) if b is not None else slice(0, 1)
+            assert np.array_equal((sums / float(rows))[:, cols], want[:, 0:3][:, cols]), rows
+            assert np.array_equal((sq / float(rows))[:, cols], want[:, 3:6][:, cols]), rows
+            assert np.array_equal(mins[:, cols], want[:, 6:9][:, cols]), rows
+
+
+@pytest.mark.parametrize("A", (1, 2, 3))
+def test_center_apply_equals_center_advantages_bitwise(lib, A):
+    rows = 2 * EMU_MOM_BLOCKS * 256 + 7
+    x, _ = pe.agent_columns(rows, A, A)
+    for center, positive in pe.CENTRE_MODES:
+        want = x.copy()
+        stats, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
+        if A == 1:
+            assert lib.madrl_center_advantages_f32(rows, _p(want), center, positive, _p(stats), _p(ws), None) == 0
+        else:
+            assert lib.madrl_center_advantages_agents_f32(rows, A, _p(want), center, positive, _p(stats), _p(ws),
+                                                          None) == 0
+        got = Guarded(x.shape, np.float32, x)
+        assert lib.madrl_center_apply_f32(rows, A, _p(got.arr), _p(stats), center, positive, None) == 0
+        assert np.array_equal(got.check("adv").view(np.uint32), want.view(np.uint32)), (center, positive)
+
+
+def test_split_entry_points_reject_bad_arguments(lib):
+    x, st, ws = np.zeros(8, np.float32), np.zeros(9), np.zeros(4096)
+    mp = lib.madrl_moments_pass_f32
+    assert mp(0, 1, _p(x), None, 0, _p(st), _p(ws), None) != 0
+    assert mp(8, 0, _p(x), None, 0, _p(st), _p(ws), None) != 0
+    assert mp(8, 1025, _p(x), None, 0, _p(st), _p(ws), None) != 0
+    assert mp(8, 1, _p(x), None, 2, _p(st), _p(ws), None) != 0
+    assert mp(8, 1, None, None, 0, _p(st), _p(ws), None) != 0
+    assert mp(8, 1, _p(x), None, 0, None, _p(ws), None) != 0
+    ca = lib.madrl_center_apply_f32
+    assert ca(0, 1, _p(x), _p(st), 1, 0, None) != 0
+    assert ca(8, 1025, _p(x), _p(st), 1, 0, None) != 0
+    assert ca(8, 1, None, _p(st), 1, 0, None) != 0
+    assert ca(8, 1, _p(x), None, 1, 0, None) != 0
+    q, i32, f64 = np.zeros(8, np.float32), np.zeros(64, np.int32), np.zeros(8)
+    tb, ta = lib.madrl_time_baseline_bins_f32, lib.madrl_time_baseline_apply_f32
+    good_b = [2, 2, 2, 0, 2, _p(q), _p(i32), _p(i32), None, _p(f64), _p(i32), _p(i32), None]
+    good_a = [2, 2, 2, 0, 2, _p(i32), None, _p(f64), _p(i32), _p(q), None]
+    for k in (0, 1, 2, 4):                  # T, E, A, L (3 is per_agent)
+        for fn, good in ((tb, good_b), (ta, good_a)):
+            bad = list(good)
+            bad[k] = 0
+            assert fn(*bad) != 0, (fn, k)
+    for k in (5, 6, 7, 9, 10, 11):
+        bad = list(good_b)
+        bad[k] = None
+        assert tb(*bad) != 0, k
+    for k in (5, 7, 8, 9):
+        bad = list(good_a)
+        bad[k] = None
+        assert ta(*bad) != 0, k
+    assert tb(2, 2, 1025, 1, 2, *good_b[5:]) != 0 and ta(2, 2, 1025, 1, 2, *good_a[5:]) != 0
