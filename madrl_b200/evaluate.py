@@ -22,7 +22,10 @@ With ``group`` (a ``torch.distributed`` group whose ranks each hold one shard of
 ``dist.make_sharded``) E is the global batch: K = ceil(n_trajs / E_global), each rank records its own envs' episodes,
 and the reading gathers every rank's records into the unsharded order k * E_global + global env id.  The env
 kernels key their random streams by the global env id and do the same work per env whatever the shard, so the
-result equals the unsharded evaluation's, on every rank.
+result equals the unsharded evaluation's, on every rank.  Before any record moves, the ranks exchange their
+shards and check that they tile [0, E_global) in group-rank order; otherwise every rank raises ValueError (an engine
+that `make_sharded` placed with torchrun's WORLD rank and size does not tile a smaller data-parallel group: build it
+with ``rank=`` and ``world=`` of the group).
 
 Differences from the reference (DESIGN §8): exactly ``n_trajs`` episodes (its workers also
 return the episodes still running when the n_trajs-th arrives); each env's first K episodes (not the first
@@ -39,14 +42,22 @@ MODES = ("centralized", "decentralized", "concurrent")
 
 
 def _global_envs(engine, group):
-    """The envs of the whole batch: the engine's own, or with a group of several ranks its shard's global size."""
-    from .dist import _world
+    """The envs of the whole batch: the engine's own, or with a group of several ranks the global size of the
+    shards, once every rank has checked that they tile it.  The ranks exchange their (lo, hi, E_global) in one
+    collective and apply the same rule to what they gathered, so they all raise or all go on."""
+    from .dist import _world, pool_cat
     if group is None or _world(group) == 1:
         return engine.n_envs
     shard = getattr(engine, "shard", None)
-    if shard is None:
-        raise ValueError("an evaluation over several ranks needs an engine built by dist.make_sharded")
-    return int(shard[2])
+    mine = (-1, -1, -1) if shard is None or int(shard[1]) - int(shard[0]) != engine.n_envs else shard
+    lo, hi, size = pool_cat(torch.tensor(mine, dtype=torch.int64, device=engine.device).view(3, 1),
+                            group).cpu().numpy()
+    E = int(size[0])
+    if not (lo[0] == 0 and (lo[1:] == hi[:-1]).all() and (hi > lo).all() and hi[-1] == E and (size == E).all()):
+        raise ValueError("an evaluation over several ranks needs engines built by dist.make_sharded whose shards "
+                         "tile the batch in group-rank order; got (lo, hi, n_envs_global) = %s"
+                         % [tuple(int(v) for v in c) for c in zip(lo, hi, size)])
+    return E
 
 
 def _plan(engine, n_trajs, discount, mode, chunk, group=None):

@@ -10,6 +10,7 @@ import numpy as np
 import pytest
 
 import postproc_edges as pe
+import sharded_edges as se
 from emu import build_emu, driver
 from emu.driver import Guarded
 from emu.driver import ptr as _p
@@ -126,6 +127,33 @@ def test_time_baseline_bins_of_two_env_halves_pool_to_the_whole_batch(lib, A):
                     assert d.max() <= 1
 
 
+@pytest.mark.parametrize("W", (3, 4))
+@pytest.mark.parametrize("A", (1, 3))
+def test_time_baseline_bins_of_uneven_shards_pool_to_the_whole_batch(lib, W, A):
+    """Shards of one env (rank 0 never done, holding the largest index; rank 1 done on every step, its own L far
+    below the pooled L), bins over the pooled L summed in rank order: the whole batch's counts exactly, its sums at
+    1e-13, each shard's simplev within one float32 ulp of the fused call's rows, and the bins of the float64
+    reference of postproc_edges.time_index."""
+    sizes = se.TB_SIZES[W]
+    for L in (127, 129):
+        for with_t0 in (False, True):
+            q, done, t0 = se.tb_case(sizes, A, L, with_t0, 7 + L)
+            shards = [(np.ascontiguousarray(q[:, lo:hi]), np.ascontiguousarray(done[:, lo:hi]),
+                       None if t0 is None else t0[lo:hi].copy()) for lo, hi in se.bounds(sizes)]
+            for per_agent in (0, 1):
+                s, c, v = _fused(lib, q, done, t0, per_agent, L)
+                parts = [_bins(lib, qs, ds, ts, per_agent, L) for qs, ds, ts in shards]
+                ps, pc = parts[0][0].copy(), parts[0][1].copy()
+                for bs, bc in parts[1:]:                 # rank order, as dist.pool_sum adds them
+                    ps, pc = ps + bs, pc + bc
+                assert np.array_equal(pc, c)
+                np.testing.assert_allclose(ps, s, rtol=1e-13, atol=1e-13)
+                got = [_apply(lib, ds, ts, per_agent, A, L, ps, pc) for _, ds, ts in shards]
+                for g, (lo, hi) in zip(got, se.bounds(sizes)):
+                    assert se.ulps(g, v[:, lo:hi]) <= 1
+                pe.check_time_baseline(np.concatenate(got, axis=1), ps, pc, q, done, t0, per_agent)
+
+
 def _passes(lib, rows, A, a, b):
     """madrl_moments_pass_f32's two passes, the means formed between them as the pooled host code forms them."""
     st = Guarded((A, 9), np.float64, np.nan)
@@ -206,3 +234,42 @@ def test_split_entry_points_reject_bad_arguments(lib):
         bad[k] = None
         assert ta(*bad) != 0, k
     assert tb(2, 2, 1025, 1, 2, *good_b[5:]) != 0 and ta(2, 2, 1025, 1, 2, *good_a[5:]) != 0
+
+
+@pytest.mark.parametrize("W", (2, 3, 4))
+def test_moment_passes_over_shards_pool_to_the_union(lib, W):
+    """madrl_moments_pass_f32 over W shards at the emulator's grid-stride edges, pooled as postproc._pooled_moments
+    pools them (sums and rows added in rank order, minima by minimum, the second pass about the pooled means): the
+    float64 moments of the union; madrl_center_apply_f32 on each shard with the pooled statistics: NumPy's centring
+    and shift of the union within one float32 ulp."""
+    s = EMU_MOM_BLOCKS * 256
+    rows = {2: (s - 1, s + 1), 3: (s - 1, 1, s + 1), 4: (255, 1, 3 * s + 5, 256)}[W]
+    A = 3
+    parts = [se.moment_shard(n, A, r, 11) for r, n in enumerate(rows)]
+    st = [np.full((A, 9), np.nan) for _ in rows]
+    ws = np.empty((A, 4096))
+    for (x, y), n, t in zip(parts, rows, st):
+        assert lib.madrl_moments_pass_f32(n, A, _p(x), _p(y), 0, _p(t), _p(ws), None) == 0
+    sums, mins = sum(np.concatenate([t[:, 0:3], np.full((A, 1), float(n))], 1) for t, n in zip(st, rows)), st[0][:, 6:9]
+    for t in st[1:]:
+        mins = np.minimum(mins, t[:, 6:9])
+    pooled = np.full((A, 9), np.nan)
+    pooled[:, 0:3], pooled[:, 6:9] = sums[:, 0:3] / sums[:, 3:4], mins
+    sq = np.zeros((A, 3))
+    for (x, y), n, t in zip(parts, rows, st):
+        t[:, 0:3] = pooled[:, 0:3]
+        assert lib.madrl_moments_pass_f32(n, A, _p(x), _p(y), 1, _p(t), _p(ws), None) == 0
+        sq = sq + t[:, 3:6]
+    pooled[:, 3:6] = sq / sums[:, 3:4]
+    x, y = np.concatenate([p[0] for p in parts]), np.concatenate([p[1] for p in parts])
+    want = se.moments_of(x, y)
+    np.testing.assert_allclose(pooled, want, rtol=1e-10, atol=1e-12 * np.abs(want).max())
+    assert np.array_equal(pooled[:, 6:9], want[:, 6:9])
+    for center, positive in pe.CENTRE_MODES:
+        got = []
+        for (xs, _), n in zip(parts, rows):
+            g = Guarded(xs.shape, np.float32, xs)
+            assert lib.madrl_center_apply_f32(n, A, _p(g.arr), _p(pooled), center, positive, None) == 0
+            got.append(g.check("adv").copy())
+        want_c = np.stack([se.centred_want(x[:, a], center, positive) for a in range(A)], 1)
+        assert se.ulps(np.concatenate(got), want_c.astype(np.float32)) <= 1, (center, positive)

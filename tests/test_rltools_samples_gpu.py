@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 import torch
 
+import sharded_edges as se
 from oracle import rltools_oracle as ro
 
 pytestmark = pytest.mark.gpu
@@ -31,33 +32,7 @@ def _ulps(got, want):
 
 
 def _replay_device(settings, rollouts, mode, dtype):
-    from madrl_b200 import rltools_sampler as rs
-    pm = "decentralized" if mode == "zero" else mode
-    A, D = rollouts[0]["obs"].shape[2:]
-    dev = torch.device("cuda")
-    od = A * D if pm == "centralized" else D
-    bl = None if mode == "zero" else rs.LinearFeatureBaseline(od, dev, settings["obsnorm"],
-                                                              n_agents=A if pm == "concurrent" else None)
-    rewnorm = rs.RunningStandardizer(1, dev) if settings["rewnorm"] else None
-    for k, it in enumerate(rollouts):
-        obs = torch.from_numpy(it["obs"]).to(dev, dtype)
-        done = torch.from_numpy(it["done"]).to(dev)
-        rew = torch.from_numpy(it["rew_cent"] if pm == "centralized" else it["rew"]).to(dev)
-        ob = None if "obs_before" not in it else torch.from_numpy(it["obs_before"]).to(dev, dtype)
-        out = None
-        if k > 0:
-            out = rs.process_samples(bl, obs, done, rew, settings["discount"], settings["gae_lambda"], rewnorm, pm,
-                                     obs_before=ob)
-        elif bl is not None:
-            if pm == "centralized":
-                bl.update_obsnorm(obs.reshape(obs.shape[0], obs.shape[1], 1, -1),
-                                  None if ob is None else ob.reshape(ob.shape[0], 1, -1))
-            else:
-                bl.update_obsnorm(obs, ob)
-        if rewnorm is not None:
-            r = rew[..., :1] if pm == "centralized" else rew
-            (rewnorm.update_per_agent if pm == "concurrent" else rewnorm.update)(r.unsqueeze(-1))
-        yield k, out, bl, rewnorm
+    return se.replay_device(settings, rollouts, mode, dtype)
 
 
 @pytest.mark.parametrize("mode", MODES)
