@@ -221,8 +221,10 @@ __device__ __forceinline__ uint32_t wr_row_stage(uint32_t empty, uint32_t phase,
 // release the slot ("empty" mbarrier s).  The copy is one cp.async.bulk (evict-first), and a slot is released
 // once the next one's bulk store is issued and the slot's own has read its source.  Without kWrBulk it is
 // 16-byte shared loads and evict-first global stores instead: the generic proxy, so the env warps need no
-// proxy fence, but the writer issues two instructions per 16 bytes.  The <= 3 elements after the last
-// 16-byte boundary of a partial last group are stored one per lane.
+// proxy fence, but the writer issues two instructions per 16 bytes.  A group's run is always a whole number of
+// 16-byte units, so `tail` below never selects an element: the host's stride rule makes E*Np*D a multiple of 4, and
+// a partial last group's k envs satisfy k = E (mod kWrEnvs) with kWrEnvs a multiple of 4, so k*Np*D is one too.
+// (The one-per-lane tail stores stay, since removing them changes this kernel's SASS.)
 template <typename real, typename O>
 __device__ __forceinline__ void ww_obs_writer(const WWParams<real, O>& p, uint32_t bar, uint32_t ring, uint32_t slot_bytes,
                                               uint32_t env_bytes, int lane) {

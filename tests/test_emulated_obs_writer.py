@@ -10,7 +10,9 @@ warp's own staging (zero hazards), and the writer's reads of the ring are not re
 The emulator has two "SMs" and one resident block each, so with 8 env warps per block 20 envs make three groups:
 block 0 steps groups 0 and 2 (a partial one of 4 envs), one after the other through the same ring.  Also the
 launches that must fall back to the one-warp kernel (a step stride or observation base that is not 16-byte aligned)
-and the argument errors of set_obs_writer."""
+and the argument errors of set_obs_writer.  Every layout of tests/ww_writer_edges.py's case table runs the same way,
+and so do the ring geometries the build allows (MADRL_WW_WRITER_SLOTS, MADRL_WW_WRITER_ENVS), with either copy of a
+slot: a new geometry or layout passes here, where a missing arrival aborts the launch, before it runs on a GPU."""
 import numpy as np
 import pytest
 
@@ -19,6 +21,7 @@ from emu import driver
 from emu.driver import Guarded
 from emu.driver import ptr as _p
 from madrl_b200 import _lib as L
+from ww_writer_edges import BY_NAME, CASES, tail_events
 
 pytestmark = driver.needs_cxx
 
@@ -37,11 +40,11 @@ def no_shared_memory_hazards():
 WRITERS = {"bulk": (), "stores": ("-DMADRL_WW_WRITER_BULK=0",)}
 
 
-def engines(E, defines=()):
+def engines(E, defines=(), cfg=C2):
     from emu.driver import EmuWaterworld
     out = []
     for mode in (L.WW_OBS_WRITER_OFF, L.WW_OBS_WRITER_ON):
-        eng = EmuWaterworld(E, seed=17, env_id_base=2, fp64=False, max_path_length=MPL, defines=defines, **C2)
+        eng = EmuWaterworld(E, seed=17, env_id_base=2, fp64=False, max_path_length=MPL, defines=defines, **cfg)
         assert eng.lib.madrl_ww_set_obs_writer(eng._h, mode) == 0
         out.append(eng)
     return out
@@ -75,24 +78,62 @@ def compare(engs, act, **kw):
     return a
 
 
+def desync_sequence(engs, T1=13, T2=11, seed=8):
+    """From reset: a T1-step auto-reset rollout, a masked reset of every other env (so that paths end at other steps
+    than their neighbours'), a T2-step one, and 3 steps without auto-reset; the writer and the one-warp kernel must
+    agree on each -> the outputs of the three rollouts."""
+    E, Np = engs[0].n_envs, engs[0].n_agents
+    for eng in engs:
+        eng.reset()
+    rs = np.random.RandomState(seed)
+    act = rs.randn(T1, E, Np, 2).astype(np.float32)
+    first = compare(engs, act, term=True)
+    assert first[2].sum() >= E * (T1 // MPL)
+    mask = (np.arange(E) % 2).astype(np.uint8)
+    for eng in engs:
+        eng.reset(mask)
+    second = compare(engs, rs.randn(T2, E, Np, 2).astype(np.float32), term=True)
+    assert (second[2][:, :-1] != second[2][:, 1:]).any()
+    return first, second, compare(engs, act[:3], auto_reset=False)
+
+
 @pytest.mark.parametrize("writer", sorted(WRITERS))
 @pytest.mark.parametrize("E", [20, 19], ids=["aligned", "odd"])
 def test_writer_equals_one_warp_kernel(E, writer):
     """E = 20: 16-byte-aligned step stride (20 * 5 * 213 floats), three groups; E = 19: the launch falls back."""
-    engs = engines(E, WRITERS[writer])
-    for eng in engs:
-        eng.reset()
-    rs = np.random.RandomState(8)
-    act = rs.randn(13, E, 5, 2).astype(np.float32)
-    done = compare(engs, act, term=True)[2]
-    assert done.sum() >= E * (13 // MPL)
-    # desynchronise the envs: reset half of them, so that their paths end at other steps than their neighbours'
-    mask = (np.arange(E) % 2).astype(np.uint8)
-    for eng in engs:
-        eng.reset(mask)
-    done = compare(engs, rs.randn(11, E, 5, 2).astype(np.float32), term=True)[2]
-    assert (done[:, :-1] != done[:, 1:]).any()
-    compare(engs, act[:3], auto_reset=False)
+    desync_sequence(engines(E, WRITERS[writer]))
+
+
+def assert_events(runs, case):
+    """Catches and both kinds of collision (the rows' tail flags) happened."""
+    assert sum(int(r[3].sum()) for r in runs) > 0, "no catch"
+    assert min(sum(tail_events(r[0].view(np.float32), case)[i] for r in runs) for i in (0, 1)) > 0, "no collision"
+
+
+@pytest.mark.parametrize("case", CASES, ids=str)
+def test_case_table_writer_equals_one_warp_kernel(case):
+    """Each layout of the case table at E = 20 (three groups over the two SMs, the last a partial one of 4 envs) and
+    odd step counts; stage_over and obj33 fall back to the one-warp kernel."""
+    assert case.E(20) == 20
+    assert_events(desync_sequence(engines(20, cfg=case.cfg), T1=9, T2=7), case)
+
+
+# ring geometries of the build: MADRL_WW_WRITER_SLOTS steps in flight, MADRL_WW_WRITER_ENVS env warps per block
+GEOMETRIES = {"slots3": ("-DMADRL_WW_WRITER_SLOTS=3",), "envs4": ("-DMADRL_WW_WRITER_ENVS=4",),
+              "envs16": ("-DMADRL_WW_WRITER_ENVS=16",)}
+
+
+@pytest.mark.parametrize("writer", sorted(WRITERS))
+@pytest.mark.parametrize("geometry", sorted(GEOMETRIES))
+@pytest.mark.parametrize("name", ["c2", "k30_plain"])
+def test_ring_geometries(name, geometry, writer):
+    """Five groups over the two SMs, so that block 0 walks three through its ring.  The last group holds 4 envs for c2
+    (a full one with 4 env warps per block) and 2 for k30_plain, whose stride allows any E."""
+    case = BY_NAME[name]
+    envs = 16 if geometry == "envs16" else (4 if geometry == "envs4" else 8)
+    E = 4 * envs + (4 if name == "c2" else 2)
+    assert case.E(E) == E
+    desync_sequence(engines(E, GEOMETRIES[geometry] + WRITERS[writer], cfg=case.cfg), T1=9, T2=7)
 
 
 def test_misaligned_observation_base_falls_back():
