@@ -79,8 +79,10 @@ struct WWParams {
 
 // 0 <= sv < best for best > 0, in one comparison for float: non-negative floats order like their bit patterns
 // and every negative one has the sign bit set, i.e. compares above any positive `best` as an unsigned integer.
-// (-0.0 would be rejected where `sv < 0` is false, but sx * jx + sy * jy in round-to-nearest only yields -0.0
-// from two negative-zero terms, and neither a position difference nor a product with one can be -0.0 here.)
+// Unlike the reference's `sv < 0` test, the float form also rejects sv = -0.0.  sx * jx + sy * jy is -0.0 when
+// the candidate sits exactly at the pursuer's position (jx = jy = +0) and neither sensor component is positive,
+// which happens when pursuers are clipped into the same corner.  Only the OPL >= 2 candidate-slot path uses it;
+// the OPL == 1 walk tests `!(sv < 0)` and matches the reference there.
 __device__ __forceinline__ bool in_zero_to(float sv, float best) { return __float_as_uint(sv) < __float_as_uint(best); }
 __device__ __forceinline__ bool in_zero_to(double sv, double best) { return !(sv < 0.0) && sv < best; }
 
@@ -206,13 +208,12 @@ __device__ __forceinline__ void obs_row_store(uint32_t slot, O* row, int n, int 
   }
 }
 
-// WRITER: shared address of element 0 of `row` in this env warp's part of the step's ring slot (`rows`), after
-// waiting, at the step's first row, until the writer warp has released the slot (`empty`, completed phase
-// parity `phase ^ 1`: the copy of what the slot held S steps ago; the first S steps find the slot free).
-template <typename O>
-__device__ __forceinline__ uint32_t wr_row_stage(uint32_t empty, uint32_t phase, uint32_t rows, const O* obs_t, const O* row) {
-  if (row == obs_t) mbar_wait(empty, phase ^ 1u);
-  return rows + (uint32_t)((row - obs_t) * sizeof(O));
+// WRITER: shared address of pursuer pi's row, `row_off` bytes into this env warp's part of the step's ring slot
+// (`rows`), after waiting, at the step's first row, until the writer warp has released the slot (`empty`, completed
+// phase parity `phase ^ 1`: the copy of what the slot held S steps ago; the first S steps find the slot free).
+__device__ __forceinline__ uint32_t wr_row_stage(uint32_t empty, uint32_t phase, uint32_t rows, int pi, uint32_t row_off) {
+  if (pi == 0) mbar_wait(empty, phase ^ 1u);
+  return rows + row_off;
 }
 
 // The writer warp of a WRITER block: for every step of every env group of the block, wait until the group's
@@ -493,8 +494,10 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
           if (dx * dx + dy * dy <= thr) { vx[c] = kf * vx[c]; vy[c] = kf * vy[c]; }
         }
         // ---- sense: one pursuer at a time -----------------------------------------------------
+        // the pursuer's row: a global pointer (one-warp staging), or (WRITER) a 32-bit byte offset into the step's rows
         O* obs_row = obs_t;
-        for (int pi = 0; pi < p.Np; ++pi, obs_row += p.D) {
+        uint32_t row_off = 0u;
+        for (int pi = 0; pi < p.Np; ++pi, obs_row += p.D, row_off += (uint32_t)(p.D * sizeof(O))) {
           const real mx = __shfl_sync(FULL_MASK, x[0], pi), my = __shfl_sync(FULL_MASK, y[0], pi);
           const real mvx = __shfl_sync(FULL_MASK, vx[0], pi), mvy = __shfl_sync(FULL_MASK, vy[0], pi);
           // nearest sensed object per class and sensor chunk (ww:64-72, 312-334)
@@ -556,7 +559,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             MADRL_WW_SCAN(endE, endP, bP, aP)
 #undef MADRL_WW_SCAN
             uint32_t srow;
-            if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), obs_t, obs_row);
+            if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), pi, row_off);
             else srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
             for (int kc = 0; kc < KCH; ++kc) {
@@ -598,44 +601,53 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
             }
             __syncwarp();   // the next pursuer's staging overwrites the slots
           } else {
-#pragma unroll
-          for (int c = 0; c < OPL; ++c) {
-            // lanes as OBJECTS: geometry, collisions (ww:278-293), conservative range cull
-            const real rx = x[c] - mx, ry = y[c] - my;
+            // OPL == 1 (objects are lanes): lanes as OBJECTS -- geometry, collisions (ww:278-293), conservative
+            // range cull, and the velocity relative to pursuer pi, which the sensors shuffle for the speed features
+            const real rx = x[0] - mx, ry = y[0] - my;
             const real d2 = rx * rx + ry * ry;
-            unsigned cm = __ballot_sync(FULL_MASK, d2 <= cull2_l[c]);
-            if (c == 0) cm &= ~(1u << pi);  // ww:70-71 `same`
-            const bool hit = d2 <= coll2_l[c];
-            if (hit) col[c] |= 1u << pi;
-            if constexpr (POLICY) { const unsigned hm = __ballot_sync(FULL_MASK, hit); tE |= hm & mE[c]; tP |= hm & mP[c]; }
-            // lanes as SENSORS: scan the surviving candidates of this chunk, ascending index
+            const real rvx = vx[0] - mvx, rvy = vy[0] - mvy;
+            const unsigned cm = __ballot_sync(FULL_MASK, d2 <= cull2_l[0]) & ~(1u << pi);   // ww:70-71 `same`
+            const bool hit = d2 <= coll2_l[0];
+            if (hit) col[0] |= 1u << pi;
+            if constexpr (POLICY) { const unsigned hm = __ballot_sync(FULL_MASK, hit); tE |= hm & mE[0]; tP |= hm & mP[0]; }
+            // lanes as SENSORS: one walk over the candidates in ascending index.  Classes are contiguous in object
+            // index, so the (warp-uniform) index picks the class, and each class still sees its candidates in
+            // ascending order: with the strict `<`, the lowest index among equal minima wins (np.argmin).
+            const real up = p.range_up;   // `sv < up` <=> `sv <= range`; a best below `up` <=> sensed
 #pragma unroll
-            for (int kc = 0; kc < KCH; ++kc) {
-              const real sx = sx_l[kc], sy = sy_l[kc];
-#define MADRL_WW_SCAN(MASK, BEST, IDX)                                                  \
-  for (unsigned m = cm & (MASK); m != 0u; m &= m - 1u) {                                 \
-    const int j = __ffs(m) - 1;                                                          \
-    const real jx = __shfl_sync(FULL_MASK, rx, j), jy = __shfl_sync(FULL_MASK, ry, j);   \
-    const real jd = __shfl_sync(FULL_MASK, d2, j);                                       \
-    const real sv = sx * jx + sy * jy;                                                   \
-    const bool ok = !((sv < (real)0) | (sv > p.range) | (jd - sv * sv > p.r_p2));        \
-    if (ok && sv < BEST) { BEST = sv; IDX = j + 32 * c; }                                \
-  }
-              MADRL_WW_SCAN(mU[c], bU[kc], iU[kc])
-              MADRL_WW_SCAN(mE[c], bE[kc], iE[kc])
-              MADRL_WW_SCAN(mP[c], bP[kc], iP[kc])
-#undef MADRL_WW_SCAN
+            for (int kc = 0; kc < KCH; ++kc) bE[kc] = bP[kc] = bU[kc] = up;
+            for (unsigned m = cm; m != 0u; m &= m - 1u) {
+              const int j = __ffs(m) - 1;
+              const real jx = __shfl_sync(FULL_MASK, rx, j), jy = __shfl_sync(FULL_MASK, ry, j);
+              const real jd = __shfl_sync(FULL_MASK, d2, j);
+#pragma unroll
+              for (int kc = 0; kc < KCH; ++kc) {
+                const real sv = sx_l[kc] * jx + sy_l[kc] * jy;
+                // ww:64-72: 0 <= sv (<= range, through the initial best) and within the pursuer's radius of the ray.
+                // `!(sv < 0)` as in the reference, not in_zero_to: a candidate exactly at the pursuer's position
+                // (pursuers clipped into the same corner) gives sv = -0.0 for sensors with no positive component,
+                // and the reference senses it at distance 0.
+                const bool ok = !(sv < (real)0) & !(jd - sv * sv > p.r_p2);
+                // a uniform branch on the class, then selects (no divergent branch on the sensor's test)
+                auto take = [&](real& best, int& at) {
+                  const bool t = ok & (sv < best);
+                  best = t ? sv : best;
+                  at = t ? j : at;
+                };
+                if (j < eLo) take(bU[kc], iU[kc]);
+                else if (j < eHi) take(bE[kc], iE[kc]);
+                else take(bP[kc], iP[kc]);
+              }
             }
-          }
           uint32_t srow;
-          if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), obs_t, obs_row);
+          if constexpr (WRITER) srow = wr_row_stage(wr.empty(), wr.phase, wr.step_rows(), pi, row_off);
           else srow = obs_row_stage(p.stage_step != 0, stage, slot_off, obs_t, obs_row, lane);
 #pragma unroll
           for (int kc = 0; kc < KCH; ++kc) {
             const real sx = sx_l[kc], sy = sy_l[kc];
             // features ww:312-353, 388-395: feature-major, sensor-minor
             const int k = lane + 32 * kc;
-            const bool hO = bO[kc] < INF, hE = bE[kc] < INF, hP = bP[kc] < INF, hU = bU[kc] < INF;
+            const bool hO = bO[kc] < INF, hE = bE[kc] < up, hP = bP[kc] < up, hU = bU[kc] < up;
             const real z = (real)0;
             const uint32_t o = srow + (uint32_t)(k * sizeof(O));   // this lane's column
             constexpr uint32_t R = sizeof(O);
@@ -647,31 +659,18 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
               }
             }
             if (speed) {
-              real oEx, oEy, oPx, oPy, oUx, oUy;
-              if (OPL == 1) {
-                oEx = __shfl_sync(FULL_MASK, vx[0], iE[kc]); oEy = __shfl_sync(FULL_MASK, vy[0], iE[kc]);
-                oPx = __shfl_sync(FULL_MASK, vx[0], iP[kc]); oPy = __shfl_sync(FULL_MASK, vy[0], iP[kc]);
-                oUx = __shfl_sync(FULL_MASK, vx[0], iU[kc]); oUy = __shfl_sync(FULL_MASK, vy[0], iU[kc]);
-              } else {
-                oEx = oEy = oPx = oPy = oUx = oUy = z;
-#pragma unroll
-                for (int c = 0; c < OPL; ++c) {
-                  const real ex_ = __shfl_sync(FULL_MASK, vx[c], iE[kc] & 31), ey_ = __shfl_sync(FULL_MASK, vy[c], iE[kc] & 31);
-                  const real px_ = __shfl_sync(FULL_MASK, vx[c], iP[kc] & 31), py_ = __shfl_sync(FULL_MASK, vy[c], iP[kc] & 31);
-                  const real ux_ = __shfl_sync(FULL_MASK, vx[c], iU[kc] & 31), uy_ = __shfl_sync(FULL_MASK, vy[c], iU[kc] & 31);
-                  if ((iE[kc] >> 5) == c) { oEx = ex_; oEy = ey_; }
-                  if ((iP[kc] >> 5) == c) { oPx = px_; oPy = py_; }
-                  if ((iU[kc] >> 5) == c) { oUx = ux_; oUy = uy_; }
-                }
-              }
+              // the winners' velocities relative to pursuer pi (index 0 when nothing was sensed, masked below)
+              const real oEx = __shfl_sync(FULL_MASK, rvx, iE[kc]), oEy = __shfl_sync(FULL_MASK, rvy, iE[kc]);
+              const real oPx = __shfl_sync(FULL_MASK, rvx, iP[kc]), oPy = __shfl_sync(FULL_MASK, rvy, iP[kc]);
+              const real oUx = __shfl_sync(FULL_MASK, rvx, iU[kc]), oUy = __shfl_sync(FULL_MASK, rvy, iU[kc]);
               if (k < K) {
                 stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
                 stage_obs<O>(o + 1 * K * R, hE ? bE[kc] : z);
-                stage_obs<O>(o + 2 * K * R, hE ? sx * (oEx - mvx) + sy * (oEy - mvy) : z);
+                stage_obs<O>(o + 2 * K * R, hE ? sx * oEx + sy * oEy : z);
                 stage_obs<O>(o + 3 * K * R, hP ? bP[kc] : z);
-                stage_obs<O>(o + 4 * K * R, hP ? sx * (oPx - mvx) + sy * (oPy - mvy) : z);
+                stage_obs<O>(o + 4 * K * R, hP ? sx * oPx + sy * oPy : z);
                 stage_obs<O>(o + 5 * K * R, hU ? bU[kc] : z);
-                stage_obs<O>(o + 6 * K * R, hU ? sx * (oUx - mvx) + sy * (oUy - mvy) : z);
+                stage_obs<O>(o + 6 * K * R, hU ? sx * oUx + sy * oUy : z);
               }
             } else if (k < K) {
               stage_obs<O>(o + 0 * K * R, hO ? bO[kc] : z);
