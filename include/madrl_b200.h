@@ -559,6 +559,37 @@ int madrl_paths_pad_u16(int T, int E, int A, int D, int P, int Lmax, const void*
 int madrl_path_sums_f32(int T, int E, int A, int P, const float* rew_dev, const float* ret_dev,
                         const int32_t* rec_dev, double* sums_dev, double* first_ret_dev, void* stream);
 
+/* Whole-path sampling (rllab's BatchMASampler with whole_paths=True; DESIGN §4.9).  E lockstep envs, all reset at
+ * step 0, run in launches of T steps; global step g = t_base + t.  Per env, carry int32 [3][E] = (last done step,
+ * end step of the kept paths, paths kept), initialised to (-1, -1, 0); acc int64 [5] = (env-steps in finished
+ * paths, t*, finished flag, N rows kept, P paths kept), initialised to (0, -1, 0, 0, 0).
+ *   madrl_whole_paths_fold    folds one launch's done uint8 [T][E]: t* = the first step at which the env-steps of
+ *                             the paths finished so far reach batch_size; env e keeps steps [0, end_e], end_e = its
+ *                             first done at or after t*.  One CTA, no atomics.  finished = t* found and every end_e
+ *                             set; then N = sum (end_e + 1) and P = the done steps in the kept rows.
+ *   madrl_whole_paths_finish  after the fold has finished: env_off int32 [2][E] (first output row and first path of
+ *                             env e, env-major), path_start int32 [P+1] (first row of each path, then N) and done_flat uint8 [N] from
+ *                             the done columns of every launch, done_stage uint8 [S][E] (S >= max end_e + 1).
+ *   madrl_whole_paths_gather  one launch's per-(step, env) slabs src [T][E][slab_bytes] -> dst [N][slab_bytes],
+ *                             row env_off[e] + g for g <= end_e.  first != NULL: src is shifted by one step (step t
+ *                             reads src[t-1], step 0 first [E][slab_bytes]), as the policy reads its observations.
+ *                             16-byte vector copies when slab_bytes and the pointers allow them.
+ * MADRL_EINVAL for sizes < 1, batch_size < 1 or >= 2^62, or a NULL required buffer. */
+int madrl_whole_paths_fold(int T, int E, int t_base, size_t batch_size, const uint8_t* done_dev, int32_t* carry_dev,
+                           int64_t* acc_dev, void* stream);
+int madrl_whole_paths_finish(int E, int S, const uint8_t* done_stage_dev, const int32_t* carry_dev,
+                             int32_t* env_off_dev, int32_t* path_start_dev, uint8_t* done_flat_dev, void* stream);
+int madrl_whole_paths_gather(int T, int E, size_t slab_bytes, int t_base, const void* src_dev, const void* first_dev,
+                             const int32_t* carry_dev, const int32_t* env_off_dev, void* dst_dev, void* stream);
+/* The path plan of a flat batch of N rows cut at path_start int32 [P+1] (the rollout view T = N, E = 1):
+ * madrl_paths_plan's seg_start / seg_len [N], n_episodes [1] = P and ep_rec [N][3] (rows >= P untouched), one thread
+ * per row / path.  madrl_gae_paths_f32: madrl_gae_f32 over the same view ([N][A] tensors, every path terminated),
+ * one thread per (path, agent), bit for bit the serial walk's arithmetic. */
+int madrl_paths_plan_flat(int N, int P, const int32_t* path_start_dev, int32_t* seg_start_dev, int32_t* seg_len_dev,
+                          int32_t* n_episodes_dev, int32_t* ep_rec_dev, void* stream);
+int madrl_gae_paths_f32(int P, int A, const int32_t* path_start_dev, const float* rew_dev, const float* value_dev,
+                        double discount, double gae_lambda, float* adv_dev, float* ret_dev, void* stream);
+
 /* rllab's LinearFeatureBaseline (rllab/rllab/baselines/linear_feature_baseline.py), decentralized mode: one
  * baseline over every (t, e, a) row of a rollout.  Row (t, e, a) uses the observation the action of step t was
  * taken in (obs_before != NULL: obs_before [E][A][D] for t = 0, obs[t-1] afterwards; NULL: obs[t]) and the time

@@ -15,10 +15,11 @@ from .hostage import BatchedHostageWorld, ContinuousHostageWorld, CircAgent  # n
 from .closed_loop import PolicyRollout  # noqa: F401
 from .replay import ReplayPool  # noqa: F401
 from .evaluate import evaluate_heuristic, evaluate_policy  # noqa: F401
+from .whole_paths import WholePathBatch, WholePathSampler  # noqa: F401
 
 __all__ = [
     "EngineError", "launch_count", "Agent", "AbstractMAEnv", "EzPickle", "Box", "Discrete",
     "BatchedMAWaterWorld", "MAWaterWorld", "Archea", "BatchedPursuitEvade", "PursuitEvade",
     "DiscreteAgent", "BatchedHostageWorld", "ContinuousHostageWorld", "CircAgent", "PolicyRollout",
-    "ReplayPool", "evaluate_policy", "evaluate_heuristic",
+    "ReplayPool", "evaluate_policy", "evaluate_heuristic", "WholePathSampler", "WholePathBatch",
 ]

@@ -185,6 +185,12 @@ def _signatures():
         "madrl_paths_pad_u32": (i32, [i32] * 6 + [vp] * 5),
         "madrl_paths_pad_u16": (i32, [i32] * 6 + [vp] * 5),
         "madrl_path_sums_f32": (i32, [i32] * 4 + [vp] * 6),
+        # whole-path sampling and the flat batch's path-parallel passes
+        "madrl_whole_paths_fold": (i32, [i32] * 3 + [sz] + [vp] * 4),
+        "madrl_whole_paths_finish": (i32, [i32] * 2 + [vp] * 6),
+        "madrl_whole_paths_gather": (i32, [i32, i32, sz, i32] + [vp] * 6),
+        "madrl_paths_plan_flat": (i32, [i32] * 2 + [vp] * 6),
+        "madrl_gae_paths_f32": (i32, [i32] * 2 + [vp] * 3 + [f64, f64] + [vp] * 3),
         # rllab's linear feature baseline, pooled and per agent
         "madrl_lfb_workspace_size": (i32, [i32, P(sz)]),
         "madrl_lfb_normal_eq_f32": (i32, [i32] * 4 + [vp] * 8),

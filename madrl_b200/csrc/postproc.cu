@@ -669,6 +669,177 @@ __global__ void time_baseline_apply_kernel(int T, int E, int A, int G, int L, co
   simplev[r] = (idx >= 0 && idx < L) ? (float)(bin_sum[b] / (double)bin_cnt[b]) : __int_as_float(0x7fc00000);
 }
 
+
+// ---- whole-path sampling (rllab's BatchMASampler with whole_paths=True; DESIGN §4.9) ---------------------------
+// E lockstep envs stand in for rllab's workers.  After each step the paths that ended there add their env-steps to
+// one global count (once per env-step, as ma_sampler.py counts lengths[0]); t* is the first step at which the count
+// reaches batch_size, and env e keeps its steps [0, end_e], end_e its first done at or after t* (the paths finished
+// by t* and the one it was running at t*, run to its end).  One CTA folds each launch: thread j owns the envs
+// j, j + kWpThreads, ..., and a block reduction per step gives the step's count increment.  Integer sums, so the
+// result does not depend on the reduction order, and no atomics.
+constexpr int kWpThreads = 256;
+
+__device__ __forceinline__ int64_t block_sum_i64(int64_t v, int64_t* sh) {
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  __syncthreads();                               // the previous call's readers are done with sh
+  if (lane == 0) sh[w] = v;
+  __syncthreads();
+  int64_t t = 0;
+  for (int i = 0; i < kWpThreads / 32; ++i) t += sh[i];
+  return t;
+}
+
+// carry [3][E] = (last done step, end_e, paths kept); acc [5] = (count, t*, finished, N, P).
+__global__ void __launch_bounds__(kWpThreads) whole_paths_fold_kernel(int T, int E, int t_base, int64_t batch_size,
+                                                                      const uint8_t* __restrict__ done,
+                                                                      int32_t* __restrict__ carry,
+                                                                      int64_t* __restrict__ acc) {
+  __shared__ int64_t sh[kWpThreads / 32];
+  int32_t* last = carry;
+  int32_t* end = carry + E;
+  int32_t* npaths = carry + 2 * (size_t)E;
+  int64_t count = acc[0], tstar = acc[1];
+  if (acc[2]) return;
+  for (int t = 0; t < T; ++t) {
+    const int g = t_base + t;
+    const uint8_t* d = done + (size_t)t * E;
+    if (tstar < 0) {
+      int64_t add = 0;
+      for (int e = threadIdx.x; e < E; e += kWpThreads)
+        if (d[e]) { add += g - last[e]; last[e] = g; ++npaths[e]; }
+      count += block_sum_i64(add, sh);
+      if (count >= batch_size) {
+        tstar = g;
+        for (int e = threadIdx.x; e < E; e += kWpThreads)
+          if (d[e]) end[e] = g;
+      }
+    } else {
+      for (int e = threadIdx.x; e < E; e += kWpThreads)
+        if (end[e] < 0 && d[e]) { end[e] = g; last[e] = g; ++npaths[e]; }
+    }
+  }
+  // finished once t* is known and every env has ended its kept paths
+  int64_t open = 0, n = 0, p = 0;
+  for (int e = threadIdx.x; e < E; e += kWpThreads) {
+    open += end[e] < 0;
+    n += end[e] + 1;
+    p += npaths[e];
+  }
+  open = block_sum_i64(open, sh);
+  n = block_sum_i64(n, sh);
+  p = block_sum_i64(p, sh);
+  if (threadIdx.x == 0) {
+    const bool fin = tstar >= 0 && open == 0;
+    acc[0] = count; acc[1] = tstar; acc[2] = fin;
+    acc[3] = fin ? n : 0; acc[4] = fin ? p : 0;
+  }
+}
+
+// env_off[e] = sum over e' < e of (end_e' + 1), path_off[e] = sum of npaths: one CTA, each thread sums a contiguous
+// run of envs, the run totals are scanned in thread order.
+__global__ void __launch_bounds__(kWpThreads) whole_paths_scan_kernel(int E, const int32_t* __restrict__ carry,
+                                                                      int32_t* __restrict__ env_off,
+                                                                      int32_t* __restrict__ path_off) {
+  __shared__ int64_t sh[2][kWpThreads];
+  const int32_t* end = carry + E;
+  const int32_t* npaths = carry + 2 * (size_t)E;
+  const int per = (E + kWpThreads - 1) / kWpThreads;
+  const int e0 = min(E, (int)threadIdx.x * per), e1 = min(E, e0 + per);
+  int64_t n = 0, p = 0;
+  for (int e = e0; e < e1; ++e) { n += end[e] + 1; p += npaths[e]; }
+  sh[0][threadIdx.x] = n;
+  sh[1][threadIdx.x] = p;
+  __syncthreads();
+  n = p = 0;
+  for (int i = 0; i < (int)threadIdx.x; ++i) { n += sh[0][i]; p += sh[1][i]; }
+  for (int e = e0; e < e1; ++e) {
+    env_off[e] = (int32_t)n;
+    path_off[e] = (int32_t)p;
+    n += end[e] + 1;
+    p += npaths[e];
+  }
+}
+
+// One thread per env walks its kept done column: done_flat of its rows and path_start of its paths.
+__global__ void whole_paths_rows_kernel(int E, const uint8_t* __restrict__ done_stage,
+                                        const int32_t* __restrict__ carry, const int32_t* __restrict__ env_off,
+                                        const int32_t* __restrict__ path_off, int32_t* __restrict__ path_start,
+                                        uint8_t* __restrict__ done_flat) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= E) return;
+  if (e == 0) path_start[0] = 0;
+  const int end = carry[E + e], off = env_off[e];
+  int j = path_off[e];
+  for (int t = 0; t <= end; ++t) {
+    const uint8_t d = done_stage[(size_t)t * E + e] ? 1 : 0;
+    done_flat[off + t] = d;
+    if (d) path_start[++j] = off + t + 1;
+  }
+}
+
+// Slab (t, e) of one launch -> row env_off[e] + t_base + t of the flat output, for the kept steps.  V = the copy
+// word (float4, moved as bits, where the slab and the pointers are 16-byte aligned); kLanes = 32 (a warp per slab) or 1 (a thread
+// per slab of at most 4 words).
+template <int kLanes, typename V>
+__global__ void whole_paths_gather_kernel(int T, int E, int W, int t_base, const V* __restrict__ src,
+                                          const V* __restrict__ first, const int32_t* __restrict__ carry,
+                                          const int32_t* __restrict__ env_off, V* __restrict__ dst) {
+  const size_t slab = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) / kLanes;   // (t, e)
+  if (slab >= (size_t)T * E) return;
+  const int t = (int)(slab / E), e = (int)(slab - (size_t)t * E), g = t_base + t;
+  if (g > carry[E + e]) return;
+  const V* in = action_obs_row(slab, (size_t)E, W, src, first);
+  V* out = dst + ((size_t)env_off[e] + g) * W;
+  if (kLanes == 1) {
+    for (int w = 0; w < W; ++w) out[w] = in[w];
+  } else {
+    for (int w = threadIdx.x % kLanes; w < W; w += kLanes) __stcs(out + w, __ldcs(in + w));
+  }
+}
+
+// The flat batch's path plan: seg_start / seg_len per row by a binary search of path_start, ep_rec per path.
+__global__ void paths_plan_flat_kernel(int N, int P, const int32_t* __restrict__ path_start,
+                                       int32_t* __restrict__ seg_start, int32_t* __restrict__ seg_len,
+                                       int32_t* __restrict__ n_episodes, int32_t* __restrict__ ep_rec) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < N) {
+    int lo = 0, hi = P - 1;                        // the last path whose start is <= i
+    while (lo < hi) {
+      const int mid = (lo + hi + 1) >> 1;
+      if (path_start[mid] <= i) lo = mid; else hi = mid - 1;
+    }
+    seg_start[i] = path_start[lo];
+    seg_len[i] = path_start[lo + 1] - path_start[lo];
+  }
+  if (i < P) {
+    int32_t* r = ep_rec + 3 * (size_t)i;
+    r[0] = path_start[i]; r[1] = path_start[i + 1] - path_start[i]; r[2] = 1;
+  }
+  if (i == 0) n_episodes[0] = P;
+}
+
+// gae_kernel's walk over one path of one agent column: the same operations in the same order, so the same bits.
+__global__ void gae_paths_kernel(int P, int A, const int32_t* __restrict__ path_start, const float* __restrict__ rew,
+                                 const float* __restrict__ val, double discount, double gae_lambda,
+                                 float* __restrict__ adv, float* __restrict__ ret) {
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)P * A) return;
+  const int p = (int)(i / A), a = (int)(i - (size_t)p * A);
+  double next_v = 0.0, run_adv = 0.0, run_ret = 0.0;
+  const double gl = discount * gae_lambda;
+  for (int t = path_start[p + 1] - 1; t >= path_start[p]; --t) {
+    const size_t k = (size_t)t * A + a;
+    const double r = (double)rew[k], v = (double)val[k];
+    const double delta = r + discount * next_v - v;                // base.py:58-60
+    run_adv = delta + gl * run_adv;                                // base.py:61-62
+    run_ret = r + discount * run_ret;                              // base.py:63
+    __stcs(adv + k, (float)run_adv);
+    __stcs(ret + k, (float)run_ret);
+    next_v = v;
+  }
+}
+
 }  // namespace madrl
 
 using namespace madrl;
@@ -1130,6 +1301,85 @@ extern "C" int madrl_time_baseline_apply_f32(int T, int E, int A, int per_agent,
   const size_t rows = (size_t)T * E * A;
   MADRL_LAUNCH(time_baseline_apply_kernel, (unsigned)((rows + 255) / 256), 256, 0, (cudaStream_t)stream, T, E, A,
                per_agent ? A : 1, L, seg_start_dev, t0_dev, bin_sum_dev, bin_count_dev, simplev_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_whole_paths_fold(int T, int E, int t_base, size_t batch_size, const uint8_t* done_dev,
+                                      int32_t* carry_dev, int64_t* acc_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && t_base >= 0, "bad sizes");
+  MADRL_REQUIRE(batch_size >= 1 && batch_size < ((size_t)1 << 62), "batch_size must be in [1, 2^62)");
+  MADRL_REQUIRE(done_dev && carry_dev && acc_dev, "NULL buffer");
+  MADRL_LAUNCH(whole_paths_fold_kernel, 1, kWpThreads, 0, (cudaStream_t)stream, T, E, t_base, (int64_t)batch_size,
+               done_dev, carry_dev, acc_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_whole_paths_finish(int E, int S, const uint8_t* done_stage_dev, const int32_t* carry_dev,
+                                        int32_t* env_off_dev, int32_t* path_start_dev, uint8_t* done_flat_dev,
+                                        void* stream) {
+  MADRL_REQUIRE(E >= 1 && S >= 1, "bad sizes");
+  MADRL_REQUIRE(done_stage_dev && carry_dev && env_off_dev && path_start_dev && done_flat_dev, "NULL buffer");
+  cudaStream_t s = (cudaStream_t)stream;
+  // the scan's path offsets go to the third carry row's copy in env_off_dev + E
+  MADRL_LAUNCH(whole_paths_scan_kernel, 1, kWpThreads, 0, s, E, carry_dev, env_off_dev, env_off_dev + E);
+  MADRL_LAUNCH(whole_paths_rows_kernel, (unsigned)((E + 127) / 128), 128, 0, s, E, done_stage_dev, carry_dev,
+               env_off_dev, env_off_dev + E, path_start_dev, done_flat_dev);
+  g_launches.fetch_add(2);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+template <typename V>
+static int whole_paths_gather(int T, int E, int W, int t_base, const void* src, const void* first,
+                              const int32_t* carry, const int32_t* env_off, void* dst, void* stream) {
+  return launch_rows(whole_paths_gather_kernel<1, V>, whole_paths_gather_kernel<32, V>, (size_t)T * E, W, stream, T,
+                     E, W, t_base, (const V*)src, (const V*)first, carry, env_off, (V*)dst);
+}
+
+extern "C" int madrl_whole_paths_gather(int T, int E, size_t slab_bytes, int t_base, const void* src_dev,
+                                        const void* first_dev, const int32_t* carry_dev, const int32_t* env_off_dev,
+                                        void* dst_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && slab_bytes >= 1 && t_base >= 0, "bad sizes");
+  MADRL_REQUIRE(src_dev && carry_dev && env_off_dev && dst_dev, "NULL buffer");
+  uintptr_t bits = (uintptr_t)slab_bytes | (uintptr_t)src_dev | (uintptr_t)dst_dev | (uintptr_t)first_dev;
+  MADRL_REQUIRE(slab_bytes / 16 < ((size_t)1 << 31), "slab too wide");
+  if (bits % 16 == 0)
+    return whole_paths_gather<float4>(T, E, (int)(slab_bytes / 16), t_base, src_dev, first_dev, carry_dev,
+                                      env_off_dev, dst_dev, stream);
+  if (bits % 4 == 0)
+    return whole_paths_gather<uint32_t>(T, E, (int)(slab_bytes / 4), t_base, src_dev, first_dev, carry_dev,
+                                        env_off_dev, dst_dev, stream);
+  if (bits % 2 == 0)
+    return whole_paths_gather<uint16_t>(T, E, (int)(slab_bytes / 2), t_base, src_dev, first_dev, carry_dev,
+                                        env_off_dev, dst_dev, stream);
+  return whole_paths_gather<uint8_t>(T, E, (int)slab_bytes, t_base, src_dev, first_dev, carry_dev, env_off_dev,
+                                     dst_dev, stream);
+}
+
+extern "C" int madrl_paths_plan_flat(int N, int P, const int32_t* path_start_dev, int32_t* seg_start_dev,
+                                     int32_t* seg_len_dev, int32_t* n_episodes_dev, int32_t* ep_rec_dev,
+                                     void* stream) {
+  MADRL_REQUIRE(N >= 1 && P >= 1 && P <= N, "bad sizes");
+  MADRL_REQUIRE(path_start_dev && seg_start_dev && seg_len_dev && n_episodes_dev && ep_rec_dev, "NULL pointer");
+  MADRL_LAUNCH(paths_plan_flat_kernel, (unsigned)((N + 255) / 256), 256, 0, (cudaStream_t)stream, N, P,
+               path_start_dev, seg_start_dev, seg_len_dev, n_episodes_dev, ep_rec_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_gae_paths_f32(int P, int A, const int32_t* path_start_dev, const float* rew_dev,
+                                   const float* value_dev, double discount, double gae_lambda, float* adv_dev,
+                                   float* ret_dev, void* stream) {
+  MADRL_REQUIRE(P >= 1 && A >= 1, "bad sizes");
+  MADRL_REQUIRE(path_start_dev && rew_dev && value_dev && adv_dev && ret_dev, "NULL buffer");
+  const size_t n = (size_t)P * A;
+  MADRL_LAUNCH(gae_paths_kernel, (unsigned)((n + 127) / 128), 128, 0, (cudaStream_t)stream, P, A, path_start_dev,
+               rew_dev, value_dev, discount, gae_lambda, adv_dev, ret_dev);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;

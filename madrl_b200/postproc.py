@@ -43,6 +43,10 @@ def _paths_plan(done, A):
     uint8 on its CUDA device, enqueued without a host synchronisation.  Returns int32 seg_s, seg_l [T,E] (start and
     length of the path holding each step), n_ep [E] (paths per env) and ep_rec [E,T,3] (per path of each env: start,
     length, terminated; zero past the env's last path)."""
+    from .whole_paths import whole_paths_of
+    wp = whole_paths_of(done)
+    if wp is not None:     # a WholePathBatch's [N, 1] view: the plan built from its path table, one thread per row
+        return wp.plan()
     T, E = done.shape
     dev = done.device
     seg_s = torch.empty((T, E), dtype=torch.int32, device=dev)
@@ -63,7 +67,9 @@ def gae(rew, values, done, discount, gae_lambda, last_value=None):
     """rew, values [T,E,A] float32 cuda; done [T,E] uint8 -> (advantages, returns) [T,E,A].
 
     Paths end where ``done`` is set (bootstrap 0, base.py:57) and at the end of the rollout
-    (bootstrap ``last_value`` [E,A] if given, else 0)."""
+    (bootstrap ``last_value`` [E,A] if given, else 0).  On the ``done`` of ``WholePathBatch.as_rollout()`` one thread
+    per (path, agent) walks the batch's paths (every one ends at ``done``, so ``last_value`` is unused, as in the
+    serial walk), with the serial walk's arithmetic."""
     T, E, A = _lib.require_tensor(rew, "rew", torch.float32, (None, None, None), None, contiguous=False).shape
     dev = rew.device
     _lib.require_tensor(values, "values", torch.float32, (T, E, A), dev, contiguous=False)
@@ -73,6 +79,14 @@ def gae(rew, values, done, discount, gae_lambda, last_value=None):
     rew, values, done = rew.contiguous(), values.contiguous(), done.contiguous()
     adv, ret = torch.empty_like(rew), torch.empty_like(rew)
     lv = last_value.contiguous() if last_value is not None else None
+    from .whole_paths import whole_paths_of
+    wp = whole_paths_of(done)
+    if wp is not None:
+        with torch.cuda.device(dev):
+            _lib.check(_lib.lib().madrl_gae_paths_f32(wp.n_paths, A, _ptr(wp.path_start), _ptr(rew), _ptr(values),
+                                                      float(discount), float(gae_lambda), _ptr(adv), _ptr(ret),
+                                                      _lib.stream(dev)))
+        return adv, ret
     with torch.cuda.device(dev):
         _lib.check(_lib.lib().madrl_gae_f32(T, E, A, _ptr(rew), _ptr(values), _ptr(done), _ptr(lv),
                                             float(discount), float(gae_lambda), _ptr(adv), _ptr(ret),
