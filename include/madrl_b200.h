@@ -479,39 +479,29 @@ int madrl_eval_episodes_f64(int T, int E, int A, int C, const double* rew_dev, c
                             const int32_t* info_dev, double discount, int K, void* carry_dev, double* ret_dev,
                             double* qsum_dev, int32_t* len_dev, int64_t* info_sum_dev, void* stream);
 
-/* Whole-batch moments, deterministic (fixed grid, fixed combination order), float64 accumulation,
- * NumPy's two-pass population variance.  Series s0 = a, s1 = b, s2 = b - a (b may be NULL):
- * stats[0..2] = means, stats[3..5] = variances, stats[6..8] = minima (MADRL_MOMENTS_STATS doubles).
- * workspace: MADRL_MOMENTS_WS doubles of device scratch.  With a = baseline prediction and
- * b = returns this gives explained_variance_1d's terms (rllab/rllab/misc/special.py:51-59):
- * var(y) = stats[4], var(y - ypred) = stats[5], var(ypred) = stats[3]. */
+/* Per-column moments, deterministic (fixed grid, fixed combination order), float64 accumulation, NumPy's two-pass
+ * population variance.  a, b are [rows][A] (A = the innermost axis, e.g. a [T][E][A] tensor with rows = T*E; the
+ * whole batch is A = 1) and every statistic is taken over one column, i.e. one agent's samples.  Series s0 = a,
+ * s1 = b, s2 = b - a (b may be NULL).  stats [A][MADRL_MOMENTS_STATS]: column c's block holds the means at [0..2],
+ * the population variances at [3..5] and the minima at [6..8]; workspace: MADRL_MOMENTS_WS * A doubles of device
+ * scratch.  With a = baseline prediction and b = returns the block gives explained_variance_1d's terms
+ * (rllab/rllab/misc/special.py:51-59): var(y) = [4], var(y - ypred) = [5], var(ypred) = [3].
+ *
+ * madrl_moments_pass_f32 runs one of the two passes and leaves the division by the rows to the caller, so that
+ * the statistics of the shards of a batch can be pooled between the passes: pass 0 writes the SUMS of the three
+ * series to stats[.][0..2] and their minima to stats[.][6..8]; pass 1 reads the means from stats[.][0..2] and
+ * writes the SUMS of squared deviations about them to stats[.][3..5].  Dividing pass 0's sums by the rows before
+ * pass 1, and pass 1's sums by the rows after it, gives the block above.
+ *
+ * madrl_center_apply_f32: center_advantages / shift_advantages_to_positive (rllab/rllab/algos/util.py:7-12,
+ * applied to the concatenated advantages at rllab/rllab/sampler/base.py:82-86), in place over adv [rows][A] with
+ * column a's statistics from stats [A][MADRL_MOMENTS_STATS] (mean [0], variance [3], minimum [6]):
+ * center: (x - mean) / (std + 1e-8); positive: (x - min) + 1e-8 (after centring when both).
+ *
+ * MADRL_EINVAL for A outside [1, MADRL_AGENTS_MAX] (declared below), rows == 0, a pass other than 0 and 1, or a
+ * NULL required buffer. */
 #define MADRL_MOMENTS_STATS 9
 #define MADRL_MOMENTS_WS 4096
-int madrl_moments_f32(size_t n, const float* a_dev, const float* b_dev, double* stats_dev,
-                      double* workspace_dev, void* stream);
-/* center_advantages / shift_advantages_to_positive (rllab/rllab/algos/util.py:7-12, applied to the
- * concatenated advantages at rllab/rllab/sampler/base.py:82-86), in place over adv [n]:
- * center: (x - mean) / (std + 1e-8); positive: (x - min) + 1e-8 (after centring when both).
- * stats_dev receives the moments of the INPUT as in madrl_moments_f32 (series 0). */
-int madrl_center_advantages_f32(size_t n, float* adv_dev, int center, int positive, double* stats_dev,
-                                double* workspace_dev, void* stream);
-/* Per-agent (column) versions for concurrent mode: a, b, adv are [rows][A] (A = the innermost axis, e.g. a
- * [T][E][A] tensor with rows = T*E) and every statistic is taken over one column, i.e. one agent's samples:
- * stats [A][MADRL_MOMENTS_STATS] (agent a's block laid out as above), workspace MADRL_MOMENTS_WS * A doubles.
- * Centring / shifting applies agent a's statistics to column a.  Same arithmetic and combination order per
- * column as the whole-batch passes, so A = 1 gives their bits.  MADRL_EINVAL for A outside
- * [1, MADRL_AGENTS_MAX] (declared below), rows == 0 or a NULL required buffer. */
-int madrl_moments_agents_f32(size_t rows, int A, const float* a_dev, const float* b_dev, double* stats_dev,
-                             double* workspace_dev, void* stream);
-int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
-                                       double* stats_dev, double* workspace_dev, void* stream);
-/* The two passes of madrl_moments_agents_f32 one at a time, for statistics pooled over the shards of a batch
- * (the same kernels, grid and combination order; A = 1 is the whole batch).  pass 0 writes the SUMS of the three
- * series to stats[.][0..2] and their minima to stats[.][6..8]; pass 1 reads means from stats[.][0..2] and writes
- * the SUMS of squared deviations about them to stats[.][3..5].  Dividing by the rows gives madrl_moments_*'s
- * bits.  madrl_center_apply_f32: the centring / shifting of madrl_center_advantages_* with the given stats
- * [A][MADRL_MOMENTS_STATS] (mean [0], variance [3], minimum [6]).  MADRL_EINVAL as madrl_moments_agents_f32, or
- * for a pass other than 0 and 1. */
 int madrl_moments_pass_f32(size_t rows, int A, const float* a_dev, const float* b_dev, int pass, double* stats_dev,
                            double* workspace_dev, void* stream);
 int madrl_center_apply_f32(size_t rows, int A, float* adv_dev, const double* stats_dev, int center, int positive,
@@ -648,26 +638,22 @@ int madrl_lfb_predict_agents_bf16(int T, int E, int A, int D, const void* obs_de
  *                            (the observation an action was taken in; shift = E*A).  ws:
  *                            madrl_running_moments_workspace_size bytes.  MADRL_EINVAL for R, D < 1, G outside
  *                            [1, MADRL_AGENTS_MAX], a shift outside [1, R*G] with first, or a NULL required buffer.
- *   madrl_time_baseline_f32  q float32 [T][E][A] -> bin_sum float64 [G][L], bin_count int32 [G][L] (G = A with
- *                            per_agent, else 1 over every agent's rows): the sum of q and the number of rows whose
- *                            time index (as madrl_lfb_*: t - seg_start, plus t0[e] on env e's first path) is i;
- *                            simplev float32 [T][E][A] = sum / count of the row's bin (NaN for an index >= L).
- *                            seg_start, n_ep, ep_rec: madrl_paths_plan's outputs.  Deterministic, no atomics.  ws:
- *                            madrl_time_baseline_workspace_size(G, L) bytes.  MADRL_EINVAL for sizes below 1,
- *                            T*E*A >= 2^31, per_agent with A > MADRL_AGENTS_MAX or a NULL required buffer. */
+ *   madrl_time_baseline_bins_f32   q float32 [T][E][A] -> bin_sum float64 [G][L], bin_count int32 [G][L] (G = A
+ *                            with per_agent, else 1 over every agent's rows): the sum of q and the number of rows
+ *                            whose time index (as madrl_lfb_*: t - seg_start, plus t0[e] on env e's first path) is
+ *                            i.  n_ep, ep_rec: madrl_paths_plan's outputs.  ws:
+ *                            madrl_time_baseline_workspace_size(G, L) bytes.
+ *   madrl_time_baseline_apply_f32  simplev float32 [T][E][A] = sum / count of the row's bin in the bins it is given
+ *                            (NaN for an index >= L); seg_start: madrl_paths_plan's.  The bins of the shards of a
+ *                            batch may be summed between the two calls.
+ *                            Both deterministic, no atomics.  MADRL_EINVAL for sizes below 1, T*E*A >= 2^31,
+ *                            per_agent with A > MADRL_AGENTS_MAX or a NULL required buffer. */
 int madrl_running_moments_workspace_size(int G, int D, size_t* bytes);
 int madrl_running_moments_f32(size_t R, int G, int D, size_t shift, const float* x_dev, const float* first_dev,
                               double* sums_dev, double* ws_dev, void* stream);
 int madrl_running_moments_bf16(size_t R, int G, int D, size_t shift, const void* x_dev, const void* first_dev,
                                double* sums_dev, double* ws_dev, void* stream);
 int madrl_time_baseline_workspace_size(int G, int L, size_t* bytes);
-int madrl_time_baseline_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
-                            const int32_t* seg_start_dev, const int32_t* n_ep_dev, const int32_t* ep_rec_dev,
-                            const int32_t* t0_dev, double* bin_sum_dev, int32_t* bin_count_dev, float* simplev_dev,
-                            void* ws_dev, void* stream);
-/* madrl_time_baseline_f32 in two calls, so that the bins of the shards of a batch can be summed in between:
- * _bins writes bin_sum / bin_count (ws as for madrl_time_baseline_f32), _apply writes simplev from the bins it is
- * given.  Same kernels; _bins then _apply on the same arguments give madrl_time_baseline_f32's bits. */
 int madrl_time_baseline_bins_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
                                  const int32_t* n_ep_dev, const int32_t* ep_rec_dev, const int32_t* t0_dev,
                                  double* bin_sum_dev, int32_t* bin_count_dev, void* ws_dev, void* stream);

@@ -172,10 +172,6 @@ def _signatures():
         "madrl_eval_episodes_f32": (i32, [i32] * 4 + [vp] * 3 + [f64, i32] + [vp] * 6),
         "madrl_eval_episodes_f64": (i32, [i32] * 4 + [vp] * 3 + [f64, i32] + [vp] * 6),
         # moments and advantage centring
-        "madrl_moments_f32": (i32, [sz, vp, vp, vp, vp, vp]),
-        "madrl_center_advantages_f32": (i32, [sz, vp, i32, i32, vp, vp, vp]),
-        "madrl_moments_agents_f32": (i32, [sz, i32, vp, vp, vp, vp, vp]),
-        "madrl_center_advantages_agents_f32": (i32, [sz, i32, vp, i32, i32, vp, vp, vp]),
         "madrl_moments_pass_f32": (i32, [sz, i32, vp, vp, i32, vp, vp, vp]),
         "madrl_center_apply_f32": (i32, [sz, i32, vp, vp, i32, i32, vp]),
         # path packing and padding
@@ -207,7 +203,6 @@ def _signatures():
         "madrl_running_moments_f32": (i32, [sz, i32, i32, sz] + [vp] * 5),
         "madrl_running_moments_bf16": (i32, [sz, i32, i32, sz] + [vp] * 5),
         "madrl_time_baseline_workspace_size": (i32, [i32, i32, P(sz)]),
-        "madrl_time_baseline_f32": (i32, [i32] * 5 + [vp] * 10),
         "madrl_time_baseline_bins_f32": (i32, [i32] * 5 + [vp] * 8),
         "madrl_time_baseline_apply_f32": (i32, [i32] * 5 + [vp] * 6),
         # rltools' linear feature baseline

@@ -958,68 +958,9 @@ extern "C" int madrl_standardize_bf16(int T, size_t n, void* x_dev, double* mean
   return standardize(T, n, (uint16_t*)x_dev, mean_dev, var_dev, alpha, eps, center, scale, enable, stream);
 }
 
-// The A columns of [n][A]; the whole batch of n elements is A = 1.
-static int run_moments(size_t n, int A, const float* a, const float* b, double* stats, double* ws, cudaStream_t s) {
-  const unsigned grid = (unsigned)(kMomBlocks * A);
-  MADRL_LAUNCH(moments_partial_kernel, grid, kMomThreads, 0, s, n, A, a, b, nullptr, ws);
-  MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 0, stats);
-  MADRL_LAUNCH(moments_partial_kernel, grid, kMomThreads, 0, s, n, A, a, b, stats, ws);
-  MADRL_LAUNCH(moments_finalize_kernel, (unsigned)A, 32, 0, s, n, ws, 1, stats);
-  g_launches.fetch_add(4);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
-}
-
-extern "C" int madrl_center_advantages_f32(size_t n, float* adv_dev, int center, int positive,
-                                           double* stats_dev, double* workspace_dev, void* stream) {
-  MADRL_REQUIRE(n >= 1, "bad sizes");
-  MADRL_REQUIRE(adv_dev && stats_dev && workspace_dev, "NULL buffer");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int rc = run_moments(n, 1, adv_dev, nullptr, stats_dev, workspace_dev, s);
-  if (rc) return rc;
-  if (center || positive) {
-    MADRL_LAUNCH(center_apply_kernel, kMomBlocks, kMomThreads, 0, s, n, adv_dev, stats_dev, center, positive);
-    g_launches.fetch_add(1);
-    MADRL_CUDA_CHECK(cudaGetLastError());
-  }
-  return MADRL_OK;
-}
-
-extern "C" int madrl_moments_f32(size_t n, const float* a_dev, const float* b_dev, double* stats_dev,
-                                 double* workspace_dev, void* stream) {
-  MADRL_REQUIRE(n >= 1, "bad sizes");
-  MADRL_REQUIRE(a_dev && stats_dev && workspace_dev, "NULL buffer");
-  return run_moments(n, 1, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
-}
-
-extern "C" int madrl_center_advantages_agents_f32(size_t rows, int A, float* adv_dev, int center, int positive,
-                                                  double* stats_dev, double* workspace_dev, void* stream) {
-  MADRL_REQUIRE(rows >= 1, "bad sizes");
-  MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
-  MADRL_REQUIRE(adv_dev && stats_dev && workspace_dev, "NULL buffer");
-  cudaStream_t s = (cudaStream_t)stream;
-  const int rc = run_moments(rows, A, adv_dev, nullptr, stats_dev, workspace_dev, s);
-  if (rc) return rc;
-  if (center || positive) {
-    MADRL_LAUNCH(center_apply_agents_kernel, kMomBlocks, kMomThreads, 0, s, rows, A, adv_dev, stats_dev, center,
-                 positive);
-    g_launches.fetch_add(1);
-    MADRL_CUDA_CHECK(cudaGetLastError());
-  }
-  return MADRL_OK;
-}
-
-extern "C" int madrl_moments_agents_f32(size_t rows, int A, const float* a_dev, const float* b_dev,
-                                        double* stats_dev, double* workspace_dev, void* stream) {
-  MADRL_REQUIRE(rows >= 1, "bad sizes");
-  MADRL_REQUIRE(A >= 1 && A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
-  MADRL_REQUIRE(a_dev && stats_dev && workspace_dev, "NULL buffer");
-  return run_moments(rows, A, a_dev, b_dev, stats_dev, workspace_dev, (cudaStream_t)stream);
-}
-
-// One pass of run_moments with its finalize dividing by 1, so the statistics of several shards can be pooled
-// between the passes: pass 0 leaves the sums (not the means), pass 1 the sums of squared deviations about the
-// means the caller wrote to stats[.][0..2] (not the variances).  Same kernels, grid and combination order.
+// One of the two moments passes over the A columns of [rows][A], its finalize dividing by 1, so that the statistics
+// of several shards can be pooled between the passes: pass 0 leaves the sums (not the means), pass 1 the sums of
+// squared deviations about the means the caller wrote to stats[.][0..2] (not the variances).
 extern "C" int madrl_moments_pass_f32(size_t rows, int A, const float* a_dev, const float* b_dev, int pass,
                                       double* stats_dev, double* workspace_dev, void* stream) {
   MADRL_REQUIRE(rows >= 1, "bad sizes");
@@ -1035,8 +976,8 @@ extern "C" int madrl_moments_pass_f32(size_t rows, int A, const float* a_dev, co
   return MADRL_OK;
 }
 
-// The centring / shifting of madrl_center_advantages_* with statistics the caller gives (series 0 of stats
-// [A][MADRL_MOMENTS_STATS]); A = 1 runs the whole-batch kernel, as madrl_center_advantages_f32 does.
+// Centring / shifting with statistics the caller gives (series 0 of stats [A][MADRL_MOMENTS_STATS]); A = 1 runs the
+// whole-batch kernel.
 extern "C" int madrl_center_apply_f32(size_t rows, int A, float* adv_dev, const double* stats_dev, int center,
                                       int positive, void* stream) {
   MADRL_REQUIRE(rows >= 1, "bad sizes");
@@ -1239,36 +1180,8 @@ extern "C" int madrl_time_baseline_workspace_size(int G, int L, size_t* bytes) {
   return MADRL_OK;
 }
 
-extern "C" int madrl_time_baseline_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
-                                       const int32_t* seg_start_dev, const int32_t* n_ep_dev,
-                                       const int32_t* ep_rec_dev, const int32_t* t0_dev, double* bin_sum_dev,
-                                       int32_t* bin_count_dev, float* simplev_dev, void* ws_dev, void* stream) {
-  MADRL_REQUIRE(T >= 1 && E >= 1 && A >= 1 && L >= 1, "bad sizes");
-  MADRL_REQUIRE((size_t)T * E * A < ((size_t)1 << 31), "T*E*A must be < 2^31");
-  MADRL_REQUIRE(!per_agent || A <= MADRL_AGENTS_MAX, "n_agents must be in [1, %d], got %d", MADRL_AGENTS_MAX, A);
-  MADRL_REQUIRE(q_dev && seg_start_dev && n_ep_dev && ep_rec_dev && bin_sum_dev && bin_count_dev && simplev_dev &&
-                ws_dev, "NULL buffer");
-  const int G = per_agent ? A : 1, S = tb_slices(G);
-  const size_t part = (size_t)S * G * L;
-  double* ws_sum = (double*)ws_dev;
-  int32_t* ws_cnt = (int32_t*)(ws_sum + part);
-  cudaStream_t s = (cudaStream_t)stream;
-  const size_t blocks = (size_t)((L + kTbThreads - 1) / kTbThreads) * S * G;
-  MADRL_REQUIRE(blocks < ((size_t)1 << 31), "too many bins for one launch");
-  MADRL_LAUNCH(time_baseline_partial_kernel, (unsigned)blocks, kTbThreads, 0, s, T, E, A, G, L, q_dev, n_ep_dev,
-               ep_rec_dev, t0_dev, ws_sum, ws_cnt);
-  const size_t nb = (size_t)G * L, rows = (size_t)T * E * A;
-  MADRL_LAUNCH(time_baseline_bins_kernel, (unsigned)((nb + 255) / 256), 256, 0, s, G, L, ws_sum, ws_cnt, bin_sum_dev,
-               bin_count_dev);
-  MADRL_LAUNCH(time_baseline_apply_kernel, (unsigned)((rows + 255) / 256), 256, 0, s, T, E, A, G, L, seg_start_dev,
-               t0_dev, bin_sum_dev, bin_count_dev, simplev_dev);
-  g_launches.fetch_add(3);
-  MADRL_CUDA_CHECK(cudaGetLastError());
-  return MADRL_OK;
-}
-
-// madrl_time_baseline_f32 split where the bins of several shards are pooled: its partial and bins kernels, then
-// (given the pooled bins) its apply kernel.
+// The time baseline in two calls, so that the bins of several shards can be pooled in between: the partial and bins
+// kernels, then (given the pooled bins) the apply kernel.
 extern "C" int madrl_time_baseline_bins_f32(int T, int E, int A, int per_agent, int L, const float* q_dev,
                                             const int32_t* n_ep_dev, const int32_t* ep_rec_dev, const int32_t* t0_dev,
                                             double* bin_sum_dev, int32_t* bin_count_dev, void* ws_dev, void* stream) {

@@ -138,6 +138,14 @@ def pool_cat(t, group):
     return torch.cat([parts[r][..., :s] for r, s in enumerate(sizes)], dim=-1)
 
 
+def _pooled(pool, t, group):
+    """``pool(t, group)``: the partial `t` pooled over the ranks of the group that shards a batch, by `pool_sum`,
+    `pool_min`, `pool_max`, `pool_cat` or a function that packs or converts `t` for one of them.  ``group=None``
+    means that this rank holds the whole batch, so `t` is returned unchanged (the public pools read None as the
+    default world group)."""
+    return t if group is None else pool(t, group)
+
+
 def _align(n, a=16):
     return (n + a - 1) // a * a
 

@@ -88,14 +88,10 @@ class EpisodeRecords(object):
         self.dtype, dev = engine.dtype, engine.device
         n, A, C = self.K * self.E, self.A, self.C
         self.carry = torch.zeros((self.E, A, _lib.EVAL_CARRY_WORDS), dtype=torch.int64, device=dev)
-        # one buffer, so that read() is one copy: ret, qsum (float64), info sums (int64), lengths (int32)
-        self._words = (n * A, n * A, n * C)
-        self._buf = torch.zeros(8 * sum(self._words) + 4 * n, dtype=torch.uint8, device=dev)
-        o1, o2, o3 = (8 * sum(self._words[:i]) for i in (1, 2, 3))
-        self.ret = self._buf[:o1].view(torch.float64).view(n, A)
-        self.qsum = self._buf[o1:o2].view(torch.float64).view(n, A)
-        self.info_sum = self._buf[o2:o3].view(torch.int64).view(n, C)
-        self.len = self._buf[o3:].view(torch.int32)
+        self.ret = torch.zeros((n, A), dtype=torch.float64, device=dev)
+        self.qsum = torch.zeros((n, A), dtype=torch.float64, device=dev)
+        self.info_sum = torch.zeros((n, C), dtype=torch.int64, device=dev)
+        self.len = torch.zeros((n,), dtype=torch.int32, device=dev)
 
     def add(self, rew, done, info):
         """Fold one launch's rew [T, E, A], done [T, E] and info [T, E, *info_tail] into the records."""
@@ -111,17 +107,11 @@ class EpisodeRecords(object):
     def read(self, n, group=None):
         """Records 0 .. n-1.  ``group``: those of the whole batch, from every rank's records gathered in one
         exchange (`dist.pool_cat` over env-contiguous shards), in the order k * E_global + global env id."""
-        if group is None:
-            buf = self._buf.cpu().numpy()
-            o1, o2, o3 = (8 * sum(self._words[:i]) for i in (1, 2, 3))
-            N, A, C = self.K * self.E, self.A, self.C
-            return (buf[:o1].view(np.float64).reshape(N, A)[:n], buf[o1:o2].view(np.float64).reshape(N, A)[:n],
-                    buf[o3:].view(np.int32)[:n], buf[o2:o3].view(np.int64).reshape(N, C)[:n])
-        from .dist import pool_cat
+        from .dist import _pooled, pool_cat
         K, E, A, C = self.K, self.E, self.A, self.C
         fields = (self.ret, self.qsum, self.info_sum, self.len.view(-1, 1))
         rec = torch.cat([f.view(K, E, -1).view(torch.uint8) for f in fields], dim=2)      # [K, E, bytes per record]
-        rec = pool_cat(rec.transpose(1, 2).contiguous(), group).transpose(1, 2).reshape(-1, rec.shape[2])[:n]
+        rec = _pooled(pool_cat, rec.transpose(1, 2), group).transpose(1, 2).reshape(-1, rec.shape[2])[:n]
         rec = rec.cpu().numpy()
         o1, o2, o3 = 8 * A, 16 * A, 16 * A + 8 * C
         return (rec[:, :o1].copy().view(np.float64), rec[:, o1:o2].copy().view(np.float64),

@@ -95,13 +95,6 @@ def gae(rew, values, done, discount, gae_lambda, last_value=None):
 
 
 MOMENTS_STATS, MOMENTS_WS = 9, 4096            # include/madrl_b200.h
-
-
-def _moments_buffers(dev):
-    return (torch.empty(MOMENTS_STATS, dtype=torch.float64, device=dev),
-            torch.empty(MOMENTS_WS, dtype=torch.float64, device=dev))
-
-
 AGENTS_MAX = 1024                               # include/madrl_b200.h MADRL_AGENTS_MAX
 
 
@@ -117,27 +110,28 @@ def _agent_columns(t, name):
     return t.numel() // A, A
 
 
-def _pooled_moments(a, b, A, group):
-    """float64 [A, 9] moments of the columns of a, b [rows, A] over every rank of a ``torch.distributed`` group:
-    the sums and row counts pooled give the means, the sums of squared deviations about those means pooled give
-    the population variances (NumPy's two passes over the union of the shards), the minima pool by their
-    minimum.  `dist.pool_sum` combines in rank order, so every rank gets the same bits; one rank gets
-    `moments_agents`'s (the division by the rows happens once, on the pooled sums)."""
-    from .dist import pool_min, pool_sum
+def _moments(a, b, A, group):
+    """float64 [A, 9] moments of the columns of a, b [rows, A] (the whole batch is A = 1), over every rank of a
+    ``torch.distributed`` group (None: this rank's rows): the sums and row counts pooled give the means, the sums of
+    squared deviations about those means pooled give the population variances (NumPy's two passes over the union
+    of the shards), the minima pool by their minimum.  `dist.pool_sum` combines in rank order, so every rank gets
+    the same bits.  The row counts stay a float64 device tensor: a division by a host scalar may be computed as a
+    multiplication by its reciprocal, which can differ in the last bit from the division."""
+    from .dist import _pooled, pool_min, pool_sum
     rows, dev = a.numel() // A, a.device
     stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=dev)
     ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=dev)
-    fn = _lib.lib().madrl_moments_pass_f32
+    fn, stream = _lib.lib().madrl_moments_pass_f32, _lib.stream(dev)
     with torch.cuda.device(dev):
-        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 0, _ptr(stats), _ptr(ws), _lib.stream(dev)))
-    count = torch.full((A, 1), float(rows), dtype=torch.float64, device=dev)
-    sums = pool_sum(torch.cat([stats[:, 0:3], count], dim=1), group)
-    stats[:, 6:9] = pool_min(stats[:, 6:9].contiguous(), group)
-    n = sums[:, 3:4]
-    stats[:, 0:3] = sums[:, 0:3] / n
-    with torch.cuda.device(dev):
-        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 1, _ptr(stats), _ptr(ws), _lib.stream(dev)))
-    stats[:, 3:6] = pool_sum(stats[:, 3:6].contiguous(), group) / n
+        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 0, _ptr(stats), _ptr(ws), stream))
+        count = torch.full((A, 1), float(rows), dtype=torch.float64, device=dev)
+        # a group pools the sums and the row counts in one exchange
+        sums, n = _pooled(lambda p, g: pool_sum(torch.cat(p, dim=1), g).split(3, dim=1), (stats[:, 0:3], count),
+                          group)
+        _pooled(lambda m, g: m.copy_(pool_min(m, g)), stats[:, 6:9], group)
+        torch.div(sums, n, out=stats[:, 0:3])
+        _lib.check(fn(rows, A, _ptr(a), _ptr(b), 1, _ptr(stats), _ptr(ws), stream))
+        torch.div(_pooled(pool_sum, stats[:, 3:6], group), n, out=stats[:, 3:6])
     return stats
 
 
@@ -153,27 +147,12 @@ def center_advantages(adv, center=True, positive=False, inplace=False, per_agent
         rows, A = _agent_columns(adv, "adv")
     _lib.require_tensor(adv, "adv", torch.float32, (...,), "cuda", contiguous=False)
     out = adv.contiguous() if inplace else adv.contiguous().clone()
-    if group is not None:
-        if not per_agent:
-            rows, A = out.numel(), 1
-        stats = _pooled_moments(out, None, A, group)
-        with torch.cuda.device(out.device):
-            _lib.check(_lib.lib().madrl_center_apply_f32(rows, A, _ptr(out), _ptr(stats), int(bool(center)),
-                                                         int(bool(positive)), _lib.stream(out.device)))
-        return out
-    if per_agent:
-        stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=out.device)
-        ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=out.device)
-        with torch.cuda.device(out.device):
-            _lib.check(_lib.lib().madrl_center_advantages_agents_f32(rows, A, _ptr(out), int(bool(center)),
-                                                                     int(bool(positive)), _ptr(stats), _ptr(ws),
-                                                                     _lib.stream(out.device)))
-        return out
-    stats, ws = _moments_buffers(out.device)
+    if not per_agent:
+        rows, A = out.numel(), 1
+    stats = _moments(out, None, A, group)
     with torch.cuda.device(out.device):
-        _lib.check(_lib.lib().madrl_center_advantages_f32(out.numel(), _ptr(out), int(bool(center)),
-                                                          int(bool(positive)), _ptr(stats), _ptr(ws),
-                                                          _lib.stream(out.device)))
+        _lib.check(_lib.lib().madrl_center_apply_f32(rows, A, _ptr(out), _ptr(stats), int(bool(center)),
+                                                     int(bool(positive)), _lib.stream(out.device)))
     return out
 
 
@@ -185,33 +164,16 @@ def moments(a, b=None, group=None):
     _lib.require_tensor(a, "a", torch.float32, (...,), None, contiguous=False)
     _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
     _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
-    a = a.contiguous()
-    b = b.contiguous() if b is not None else None
-    if group is not None:
-        return _pooled_moments(a, b, 1, group)[0]
-    stats, ws = _moments_buffers(a.device)
-    with torch.cuda.device(a.device):
-        _lib.check(_lib.lib().madrl_moments_f32(a.numel(), _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
-                                                _lib.stream(a.device)))
-    return stats
+    return _moments(a.contiguous(), None if b is None else b.contiguous(), 1, group)[0]
 
 
 def moments_agents(a, b=None, group=None):
     """float64 [A, 9] cuda tensor: ``moments`` of each agent's samples, the agent being the last axis of
     a (and b), e.g. [T,E,A].  ``group`` as for `moments`."""
-    rows, A = _agent_columns(a, "a")
+    _, A = _agent_columns(a, "a")
     _lib.require_tensor(b, "b", torch.float32, tuple(a.shape), a.device, contiguous=False, optional=True)
     _lib.require_tensor(a, "a", torch.float32, (...,), "cuda", contiguous=False)
-    a = a.contiguous()
-    b = b.contiguous() if b is not None else None
-    if group is not None:
-        return _pooled_moments(a, b, A, group)
-    stats = torch.empty((A, MOMENTS_STATS), dtype=torch.float64, device=a.device)
-    ws = torch.empty((A, MOMENTS_WS), dtype=torch.float64, device=a.device)
-    with torch.cuda.device(a.device):
-        _lib.check(_lib.lib().madrl_moments_agents_f32(rows, A, _ptr(a), _ptr(b), _ptr(stats), _ptr(ws),
-                                                       _lib.stream(a.device)))
-    return stats
+    return _moments(a.contiguous(), None if b is None else b.contiguous(), A, group)
 
 
 def _explained_variance_1d(st):
@@ -225,10 +187,9 @@ def explained_variance(ypred, y, per_agent=False, group=None):
     """``special.explained_variance_1d`` (special.py:51-59) of baseline predictions against returns,
     over every sample of the batch; one 72-byte device->host read.  ``per_agent=True``: one value per
     agent (the last axis), over that agent's samples -- a list of A floats.  ``group`` as for `moments`."""
-    kw = {} if group is None else dict(group=group)
     if per_agent:
-        return [_explained_variance_1d(st) for st in moments_agents(ypred, y, **kw).cpu().numpy()]
-    return _explained_variance_1d(moments(ypred, y, **kw).cpu().numpy())
+        return [_explained_variance_1d(st) for st in moments_agents(ypred, y, group).cpu().numpy()]
+    return _explained_variance_1d(moments(ypred, y, group).cpu().numpy())
 
 
 class FrameStack(object):
@@ -582,10 +543,9 @@ def _sampler_core(baseline, obs, done, rew, discount, gae_lambda, obs_before, t0
     else:
         values = baseline.predict(obs, done, obs_before, t0)
         adv, ret = gae(rew, values, done, discount, gae_lambda)
-    kw = {} if group is None else dict(group=group)
-    ev = explained_variance(values, ret, per_agent=per_agent, **kw)
+    ev = explained_variance(values, ret, per_agent, group)
     if center or positive:
-        adv = center_advantages(adv, center, positive, inplace=True, per_agent=per_agent, **kw)
+        adv = center_advantages(adv, center, positive, inplace=True, per_agent=per_agent, group=group)
     return values, adv, ret, ev
 
 
@@ -854,10 +814,8 @@ def _pooled_statistics(sums, first_ret, group):
     """`_statistics` over the paths of every rank of `group` (None: this rank's): each rank's per-path values,
     8 bytes each, gathered in rank order (`dist.pool_cat`) -- for env-contiguous shards the unsharded batch's
     path order, so the statistics are the unsharded ones bit for bit, and those of one rank its own."""
-    if group is not None:
-        from .dist import pool_cat
-        sums, first_ret = pool_cat(torch.stack([sums, first_ret]), group).unbind(0)
-    return _statistics(sums, first_ret)
+    from .dist import _pooled, pool_cat
+    return _statistics(*_pooled(lambda p, g: pool_cat(torch.stack(p), g).unbind(0), (sums, first_ret), group))
 
 
 def path_returns(rew, ret, done, per_agent=False):

@@ -23,7 +23,7 @@ import torch
 
 from . import _lib, postproc
 from ._lib import _ptr
-from .dist import pool_cat, pool_max, pool_sum
+from .dist import _pooled, pool_cat, pool_max, pool_sum
 from .postproc import _OBS_DTYPES, AGENTS_MAX, _check_mode, _paths_plan
 
 
@@ -117,10 +117,9 @@ class RunningStandardizer(object):
     def _pooled_sums(self, x, obs_before, groups, group):
         """`_sums`, summed over the ranks of a ``torch.distributed`` ``group`` (`dist.pool_sum`) if one is given."""
         sums, n = self._sums(x, obs_before, groups)
-        if group is not None:
-            sums = pool_sum(sums, group)
-            n = int(pool_sum(torch.tensor([n], dtype=torch.int64, device=sums.device), group)[0])
-        return sums, n
+        sums = _pooled(pool_sum, sums, group)
+        rows = lambda r, g: int(pool_sum(torch.tensor([r], dtype=torch.int64, device=sums.device), g)[0])  # noqa: E731
+        return sums, _pooled(rows, n, group)
 
     def update(self, x, obs_before=None, group=None):
         """x [..., D] (every row; [..., A, D] with n_agents: agent a's rows update standardiser a); rows of a
@@ -255,9 +254,8 @@ def time_baseline(q, done, t0=None, per_agent=False, group=None):
     last = ep_rec[:, :, 1].max()
     if t0 is not None:
         last = torch.maximum(last, (t0.to(torch.int32) + ep_rec[:, 0, 1]).max())
-    if group is not None:
-        last = pool_max(last.to(torch.int64).reshape(1), group)[0]
-    L = int(last)
+    # the pools take int64 partials: int32 values widen only when a group pools them
+    L = int(_pooled(lambda x, g: pool_max(x.to(torch.int64).reshape(1), g)[0], last, group))
     if L < 1:
         raise ValueError("t0 must be >= 0")
     q, t0 = q.contiguous(), (None if t0 is None else t0.contiguous())
@@ -268,21 +266,14 @@ def time_baseline(q, done, t0=None, per_agent=False, group=None):
     bin_sum = torch.empty((G, L), dtype=torch.float64, device=dev)
     bin_cnt = torch.empty((G, L), dtype=torch.int32, device=dev)
     simplev = torch.empty_like(q)
-    if group is not None:
-        with torch.cuda.device(dev):
-            _lib.check(lib.madrl_time_baseline_bins_f32(T, E, A, int(bool(per_agent)), L, _ptr(q), _ptr(n_ep),
-                                                        _ptr(ep_rec), _ptr(t0), _ptr(bin_sum), _ptr(bin_cnt), _ptr(ws),
-                                                        _lib.stream(dev)))
-        bin_sum = pool_sum(bin_sum, group).contiguous()
-        bin_cnt = pool_sum(bin_cnt.to(torch.int64), group).to(torch.int32).contiguous()
-        with torch.cuda.device(dev):
-            _lib.check(lib.madrl_time_baseline_apply_f32(T, E, A, int(bool(per_agent)), L, _ptr(seg_s), _ptr(t0),
-                                                         _ptr(bin_sum), _ptr(bin_cnt), _ptr(simplev), _lib.stream(dev)))
-        return simplev, bin_sum, bin_cnt
     with torch.cuda.device(dev):
-        _lib.check(lib.madrl_time_baseline_f32(T, E, A, int(bool(per_agent)), L, _ptr(q), _ptr(seg_s), _ptr(n_ep),
-                                               _ptr(ep_rec), _ptr(t0), _ptr(bin_sum), _ptr(bin_cnt), _ptr(simplev),
-                                               _ptr(ws), _lib.stream(dev)))
+        _lib.check(lib.madrl_time_baseline_bins_f32(T, E, A, int(bool(per_agent)), L, _ptr(q), _ptr(n_ep),
+                                                    _ptr(ep_rec), _ptr(t0), _ptr(bin_sum), _ptr(bin_cnt), _ptr(ws),
+                                                    _lib.stream(dev)))
+        bin_sum = _pooled(pool_sum, bin_sum, group)
+        bin_cnt = _pooled(lambda c, g: pool_sum(c.to(torch.int64), g).to(torch.int32), bin_cnt, group)
+        _lib.check(lib.madrl_time_baseline_apply_f32(T, E, A, int(bool(per_agent)), L, _ptr(seg_s), _ptr(t0),
+                                                     _ptr(bin_sum), _ptr(bin_cnt), _ptr(simplev), _lib.stream(dev)))
     return simplev, bin_sum, bin_cnt
 
 
@@ -353,10 +344,7 @@ def process_samples(baseline, obs, done, rew, discount, gae_lambda, rewnorm=None
     adv, q = postproc.gae(rew_n, values, done, discount, gae_lambda)
     simplev = time_baseline(q, done, t0, per_agent, group)[0]
     mom = postproc.moments_agents if per_agent else postproc.moments
-    if group is None:
-        st = torch.stack([mom(q, values), mom(q, simplev)]).cpu().numpy()
-    else:
-        st = torch.stack([mom(q, values, group=group), mom(q, simplev, group=group)]).cpu().numpy()
+    st = torch.stack([mom(q, values, group), mom(q, simplev, group)]).cpu().numpy()
     v_r, tv_r = _explained(st[0]), _explained(st[1])
     fallback = v_r < 0
     if np.any(fallback):
@@ -389,8 +377,7 @@ def sample_fields(rew, done, mode="decentralized", group=None):
     table = postproc._PathTable(done, rew.shape[2], per_agent)
     sums, _ = table.sums(rew, rew)
     lens = table.rec[:, 3].view(table.lead).double()
-    if group is not None:
-        sums, lens = pool_cat(torch.stack([sums, lens]), group).unbind(0)
+    sums, lens = _pooled(lambda p, g: pool_cat(torch.stack(p), g).unbind(0), (sums, lens), group)
     steps = lens.sum(-1)
     vals = torch.stack([sums.mean(-1), sums.sum(-1) / steps, lens.mean(-1), lens.max(-1).values,
                         lens.min(-1).values], dim=-1).reshape(-1, 5).cpu().numpy()

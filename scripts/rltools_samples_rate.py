@@ -1,5 +1,5 @@
 """Throughput of rltools' sample processing on the device (madrl_b200.rltools_sampler, csrc/postproc.cu
-madrl_running_moments_* / madrl_time_baseline_f32, csrc/baseline.cu madrl_lfbr_*) on full rollout launches, against
+madrl_running_moments_* / madrl_time_baseline_*_f32, csrc/baseline.cu madrl_lfbr_*) on full rollout launches, against
 the PyTorch implementation of the same steps (oracle/rltools_oracle.py torch_process_samples: float64 features
 materialised, a backward loop over time, scatter_add bins for the time baseline, a DGEMM Gram and
 torch.linalg.cholesky).

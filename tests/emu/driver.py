@@ -67,6 +67,26 @@ def paths_plan(lib, done, A):
     return seg_s, seg_l, n_ep, ep_rec
 
 
+def moments(lib, rows, A, a, b=None):
+    """stats float64 [A, 9] of the columns of a, b [rows, A] as madrl_b200.postproc combines madrl_moments_pass_f32:
+    pass 0, its sums divided by the rows in float64, pass 1 about those means, its sums divided by the rows again."""
+    st = Guarded((A, 9), np.float64, np.nan)
+    ws = np.empty((A, 4096))
+    assert lib.madrl_moments_pass_f32(rows, A, ptr(a), ptr(b), 0, ptr(st.arr), ptr(ws), None) == 0
+    st.arr[:, 0:3] /= np.float64(rows)
+    assert lib.madrl_moments_pass_f32(rows, A, ptr(a), ptr(b), 1, ptr(st.arr), ptr(ws), None) == 0
+    st.arr[:, 3:6] /= np.float64(rows)
+    return st.check("stats").copy()
+
+
+def center_advantages(lib, rows, A, x, center, positive):
+    """madrl_b200.postproc.center_advantages of x [rows, A] in place: `moments`, then madrl_center_apply_f32 ->
+    the statistics it used."""
+    stats = moments(lib, rows, A, x)
+    assert lib.madrl_center_apply_f32(rows, A, ptr(x), ptr(stats), center, positive, None) == 0
+    return stats
+
+
 GUARD = 1 << 16   # bytes of canary on either side of every output buffer
 
 

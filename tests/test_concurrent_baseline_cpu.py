@@ -177,7 +177,7 @@ def test_emulated_agent_kernels_match_oracle(lib, shape):
 
 @needs_cxx
 @pytest.mark.parametrize("bf16", [False, True], ids=["f32", "bf16"])
-def test_emulated_one_agent_equals_pooled_bitwise(lib, bf16):
+def test_emulated_one_agent_equals_whole_batch_bitwise(lib, bf16):
     rs = np.random.RandomState(5)
     T, E, D = 37, 3, 9
     obs = (rs.randn(T, E, 1, D) * 6).astype(np.float32)
@@ -196,30 +196,26 @@ def test_emulated_one_agent_equals_pooled_bitwise(lib, bf16):
     Ga, va = _run(lib, obs, obs_before, done, ret, t0, coef, bf16, True)
     assert np.array_equal(Ga[0], Gp) and np.array_equal(va, vp)
     adv = (rs.randn(T, E, 1) * 3 + 1).astype(np.float32)
-    stats_p, stats_a = np.empty(9), np.empty((1, 9))
-    ws = np.empty(4096)
-    assert lib.madrl_moments_f32(adv.size, _p(adv), _p(ret), _p(stats_p), _p(ws), None) == 0
-    assert lib.madrl_moments_agents_f32(adv.size, 1, _p(adv), _p(ret), _p(stats_a), _p(ws), None) == 0
+    stats_p = driver.moments(lib, adv.size, 1, adv.reshape(-1), ret.reshape(-1))[0]       # the whole batch
+    stats_a = driver.moments(lib, adv.size, 1, adv, ret)                                 # agent 0 of [T, E, 1]
     assert np.array_equal(stats_a[0], stats_p)
     for center, positive in ((1, 0), (1, 1), (0, 1)):
-        x_p, x_a = adv.copy(), adv.copy()
-        assert lib.madrl_center_advantages_f32(x_p.size, _p(x_p), center, positive, _p(stats_p), _p(ws), None) == 0
-        assert lib.madrl_center_advantages_agents_f32(x_a.size, 1, _p(x_a), center, positive, _p(stats_a), _p(ws),
-                                                      None) == 0
-        assert np.array_equal(x_a, x_p)
+        x_p, x_a = adv.reshape(-1).copy(), adv.copy()
+        driver.center_advantages(lib, x_p.size, 1, x_p, center, positive)
+        driver.center_advantages(lib, x_a.size, 1, x_a, center, positive)
+        assert np.array_equal(x_a.reshape(-1), x_p)
     assert driver.races() == 0
 
 
 @needs_cxx
 @pytest.mark.parametrize("A", [1, 3, 7])
-def test_emulated_agent_moments_and_centring(lib, A):
+def test_emulated_agent_moment_passes_and_centring(lib, A):
     rs = np.random.RandomState(A)
     rows = 997
     a = (rs.randn(rows, A) * np.arange(1, A + 1) + np.arange(A) * 3).astype(np.float32)
     b = (a + rs.randn(rows, A)).astype(np.float32)
-    stats, ws = np.empty((A, 9)), np.empty(4096 * A)
     driver.races()
-    assert lib.madrl_moments_agents_f32(rows, A, _p(a), _p(b), _p(stats), _p(ws), None) == 0
+    stats = driver.moments(lib, rows, A, a, b)
     for c in range(A):
         s = [a[:, c].astype(np.float64), b[:, c].astype(np.float64)]
         s.append(s[1] - s[0])
@@ -230,7 +226,7 @@ def test_emulated_agent_moments_and_centring(lib, A):
         assert abs(got - ev) <= 1e-12
     for center, positive in ((1, 0), (1, 1), (0, 1)):
         x = a.copy()
-        assert lib.madrl_center_advantages_agents_f32(rows, A, _p(x), center, positive, _p(stats), _p(ws), None) == 0
+        driver.center_advantages(lib, rows, A, x, center, positive)
         for c in range(A):
             want = a[:, c].astype(np.float64)
             if center:
@@ -242,7 +238,7 @@ def test_emulated_agent_moments_and_centring(lib, A):
 
 
 @needs_cxx
-def test_emulated_agent_workspace_and_bad_sizes(lib):
+def test_emulated_agent_workspace_and_pass_bad_sizes(lib):
     nbytes = C.c_size_t()
     assert lib.madrl_lfb_agents_workspace_size(213, 5, C.byref(nbytes)) == 0
     assert nbytes.value == 5 * 1 * 28 * 64 * 64 * 8                    # emulator build: 3 slices -> 1 per agent
@@ -265,12 +261,13 @@ def test_emulated_agent_workspace_and_bad_sizes(lib):
     assert p(1, 1, 1025, 4, _p(x), None, _p(seg), None, _p(x), _p(x), None) != 0
     assert p(1, 1, 2, 4, _p(x), None, _p(seg), None, None, _p(x), None) != 0                       # NULL coef
     s = np.zeros(9 * 4)
-    assert lib.madrl_moments_agents_f32(0, 2, _p(x), None, _p(s), _p(s), None) != 0
-    assert lib.madrl_moments_agents_f32(4, 0, _p(x), None, _p(s), _p(s), None) != 0
-    assert lib.madrl_moments_agents_f32(4, 1025, _p(x), None, _p(s), _p(s), None) != 0
-    assert lib.madrl_moments_agents_f32(4, 2, None, None, _p(s), _p(s), None) != 0
-    assert lib.madrl_center_advantages_agents_f32(4, 2, _p(x), 1, 0, None, _p(s), None) != 0
-    assert lib.madrl_center_advantages_agents_f32(4, 1025, _p(x), 1, 0, _p(s), _p(s), None) != 0
+    for pass_ in (0, 1):
+        assert lib.madrl_moments_pass_f32(0, 2, _p(x), None, pass_, _p(s), _p(s), None) != 0
+        assert lib.madrl_moments_pass_f32(4, 0, _p(x), None, pass_, _p(s), _p(s), None) != 0
+        assert lib.madrl_moments_pass_f32(4, 1025, _p(x), None, pass_, _p(s), _p(s), None) != 0
+        assert lib.madrl_moments_pass_f32(4, 2, None, None, pass_, _p(s), _p(s), None) != 0
+    assert lib.madrl_center_apply_f32(4, 2, _p(x), None, 1, 0, None) != 0
+    assert lib.madrl_center_apply_f32(4, 1025, _p(x), _p(s), 1, 0, None) != 0
 
 
 # ---------------------------------------------------------------- argument validation (no library call)

@@ -1,9 +1,9 @@
 """The entry points that split a statistic where the shards of a batch are pooled, executed on the CPU by the warp
-emulator of tests/emu through the C ABI: madrl_time_baseline_bins_f32 + madrl_time_baseline_apply_f32 against the
-fused madrl_time_baseline_f32, madrl_moments_pass_f32 against madrl_moments_f32 / madrl_moments_agents_f32 and
-madrl_center_apply_f32 against madrl_center_advantages_*.  On the same arguments the split calls give the fused
-calls' bits; the bins of two env halves, summed, give the whole batch's counts exactly and its simplev within one
-float32 ulp.  Outputs sit in canary-guarded buffers; the argument checks (MADRL_EINVAL, no launch) are exercised."""
+emulator of tests/emu through the C ABI: the bins of madrl_time_baseline_bins_f32 over env shards, summed, give the
+whole batch's counts exactly and its simplev (madrl_time_baseline_apply_f32) within one float32 ulp;
+madrl_moments_pass_f32 over row shards, pooled, gives the float64 moments of the union, and madrl_center_apply_f32 on
+each shard with them NumPy's centring of the union.  Outputs sit in canary-guarded buffers; the argument checks
+(MADRL_EINVAL, no launch) are exercised."""
 import ctypes as C
 
 import numpy as np
@@ -33,16 +33,6 @@ def _ws(lib, G, L):
     return np.zeros(nbytes.value, np.uint8)
 
 
-def _fused(lib, q, done, t0, per_agent, L):
-    T, E, A = q.shape
-    G = A if per_agent else 1
-    seg_s, _, n_ep, ep_rec = driver.paths_plan(lib, done, A)
-    s, c, v = np.full((G, L), np.nan), np.full((G, L), -1, np.int32), np.full((T, E, A), np.nan, np.float32)
-    assert lib.madrl_time_baseline_f32(T, E, A, per_agent, L, _p(q), _p(seg_s), _p(n_ep), _p(ep_rec), _p(t0), _p(s),
-                                       _p(c), _p(v), _p(_ws(lib, G, L)), None) == 0
-    return s, c, v
-
-
 def _bins(lib, q, done, t0, per_agent, L):
     T, E, A = q.shape
     G = A if per_agent else 1
@@ -60,6 +50,12 @@ def _apply(lib, done, t0, per_agent, A, L, s, c):
     assert lib.madrl_time_baseline_apply_f32(T, E, A, per_agent, L, _p(seg_s), _p(t0), _p(s), _p(c), _p(v.arr),
                                              None) == 0, lib.madrl_last_error()
     return v.check("simplev").copy()
+
+
+def _whole(lib, q, done, t0, per_agent, L):
+    """The whole batch's bins and simplev, from one rank's calls."""
+    s, c = _bins(lib, q, done, t0, per_agent, L)
+    return s, c, _apply(lib, done, t0, per_agent, q.shape[2], L, s, c)
 
 
 def _case(A, k):
@@ -85,22 +81,8 @@ def _last_index(done, t0):
     return L
 
 
-@pytest.mark.parametrize("A", (1, 2, 3, 5))
-def test_time_baseline_bins_then_apply_equal_the_fused_call(lib, A):
-    for k in range(len(TB_SHAPES)):
-        q, done, t0s = _case(A, k)
-        for t0 in t0s:
-            L = _last_index(done, t0)
-            for per_agent in (0, 1):
-                s, c, v = _fused(lib, q, done, t0, per_agent, L)
-                bs, bc = _bins(lib, q, done, t0, per_agent, L)
-                assert np.array_equal(bs, s) and np.array_equal(bc, c)
-                got = _apply(lib, done, t0, per_agent, A, L, bs, bc)
-                assert np.array_equal(got.view(np.uint32), v.view(np.uint32)), (k, per_agent)
-
-
 @pytest.mark.parametrize("A", (1, 3))
-def test_time_baseline_bins_of_two_env_halves_pool_to_the_whole_batch(lib, A):
+def test_time_baseline_bins_of_two_env_halves_sum_to_the_whole_batch(lib, A):
     """Each half's bins over the pooled L (a larger L than the half's own: zero bins past its paths), summed: the
     whole batch's counts exactly, its sums to rounding, and each half's simplev within one float32 ulp of the
     whole batch's rows."""
@@ -115,7 +97,7 @@ def test_time_baseline_bins_of_two_env_halves_pool_to_the_whole_batch(lib, A):
             halves = [(slice(0, h), None if t0 is None else t0[:h].copy()),
                       (slice(h, E), None if t0 is None else t0[h:].copy())]
             for per_agent in (0, 1):
-                s, c, v = _fused(lib, q, done, t0, per_agent, L)
+                s, c, v = _whole(lib, q, done, t0, per_agent, L)
                 parts = [_bins(lib, np.ascontiguousarray(q[:, sl]), np.ascontiguousarray(done[:, sl]), t, per_agent,
                                L) for sl, t in halves]
                 ps, pc = parts[0][0] + parts[1][0], parts[0][1] + parts[1][1]
@@ -129,10 +111,10 @@ def test_time_baseline_bins_of_two_env_halves_pool_to_the_whole_batch(lib, A):
 
 @pytest.mark.parametrize("W", (3, 4))
 @pytest.mark.parametrize("A", (1, 3))
-def test_time_baseline_bins_of_uneven_shards_pool_to_the_whole_batch(lib, W, A):
+def test_time_baseline_bins_of_uneven_shards_sum_to_the_whole_batch(lib, W, A):
     """Shards of one env (rank 0 never done, holding the largest index; rank 1 done on every step, its own L far
     below the pooled L), bins over the pooled L summed in rank order: the whole batch's counts exactly, its sums at
-    1e-13, each shard's simplev within one float32 ulp of the fused call's rows, and the bins of the float64
+    1e-13, each shard's simplev within one float32 ulp of the whole batch's rows, and the bins of the float64
     reference of postproc_edges.time_index."""
     sizes = se.TB_SIZES[W]
     for L in (127, 129):
@@ -141,7 +123,7 @@ def test_time_baseline_bins_of_uneven_shards_pool_to_the_whole_batch(lib, W, A):
             shards = [(np.ascontiguousarray(q[:, lo:hi]), np.ascontiguousarray(done[:, lo:hi]),
                        None if t0 is None else t0[lo:hi].copy()) for lo, hi in se.bounds(sizes)]
             for per_agent in (0, 1):
-                s, c, v = _fused(lib, q, done, t0, per_agent, L)
+                s, c, v = _whole(lib, q, done, t0, per_agent, L)
                 parts = [_bins(lib, qs, ds, ts, per_agent, L) for qs, ds, ts in shards]
                 ps, pc = parts[0][0].copy(), parts[0][1].copy()
                 for bs, bc in parts[1:]:                 # rank order, as dist.pool_sum adds them
@@ -152,54 +134,6 @@ def test_time_baseline_bins_of_uneven_shards_pool_to_the_whole_batch(lib, W, A):
                 for g, (lo, hi) in zip(got, se.bounds(sizes)):
                     assert se.ulps(g, v[:, lo:hi]) <= 1
                 pe.check_time_baseline(np.concatenate(got, axis=1), ps, pc, q, done, t0, per_agent)
-
-
-def _passes(lib, rows, A, a, b):
-    """madrl_moments_pass_f32's two passes, the means formed between them as the pooled host code forms them."""
-    st = Guarded((A, 9), np.float64, np.nan)
-    ws = np.empty((A, 4096))
-    assert lib.madrl_moments_pass_f32(rows, A, _p(a), _p(b), 0, _p(st.arr), _p(ws), None) == 0
-    sums = st.arr[:, 0:3].copy()
-    st.arr[:, 0:3] = sums / float(rows)
-    assert lib.madrl_moments_pass_f32(rows, A, _p(a), _p(b), 1, _p(st.arr), _p(ws), None) == 0
-    out = st.check("stats").copy()
-    return sums, out[:, 3:6].copy(), out[:, 6:9].copy(), out
-
-
-@pytest.mark.parametrize("A", (1, 2, 3))
-def test_moment_passes_equal_the_fused_moments_bitwise(lib, A):
-    """Sums over rows give madrl_moments_*'s means, the second pass about those means over rows its variances, and
-    the minima are its minima, bit for bit, at the grid-stride edges and with and without b."""
-    for rows in pe.stride_sizes(EMU_MOM_BLOCKS):
-        x, y = pe.agent_columns(rows, A, A)
-        for b in (y, None):
-            want, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
-            if A == 1:
-                assert lib.madrl_moments_f32(rows, _p(x), _p(b), _p(want), _p(ws), None) == 0
-            else:
-                assert lib.madrl_moments_agents_f32(rows, A, _p(x), _p(b), _p(want), _p(ws), None) == 0
-            sums, sq, mins, got = _passes(lib, rows, A, x, b)
-            cols = slice(0, 3) if b is not None else slice(0, 1)
-            assert np.array_equal((sums / float(rows))[:, cols], want[:, 0:3][:, cols]), rows
-            assert np.array_equal((sq / float(rows))[:, cols], want[:, 3:6][:, cols]), rows
-            assert np.array_equal(mins[:, cols], want[:, 6:9][:, cols]), rows
-
-
-@pytest.mark.parametrize("A", (1, 2, 3))
-def test_center_apply_equals_center_advantages_bitwise(lib, A):
-    rows = 2 * EMU_MOM_BLOCKS * 256 + 7
-    x, _ = pe.agent_columns(rows, A, A)
-    for center, positive in pe.CENTRE_MODES:
-        want = x.copy()
-        stats, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
-        if A == 1:
-            assert lib.madrl_center_advantages_f32(rows, _p(want), center, positive, _p(stats), _p(ws), None) == 0
-        else:
-            assert lib.madrl_center_advantages_agents_f32(rows, A, _p(want), center, positive, _p(stats), _p(ws),
-                                                          None) == 0
-        got = Guarded(x.shape, np.float32, x)
-        assert lib.madrl_center_apply_f32(rows, A, _p(got.arr), _p(stats), center, positive, None) == 0
-        assert np.array_equal(got.check("adv").view(np.uint32), want.view(np.uint32)), (center, positive)
 
 
 def test_split_entry_points_reject_bad_arguments(lib):
@@ -238,7 +172,7 @@ def test_split_entry_points_reject_bad_arguments(lib):
 
 @pytest.mark.parametrize("W", (2, 3, 4))
 def test_moment_passes_over_shards_pool_to_the_union(lib, W):
-    """madrl_moments_pass_f32 over W shards at the emulator's grid-stride edges, pooled as postproc._pooled_moments
+    """madrl_moments_pass_f32 over W shards at the emulator's grid-stride edges, pooled as postproc._moments
     pools them (sums and rows added in rank order, minima by minimum, the second pass about the pooled means): the
     float64 moments of the union; madrl_center_apply_f32 on each shard with the pooled statistics: NumPy's centring
     and shift of the union within one float32 ulp."""

@@ -1,11 +1,12 @@
 """The trajectory post-processing kernels (madrl_b200/csrc/postproc.cu: GAE, frame stack,
-standardiser, episode statistics, whole-batch moments / advantage centring) executed on the CPU by
+standardiser, episode statistics, per-column moments / advantage centring) executed on the CPU by
 the warp emulator of tests/emu and compared with oracle/postproc_oracle.py -- the GPU test
 tests/test_postproc.py::test_cuda_* at small sizes, through the same C ABI."""
 import numpy as np
 import pytest
 
 import postproc_edges as pe
+import sharded_edges as se
 from emu import build_emu, driver
 from emu.driver import Guarded
 from emu.driver import ptr as _p
@@ -100,20 +101,19 @@ def test_episode_stats(lib):
             assert outs['ln'][t, e] == length
 
 
-def test_moments_and_advantage_centring(lib):
+def test_moment_passes_and_advantage_centring(lib):
     rs = np.random.RandomState(9)
     for n in (1, 3, 1050, 20000):        # 20000: every block of the (narrowed, see build_emu.py) grid loops
         adv = (rs.randn(n) * 3 + 1).astype(np.float32)
         ret = rs.randn(n).astype(np.float32)
-        stats, ws = np.empty(9), np.empty(4096)
-        assert lib.madrl_moments_f32(n, _p(adv), _p(ret), _p(stats), _p(ws), None) == 0
+        stats = driver.moments(lib, n, 1, adv, ret)[0]
         a64, r64 = adv.astype(np.float64), ret.astype(np.float64)
         want = np.array([a64.mean(), r64.mean(), (r64 - a64).mean(), a64.var(), r64.var(), (r64 - a64).var(),
                          a64.min(), r64.min(), (r64 - a64).min()])
         assert np.allclose(stats, want, rtol=1e-10, atol=1e-12)
         for center, positive in ((1, 0), (0, 1), (1, 1)):
             x = adv.copy()
-            assert lib.madrl_center_advantages_f32(n, _p(x), center, positive, _p(stats), _p(ws), None) == 0
+            driver.center_advantages(lib, n, 1, x, center, positive)
             w = a64
             if center:
                 w = po.center_advantages(w)
@@ -196,41 +196,50 @@ def test_standardizer_with_terminal_observations_follows_the_reference_order(lib
 EMU_MOM_BLOCKS = build_emu.GRID["MADRL_MOM_BLOCKS"]
 
 
-def test_moments_at_the_grid_stride_edges(lib):
-    """n at the block edge and at one and three grid strides, data offset by 1e4 (a one-pass variance fails)."""
+def test_moment_passes_at_the_grid_stride_edges(lib):
+    """n at the block edge and at one and three grid strides, data offset by 1e4 (a one-pass variance fails); then
+    the same rows per column of 1, 2 and 3 agents, with and without b (b = 0: series s1 = 0 and s2 = -a)."""
     for n in pe.stride_sizes(EMU_MOM_BLOCKS):
         a, b = pe.offset_series(n, n)
-        stats, ws = np.full(9, np.nan), np.empty(4096)
-        assert lib.madrl_moments_f32(n, _p(a), _p(b), _p(stats), _p(ws), None) == 0
+        stats = driver.moments(lib, n, 1, a, b)[0]
         assert np.allclose(stats, pe.moments_want(a, b), rtol=1e-10, atol=1e-12), n
+    for A in (1, 2, 3):
+        for n in pe.stride_sizes(EMU_MOM_BLOCKS):
+            x, y = pe.agent_columns(n, A, A)
+            for b in (y, None):
+                stats = driver.moments(lib, n, A, x, b)
+                want = se.moments_of(x, np.zeros_like(x) if b is None else b)
+                np.testing.assert_allclose(stats, want, rtol=1e-10, atol=1e-12, err_msg=str((A, n)))
+                assert np.array_equal(stats[:, 6:9], want[:, 6:9])
 
 
 @pytest.mark.parametrize("A", [1, 2, 3, 257])
-def test_agent_moments_and_centring_equal_pooled_bitwise(lib, A):
-    """Agent a's statistics and centred column are the pooled call's on that column alone, bit for bit (same block
-    loop, fold order and constant expressions).  A = 257: the per-agent constants of the centring kernel take a
+def test_agent_moments_and_centring_equal_whole_batch_bitwise(lib, A):
+    """Agent a's statistics and centred column are the whole-batch call's on that column alone, bit for bit (same
+    block loop, fold order and constant expressions), and NumPy's within rounding: the float64 moments, and the
+    centring and shift within one float32 ulp.  A = 257: the per-agent constants of the centring kernel take a
     second pass of its strided loop; a launch then has 6 x 257 CTAs of fibers, so that case runs one centring
     mode and compares the agents on either side of 256 (the GPU test covers every agent and mode)."""
     rows = 2 * EMU_MOM_BLOCKS * 256 + 7 if A <= 3 else 45
     x, y = pe.agent_columns(rows, A, A)
     agents, modes = (range(A), pe.CENTRE_MODES) if A <= 3 else ((0, 255, 256), ((1, 1),))
-    stats, ws = np.full((A, 9), np.nan), np.empty((A, 4096))
-    st1, ws1 = np.empty(9), np.empty(4096)
     if A <= 3:
-        assert lib.madrl_moments_agents_f32(rows, A, _p(x), _p(y), _p(stats), _p(ws), None) == 0
+        stats = driver.moments(lib, rows, A, x, y)
+        want = se.moments_of(x, y)
+        np.testing.assert_allclose(stats, want, rtol=1e-10, atol=1e-12 * np.abs(want).max())
         for a in agents:
             xa, ya = np.ascontiguousarray(x[:, a]), np.ascontiguousarray(y[:, a])
-            assert lib.madrl_moments_f32(rows, _p(xa), _p(ya), _p(st1), _p(ws1), None) == 0
-            assert np.array_equal(stats[a], st1), a
+            assert np.array_equal(stats[a], driver.moments(lib, rows, 1, xa, ya)[0]), a
     for center, positive in modes:
         xs = Guarded(x.shape, np.float32, x)
-        assert lib.madrl_center_advantages_agents_f32(rows, A, _p(xs.arr), center, positive, _p(stats), _p(ws),
-                                                      None) == 0
+        stats = driver.center_advantages(lib, rows, A, xs.arr, center, positive)
         got = xs.check("adv")
         for a in agents:
             xa = x[:, a].copy()
-            assert lib.madrl_center_advantages_f32(rows, _p(xa), center, positive, _p(st1), _p(ws1), None) == 0
-            assert np.array_equal(stats[a], st1) and np.array_equal(got[:, a], xa), (center, positive, a)
+            st1 = driver.center_advantages(lib, rows, 1, xa, center, positive)
+            assert np.array_equal(stats[a], st1[0]) and np.array_equal(got[:, a], xa), (center, positive, a)
+            if A <= 3:
+                assert se.ulps(got[:, a], se.centred_want(x[:, a], center, positive)) <= 1, (center, positive, a)
 
 
 def test_frame_stack_every_buffer_size(lib):

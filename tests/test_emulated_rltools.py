@@ -1,7 +1,7 @@
 """rltools' sample-processing kernels executed on the CPU by the warp emulator of tests/emu, through the C ABI, against
 NumPy and oracle/rltools_oracle.py: madrl_running_moments_{f32,bf16} (column sums of x and x^2, pooled and per agent,
-with and without the one-step observation shift), madrl_time_baseline_f32 (bins, counts and simplev, pooled and per
-agent, with t0), and rltools' feature map of the linear-baseline kernels (madrl_lfbr_*), with and without an obsnorm.
+with and without the one-step observation shift), madrl_time_baseline_bins_f32 then madrl_time_baseline_apply_f32
+(bins, counts and simplev, pooled and per agent, with t0), and rltools' feature map of the linear-baseline kernels (madrl_lfbr_*), with and without an obsnorm.
 The shapes cross the row-slice, warp-stride and 32-column edges of the kernels; A runs from 1 to 8.  Outputs sit in
 canary-guarded buffers, and every new entry point's argument checks (MADRL_EINVAL, no launch) are exercised."""
 import ctypes as C
@@ -119,7 +119,7 @@ TB_SHAPES = ((5, 2, 0.3), (9, 7, 0.2), (140, 4, 0.0), (33, 11, 0.1))
 
 
 @pytest.mark.parametrize("A", (1, 2, 3, 5, 8))
-def test_time_baseline_against_numpy(lib, A):
+def test_time_baseline_bins_and_apply_against_numpy(lib, A):
     for k, (T, E, p) in enumerate(TB_SHAPES):
         rs = np.random.RandomState(100 * A + k)
         done = (rs.rand(T, E) < p).astype(np.uint8)
@@ -137,8 +137,10 @@ def test_time_baseline_against_numpy(lib, A):
                 ws = np.zeros(nbytes.value, np.uint8)
                 s, c = Guarded((G, L), np.float64, np.nan), Guarded((G, L), np.int32, -1)
                 v = Guarded((T, E, A), np.float32, np.nan)
-                assert lib.madrl_time_baseline_f32(T, E, A, per_agent, L, _p(q), _p(seg_s), _p(n_ep), _p(ep_rec),
-                                                   _p(t0), _p(s.arr), _p(c.arr), _p(v.arr), _p(ws), None) == 0
+                assert lib.madrl_time_baseline_bins_f32(T, E, A, per_agent, L, _p(q), _p(n_ep), _p(ep_rec), _p(t0),
+                                                        _p(s.arr), _p(c.arr), _p(ws), None) == 0
+                assert lib.madrl_time_baseline_apply_f32(T, E, A, per_agent, L, _p(seg_s), _p(t0), _p(s.arr),
+                                                         _p(c.arr), _p(v.arr), None) == 0
                 ws_, wc = np.zeros((G, L)), np.zeros((G, L), np.int64)
                 for a in range(A):
                     np.add.at(ws_[a if per_agent else 0], idx, q[..., a].astype(np.float64))
@@ -151,7 +153,7 @@ def test_time_baseline_against_numpy(lib, A):
                 np.testing.assert_allclose(got, want, rtol=2e-7, atol=1e-7)
 
 
-def test_time_baseline_is_the_reference_nanmean(lib):
+def test_time_baseline_bins_are_the_reference_nanmean(lib):
     """simplev of a rollout's paths equals Sampler.process's nanmean over the padded q (the oracle's)."""
     rs = np.random.RandomState(4)
     T, E, A = 12, 5, 3
@@ -163,8 +165,9 @@ def test_time_baseline_is_the_reference_nanmean(lib):
     assert lib.madrl_time_baseline_workspace_size(1, L, C.byref(nbytes)) == 0
     ws = np.zeros(nbytes.value, np.uint8)
     s, c, v = np.zeros((1, L)), np.zeros((1, L), np.int32), np.zeros((T, E, A), np.float32)
-    assert lib.madrl_time_baseline_f32(T, E, A, 0, L, _p(q), _p(seg_s), _p(n_ep), _p(ep_rec), None, _p(s), _p(c),
-                                       _p(v), _p(ws), None) == 0
+    assert lib.madrl_time_baseline_bins_f32(T, E, A, 0, L, _p(q), _p(n_ep), _p(ep_rec), None, _p(s), _p(c), _p(ws),
+                                            None) == 0
+    assert lib.madrl_time_baseline_apply_f32(T, E, A, 0, L, _p(seg_s), None, _p(s), _p(c), _p(v), None) == 0
     paths = ro.batches(np.zeros((T, E, A, 1), np.float32), q.astype(np.float64), done, None, "decentralized")[0]
     rows = ro._padded([p["rewards"] for p in paths], np.nan)
     np.testing.assert_allclose(s[0] / c[0], np.nanmean(rows, axis=0), rtol=1e-13)
@@ -233,7 +236,7 @@ def test_rltools_feature_map_against_numpy(lib, A, D, obsnorm, shifted, bf16):
     assert int(lib.madrl_emu_race_count()) == 0
 
 
-def test_argument_errors(lib):
+def test_sample_entry_points_refuse_bad_arguments(lib):
     """MADRL_EINVAL, and no launch, for sizes below 1, group counts past MADRL_AGENTS_MAX, a shift outside the rows
     and NULL buffers, at every new entry point."""
     x, d, i32 = np.zeros(64, np.float32), np.zeros(64), np.zeros(64, np.int32)
@@ -251,14 +254,17 @@ def test_argument_errors(lib):
     for G, L in ((0, 1), (1, 0), (1025, 1)):
         assert lib.madrl_time_baseline_workspace_size(G, L, C.byref(n)) != 0
     assert lib.madrl_time_baseline_workspace_size(1, 1, None) != 0
-    ok = [_p(x), _p(i32), _p(i32), _p(i32), None, _p(d), _p(i32), _p(x), _p(d)]
-    tb = lib.madrl_time_baseline_f32
-    for sizes in ((0, 1, 1, 0, 1), (1, 0, 1, 0, 1), (1, 1, 0, 0, 1), (1, 1, 1, 0, 0), (1, 1, 1025, 1, 1)):
-        assert tb(*sizes, *ok, None) != 0, sizes
-    for k in (0, 1, 2, 3, 5, 6, 7, 8):
-        args = list(ok)
-        args[k] = None
-        assert tb(1, 1, 1, 0, 1, *args, None) != 0, k
+    # (entry point, its buffers: q, n_ep, ep_rec, t0, bin_sum, bin_count, ws / seg_start, t0, bin_sum, bin_count,
+    # simplev, and the positions of the required ones)
+    for tb, ok, required in ((lib.madrl_time_baseline_bins_f32, [_p(x), _p(i32), _p(i32), None, _p(d), _p(i32), _p(d)],
+                              (0, 1, 2, 4, 5, 6)),
+                             (lib.madrl_time_baseline_apply_f32, [_p(i32), None, _p(d), _p(i32), _p(x)], (0, 2, 3, 4))):
+        for sizes in ((0, 1, 1, 0, 1), (1, 0, 1, 0, 1), (1, 1, 0, 0, 1), (1, 1, 1, 0, 0), (1, 1, 1025, 1, 1)):
+            assert tb(*sizes, *ok, None) != 0, sizes
+        for k in required:
+            args = list(ok)
+            args[k] = None
+            assert tb(1, 1, 1, 0, 1, *args, None) != 0, k
     for D in (0, 8193):
         assert lib.madrl_lfbr_workspace_size(D, C.byref(n)) != 0
         assert lib.madrl_lfbr_agents_workspace_size(D, 2, C.byref(n)) != 0

@@ -1,6 +1,7 @@
 """dist.pool_sum / pool_max / pool_min / pool_cat over a gloo group of spawned CPU processes: the partials combine in
 ascending rank order (three ranks, so that float64 addition order shows), every rank gets the same bytes, int64
-partials sum exactly, ragged last axes concatenate in rank order, and a one-rank group returns the partial itself."""
+partials sum exactly, ragged last axes concatenate in rank order, and a one-rank group returns the partial itself, as
+the sample-processing helper `_pooled` does without a group (while the pools read None as the world group)."""
 import os
 import socket
 
@@ -8,7 +9,7 @@ import torch
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-from madrl_b200.dist import pool_cat, pool_max, pool_min, pool_sum
+from madrl_b200.dist import _pooled, pool_cat, pool_max, pool_min, pool_sum
 
 WORLD = 3
 # in rank order (1e16 + 1) + -1e16 = 0 (1e16 + 1 rounds back to 1e16); in another order the sum is 1
@@ -36,6 +37,7 @@ def _worker(rank, port, q):
             out["refused_f32"] = True
         own, _ = dist.new_subgroups(group_size=1)                     # this rank alone
         out["one_rank_identity"] = pool_sum(f, own) is f and pool_min(i, own) is i and pool_cat(f, own) is f
+        out["no_group_identity"] = all(_pooled(p, f, None) is f for p in (pool_sum, pool_max, pool_min, pool_cat))
         q.put((rank, {k: (v.numpy().tobytes(), tuple(v.shape)) if torch.is_tensor(v) else v for k, v in out.items()}))
     finally:
         dist.destroy_process_group()
@@ -69,7 +71,7 @@ def test_pool_helpers_over_three_gloo_ranks():
     for r in range(1, WORLD):
         assert got[r] == got[0]                                        # the same bytes on every rank
     res = got[0]
-    assert res["refused_f32"] and res["one_rank_identity"]
+    assert res["refused_f32"] and res["one_rank_identity"] and res["no_group_identity"]
     parts = [_partials(r) for r in range(WORLD)]
     want = parts[0][0].clone()
     for r in range(1, WORLD):

@@ -146,8 +146,8 @@ def test_cuda_postproc_matches_oracle():
 
 @pytest.mark.gpu
 def test_cuda_batch_statistics_match_oracle():
-    """madrl_center_advantages_f32 / madrl_moments_f32 against the oracle (float64 NumPy on the same
-    float32 inputs); tolerance 1e-5 relative to the value scale, results deterministic."""
+    """center_advantages / moments (madrl_moments_pass_f32, madrl_center_apply_f32) against the oracle (float64
+    NumPy on the same float32 inputs); tolerance 1e-5 relative to the value scale, results deterministic."""
     import torch
     from madrl_b200.postproc import center_advantages, explained_variance, moments
     import postproc_edges as pe
@@ -186,6 +186,40 @@ def test_cuda_batch_statistics_match_oracle():
     assert explained_variance(torch.as_tensor(rs.randn(64).astype(np.float32), device='cuda'), const) == 0
     out = center_advantages(const.clone(), inplace=True)                  # zero variance: 0 / 1e-8
     assert torch.equal(out, torch.zeros_like(out))
+
+
+@pytest.mark.gpu
+def test_cuda_moments_divide_the_pass_sums_by_the_rows():
+    """`moments` and `moments_agents` equal, bit for bit, madrl_moments_pass_f32's two passes called directly with
+    their sums divided by the rows in NumPy float64 (one IEEE division per value).  rows = 3 x 5^7, whose reciprocal
+    is not exact: a multiplication by 1 / rows would differ in the last bit of some of the values."""
+    import torch
+    from madrl_b200 import _lib
+    from madrl_b200._lib import _ptr
+    from madrl_b200.postproc import moments, moments_agents
+    rows, lib = 3 * 5 ** 7, _lib.lib()
+    rs = np.random.RandomState(12)
+
+    def passes(x, b, A):
+        st = torch.full((A, 9), float("nan"), dtype=torch.float64, device="cuda")
+        ws = torch.empty((A, 4096), dtype=torch.float64, device="cuda")
+        want = np.empty((A, 9))
+        for p in (0, 1):
+            _lib.check(lib.madrl_moments_pass_f32(rows, A, _ptr(x), _ptr(b), p, _ptr(st), _ptr(ws),
+                                                  _lib.stream(x.device)))
+            want[:] = st.cpu().numpy()
+            want[:, 3 * p:3 * p + 3] /= np.float64(rows)
+            st.copy_(torch.from_numpy(want))
+        return want
+
+    for A in (1, 3):
+        x = torch.as_tensor((rs.randn(rows, A) * 3 + 1e4).astype(np.float32), device="cuda")
+        y = torch.as_tensor((rs.randn(rows, A) + 1).astype(np.float32), device="cuda")
+        for b in (y, None):
+            want = passes(x, b, A)
+            assert np.array_equal(moments_agents(x, b).cpu().numpy(), want), (A, b is None)
+            if A == 1:
+                assert np.array_equal(moments(x.view(-1), None if b is None else b.view(-1)).cpu().numpy(), want[0])
 
 
 @pytest.mark.gpu

@@ -1,4 +1,4 @@
-"""rltools' sample kernels (madrl_running_moments_*, madrl_time_baseline_f32, madrl_lfbr_*), the padded-path kernels
+"""rltools' sample kernels (madrl_running_moments_*, madrl_time_baseline_*_f32, madrl_lfbr_*), the padded-path kernels
 (madrl_paths_pad_*, madrl_path_sums_f32) and the closed loop's per-step wrapper (madrl_obs_wrap_step_*) on the GPU,
 at the edges of the product build's grids: the row slices of each group (ceil(S / G) of them, S read from the
 sources), the 8-warp row stride and 32-column blocks of the running moments, the 128-bin blocks of the time
@@ -157,8 +157,8 @@ def test_time_baseline_per_agent_at_the_slice_and_bin_edges(A):
 
 
 @pytest.mark.parametrize("T", (257, 64), ids=("through_T", "through_t0"))
-def test_time_baseline_with_fewer_bins_than_indices(T):
-    """madrl_time_baseline_f32 given an L below the largest time index (257 bins' worth of rows): the rows whose
+def test_time_baseline_bins_and_apply_with_fewer_bins_than_indices(T):
+    """madrl_time_baseline_bins_f32 then _apply_f32 given an L below the largest time index (257 bins' worth of rows): the rows whose
     index is L or more get NaN, and the bins below L are those of the full call, bit for bit."""
     from madrl_b200 import _lib
     from madrl_b200._lib import _ptr
@@ -179,9 +179,10 @@ def test_time_baseline_with_fewer_bins_than_indices(T):
         s = torch.full((G, L), float("nan"), dtype=torch.float64, device=DEV)
         c = torch.full((G, L), -1, dtype=torch.int32, device=DEV)
         v = torch.zeros_like(qt)
-        _lib.check(lib.madrl_time_baseline_f32(T, E, A, int(per_agent), L, _ptr(qt), _ptr(seg_s), _ptr(n_ep),
-                                               _ptr(ep_rec), _ptr(t0t), _ptr(s), _ptr(c), _ptr(v), _ptr(ws),
-                                               _lib.stream(qt.device)))
+        _lib.check(lib.madrl_time_baseline_bins_f32(T, E, A, int(per_agent), L, _ptr(qt), _ptr(n_ep), _ptr(ep_rec),
+                                                    _ptr(t0t), _ptr(s), _ptr(c), _ptr(ws), _lib.stream(qt.device)))
+        _lib.check(lib.madrl_time_baseline_apply_f32(T, E, A, int(per_agent), L, _ptr(seg_s), _ptr(t0t), _ptr(s),
+                                                     _ptr(c), _ptr(v), _lib.stream(qt.device)))
         return v.cpu().numpy(), s.cpu().numpy(), c.cpu().numpy()
 
     for per_agent in (False, True):
