@@ -32,6 +32,13 @@ def launched(fn):
     """fn() under torch.profiler -> (its result, [(name, grid)] of the ww_kernel launches, in launch order).  The
     names are the demangled ones CUPTI reports (ww_writer_edges.writer_kernel), the grid is the launch's gridDim.x."""
     from torch.profiler import ProfilerActivity, profile
+    # By default each session tears CUPTI down at its end and the next one re-initialises it.  That re-initialisation
+    # is unreliable in a process that has captured CUDA graphs, as the closed-loop and whole-path tests that run
+    # before this file do: torch.profiler applies these two settings for its own CUDA graphs ("CUDA Graph does not
+    # work well with CUPTI teardown"), and sessions here have recorded no kernel at all without them.  CUPTI then
+    # stays initialised for the rest of the process.  setdefault: a caller's own choice stands.
+    os.environ.setdefault("DISABLE_CUPTI_LAZY_REINIT", "1")
+    os.environ.setdefault("TEARDOWN_CUPTI", "0")
     torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         out = fn()
