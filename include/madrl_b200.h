@@ -151,6 +151,12 @@ int madrl_ww_set_launch(madrl_ww* h, int warps_per_block, int blocks_per_sm);
  * one-warp blocks.  Resets, heuristic-policy and peer-exchange rollouts always use as many as fit.
  * Negative on error. */
 int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T);
+/* Which kernel each Waterworld launch ran, for tests of the launch paths.  Returns the number of ww_kernel launches
+ * (of any handle) since the previous call, copies the first min(that, max_records, 4096) records into `records`
+ * (10 int32 each: sizeof(real), sizeof(observation element), OPL, KCH, KC, PEER, POLICY, KEEP, WRITER and the
+ * launch's grid), clears the log and turns logging on (enable != 0) or off (the default).  A launch is logged when
+ * it is enqueued, or when it is recorded under stream capture.  MADRL_EINVAL if max_records > 0 and records is NULL. */
+int madrl_ww_launch_log(int enable, int32_t* records, int max_records);
 /* Observation write path of Waterworld's float32 open-loop rollouts (madrl_ww_rollout / _step / _rollout_host*).
  * The writer-warp kernel runs blocks of 8 warps that step 8 adjacent envs and stage each step's rows in shared
  * memory, plus one warp that copies those rows to the observation tensor (DESIGN §4.1).  It needs at most 32
@@ -184,7 +190,10 @@ int madrl_ww_set_obs_cache(madrl_ww* h, int mode);
  *   rew  real  [n_slots][E][t_max][Np]    done uint8 [n_slots][E][t_max]
  *   info int32 [n_slots][E][t_max][2]
  * Rows are staged in registers and written as coalesced runs.  A stream-ordered barrier between the
- * ranks after the rollout completes the gather.  n_dest = 0 disables. */
+ * ranks after the rollout completes the gather.  n_dest = 0 disables.
+ * Every launch writes steps [0, T) of the buffers, so a rollout must be one launch: the device rollout or
+ * step.  madrl_ww_rollout_host2 (and _host), which cut a rollout into chunked launches, return MADRL_EINVAL
+ * while peers are set.  madrl_ww_rollout_heuristic writes no peer rows. */
 int madrl_ww_set_peers(madrl_ww* h, int n_dest, int slot, int t_max, void* const* rew_dest,
                        void* const* done_dest, void* const* info_dest);
 
@@ -221,7 +230,8 @@ int madrl_ww_step(madrl_ww* h, const void* actions_dev, void* obs_dev, void* rew
  * queued on other streams must be synchronised by the caller.
  * `_host2` takes flags: MADRL_HOST_OBS_LAST = only the LAST step's observations come back (obs_host is
  * then [E][Np][D]) -- the policy-on-device mode: rewards / dones / infos of every step + the
- * observation needed to continue; the call then runs at the kernel's rate instead of PCIe's. */
+ * observation needed to continue; the call then runs at the kernel's rate instead of PCIe's.
+ * Waterworld's host variants return MADRL_EINVAL while madrl_ww_set_peers is set. */
 #define MADRL_HOST_OBS_LAST 1
 int madrl_ww_reset_host(madrl_ww* h, const uint8_t* mask_host, void* obs_host);
 int madrl_ww_rollout_host(madrl_ww* h, int T, const void* actions_host, void* obs_host,

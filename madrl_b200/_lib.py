@@ -149,6 +149,7 @@ def _signatures():
             ("rollout_host2", (i32, [vp, i32, vp, vp, vp, vp, vp, i32, i32]))))
     sig.update({
         "madrl_ww_default_blocks_per_sm": (i32, [vp, i32]),
+        "madrl_ww_launch_log": (i32, [i32, vp, i32]),
         "madrl_ww_set_obs_writer": (i32, [vp, i32]),
         "madrl_ww_set_heuristic_norm": (i32, [vp, i32]),
         "madrl_ww_set_peers": (i32, [vp, i32, i32, i32, P(vp), P(vp), P(vp)]),

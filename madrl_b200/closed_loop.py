@@ -71,10 +71,11 @@ class PolicyRollout(object):
     the float64 verification engines, which have no KEEP kernels (asking for KEEP there raises EngineError).
 
     The capture is redone when T, the engine, its obs dtype, its terminal-observation tensor, the state's shapes or
-    any host-side setting a launch copies into its kernel parameters changes: ``engine.seed``, ``set_launch``,
-    Pursuit's ``set_params`` (the curriculum hook), Waterworld's ``set_peers`` / ``clear_peers``
-    (``engine.launch_settings`` counts them).  So a curriculum update or a re-seed between calls takes effect as it
-    would in an eager loop.  The first call with graph=True first runs the policy twice on a side stream
+    any host-side setting a launch copies into its kernel parameters changes: ``engine.seed``, ``set_launch`` and
+    Pursuit's ``set_params`` (the curriculum hook) (``engine.launch_settings`` counts them).  So a curriculum update
+    or a re-seed between calls takes effect as it would in an eager loop.  A call raises ValueError while
+    Waterworld's ``set_peers`` is in effect: each launch of the fused peer exchange writes its rows from step 0 of
+    the gather buffers, so one-step launches would overwrite each other.  The first call with graph=True first runs the policy twice on a side stream
     (torch.cuda.graphs' warm-up: lazy library initialisation must not happen during capture); this touches no env
     state.
 
@@ -286,6 +287,9 @@ class PolicyRollout(object):
 
     def __call__(self, obs0, state0=None):
         eng = self.engine
+        if getattr(eng, "_peer_keepalive", None) is not None:
+            raise ValueError("PolicyRollout runs one launch per step, and every launch would write its peer rows "
+                             "from step 0 of the gather buffers: clear_peers() first")
         _lib.require_tensor(obs0, "obs0", eng.obs_dtype, self._obs0_shape(), eng.device, contiguous=False)
         with torch.cuda.device(eng.device):
             key = self._settings(state0)

@@ -120,10 +120,10 @@ inline int engine_set_launch(EngineCore* h, int warps_per_block, int blocks_per_
 
 // One launch of a warp-per-env kernel over E envs: one 32-thread block per env, or a single
 // persistent wave (SMs x resident blocks per SM, capped by set_launch, else by the family's
-// `default_blocks_per_sm` when that is not 0) whose warps loop over the envs.
+// `default_blocks_per_sm` when that is not 0) whose warps loop over the envs.  `grid_out`: the launch's grid.
 template <class Kernel, class Params>
 int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStream_t stream, const Params& p,
-                  int default_blocks_per_sm = 0) {
+                  int default_blocks_per_sm = 0, int* grid_out = nullptr) {
   if (smem > 48 * 1024)
     MADRL_CUDA_CHECK(cudaFuncSetAttribute(kfn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int resident = 0;
@@ -136,6 +136,7 @@ int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStrea
   MADRL_LAUNCH(kfn, grid, 32, smem, stream, p);
   g_launches.fetch_add(1);   // under stream capture: counted once, when recorded, not at each graph replay
   MADRL_CUDA_CHECK(cudaGetLastError());
+  if (grid_out != nullptr) *grid_out = grid;
   return MADRL_OK;
 }
 

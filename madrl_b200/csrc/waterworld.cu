@@ -21,7 +21,9 @@
 //     <= thr (computed on the host), which is exactly equivalent.
 //   * fp32 production instantiation and fp64 verification instantiation of the same template.
 #include <math.h>
+#include <atomic>
 #include <cmath>
+#include <mutex>
 #include <new>
 #include <type_traits>
 
@@ -984,11 +986,47 @@ extern "C" int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T) {
   return ww_default_blocks_per_sm(h, T);
 }
 
+// The launch log (madrl_ww_launch_log): while it is on, every ww_kernel launch appends the template arguments of the
+// instantiation it ran and its grid, so that a test can check which kernel a launch path takes without a profiler.
+// Off, the default, it costs one relaxed load per launch.
+constexpr int kWwLogFields = 10, kWwLogMax = 4096;
+static std::atomic<bool> g_ww_log_on{false};
+static std::mutex g_ww_log_mu;
+static int32_t g_ww_log[kWwLogMax][kWwLogFields];
+static int g_ww_log_n = 0;   // launches since the log was last read, including those past kWwLogMax
+
+template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY, bool KEEP, bool WRITER>
+static void ww_log_launch(int grid) {
+  if (!g_ww_log_on.load(std::memory_order_relaxed)) return;
+  std::lock_guard<std::mutex> lock(g_ww_log_mu);
+  if (g_ww_log_n < kWwLogMax) {
+    const int32_t rec[kWwLogFields] = {(int32_t)sizeof(real), (int32_t)sizeof(O), OPL, KCH, KC, PEER, POLICY, KEEP,
+                                       WRITER, grid};
+    for (int i = 0; i < kWwLogFields; ++i) g_ww_log[g_ww_log_n][i] = rec[i];
+  }
+  ++g_ww_log_n;
+}
+
+extern "C" int madrl_ww_launch_log(int enable, int32_t* records, int max_records) {
+  MADRL_REQUIRE(max_records >= 0 && (max_records == 0 || records != nullptr), "bad launch-log buffer");
+  std::lock_guard<std::mutex> lock(g_ww_log_mu);
+  const int n = g_ww_log_n;
+  const int keep = n < kWwLogMax ? n : kWwLogMax;
+  for (int r = 0; r < keep && r < max_records; ++r)
+    for (int i = 0; i < kWwLogFields; ++i) records[r * kWwLogFields + i] = g_ww_log[r][i];
+  g_ww_log_n = 0;
+  g_ww_log_on.store(enable != 0, std::memory_order_relaxed);
+  return n;
+}
+
 template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY, bool KEEP = false>
 static int ww_launch_inst2(madrl_ww* h, const WWParams<real, O>& p, int cap, cudaStream_t stream) {
   const size_t smem = ww_cand_bytes<real>(OPL, p.Nall) + (p.stage_step ? obs_stage_bytes(p.Np * p.D, sizeof(O))
                                                                         : 2 * obs_stage_bytes(p.K * (p.speed_features ? 7 : 4), sizeof(O)));
-  return engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY, KEEP>, smem, p.E, stream, p, cap);
+  int grid = 0;
+  const int rc = engine_launch(h, ww_kernel<real, O, OPL, KCH, KC, PEER, POLICY, KEEP>, smem, p.E, stream, p, cap, &grid);
+  if (rc == MADRL_OK) ww_log_launch<real, O, OPL, KCH, KC, PEER, POLICY, KEEP, false>(grid);
+  return rc;
 }
 
 // Whether a plain open-loop float32 rollout (no policy, peers or KEEP) of at most 32 objects runs on the writer-warp
@@ -1018,6 +1056,7 @@ static int ww_launch_writer(madrl_ww* h, const WWParams<float, float>& p, cudaSt
   MADRL_LAUNCH(kfn, grid, kWrThreads, smem, stream, p);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
+  ww_log_launch<float, float, OPL, KCH, KC, false, 0, false, true>(grid);
   return MADRL_OK;
 }
 
@@ -1177,6 +1216,11 @@ extern "C" int madrl_ww_reset_host(madrl_ww* h, const uint8_t* mask_host, void* 
 extern "C" int madrl_ww_rollout_host2(madrl_ww* h, int T, const void* actions_host, void* obs_host,
                                       void* rew_host, uint8_t* done_host, int32_t* info_host,
                                       int auto_reset, int flags) {
+  // Each chunk is a launch of its own, and a launch writes its peer rows from step 0 of the gather buffers.
+  // Refused whatever the chunk count, which depends on the buffer sizes (madrl_set_host_chunk_bytes).
+  MADRL_REQUIRE(h == nullptr || h->n_peers == 0,
+                "the host-buffer rollout runs in chunked launches, which the fused peer exchange does not support: "
+                "clear set_peers first");
   return engine_rollout_host(h, T, actions_host, obs_host, rew_host, done_host, info_host, flags,
                              [&](int Tc, char* a, char* o, char* r, char* d, char* i, cudaStream_t st) {
                                return madrl_ww_rollout(h, Tc, a, o, r, (uint8_t*)d, (int32_t*)i, auto_reset, st);

@@ -112,8 +112,25 @@ class BatchedMAWaterWorld(BatchedEngine):
     def set_peers(self, rank, t_max, rew_peers, done_peers, info_peers):
         """Enable the fused exchange: `*_peers` are lists (one per DESTINATION rank) of tensors
         aliasing the destination gather buffers; this rank writes slot `rank` of each
-        (see madrl_b200.dist.PeerGather)."""
+        (see madrl_b200.dist.PeerGather).  Each destination is contiguous on the engine's device, with S > rank
+        slots: rewards (S, E, t_max, Np) of the engine's dtype, dones (S, E, t_max) uint8 and infos
+        (S, E, t_max, 2) int32.  Every rollout must then be one launch: rollout() or step().  rollout_host and
+        PolicyRollout, which run a rollout as several launches, refuse to run while peers are set."""
         n = len(rew_peers)
+        if not 1 <= n <= 8 or len(done_peers) != n or len(info_peers) != n:
+            raise ValueError("set_peers needs 1 to 8 destinations and as many reward, done and info buffers, got "
+                             "%d, %d and %d" % (n, len(done_peers), len(info_peers)))
+        rank, t_max = int(rank), int(t_max)
+        if rank < 0 or t_max < 1:
+            raise ValueError("set_peers needs rank >= 0 and t_max >= 1, got %d and %d" % (rank, t_max))
+        E, Np = self.n_envs, self.n_pursuers
+        for d in range(n):
+            for t, name, dt, tail in ((rew_peers[d], "rew_peers", self.dtype, (Np,)),
+                                      (done_peers[d], "done_peers", torch.uint8, ()),
+                                      (info_peers[d], "info_peers", torch.int32, (2,))):
+                _lib.require_tensor(t, "%s[%d]" % (name, d), dt, (None, E, t_max) + tail, self.device)
+                if t.shape[0] <= rank:
+                    raise ValueError("%s[%d] has %d slots, rank %d writes slot %d" % (name, d, t.shape[0], rank, rank))
         arr = lambda ts: (C.c_void_p * n)(*[t.data_ptr() for t in ts])
         self._peer_keepalive = (rew_peers, done_peers, info_peers)
         _lib.check(self._L.madrl_ww_set_peers(self._h, n, rank, t_max, arr(rew_peers), arr(done_peers),

@@ -618,6 +618,107 @@ def test_waterworld_fused_peer_gather_layout(variant):
             assert np.isnan(d['rew'][rank, :, T:]).all() and (d['done'][rank, :, T:] == 255).all()
 
 
+def _peer_dests(n_dest, n_slots, E, t_max, Np):
+    """Destination gather buffers filled with sentinels, and the ctypes pointer tables of set_peers."""
+    import ctypes as C
+    dests = [dict(rew=np.full((n_slots, E, t_max, Np), np.nan), done=np.full((n_slots, E, t_max), 255, np.uint8),
+                  info=np.full((n_slots, E, t_max, 2), -1, np.int32)) for _ in range(n_dest)]
+    return dests, lambda k: (C.c_void_p * n_dest)(*[d[k].ctypes.data for d in dests])
+
+
+@pytest.mark.parametrize("name,T,mpl", [("minimum", 1, 0), ("minimum", 33, 11), ("np32_k64", 1, 1)])
+def test_waterworld_fused_peer_gather_edge_shapes(name, T, mpl):
+    """The peer rows at the staging edges: one pursuer (32-step reward runs: T = 1 is a partial run of one step,
+    T = 33 a full run and a partial one, with a reset on the last step) and 32 pursuers (one step per run).  Two
+    ranks of 3 envs each write slot `rank` of a 3-slot buffer; the emulated grid has 2 warps, so one warp steps two
+    envs.  The rows equal an unsharded rollout of all 6 envs without peers, and the rest stays as it was."""
+    from emu.driver import EmuWaterworld
+    cfg = WW[name]
+    Np, E, W, t_max = cfg["n_pursuers"], 3, 2, T + 3
+    dests, arr = _peer_dests(2, W + 1, E, t_max, Np)
+    act = np.random.RandomState(T).randn(T, W * E, Np, 2) * 0.6
+    ref = EmuWaterworld(W * E, seed=6, max_path_length=mpl, **cfg)
+    ref.reset()
+    want = ref.rollout(act, auto_reset=mpl > 0)
+    for rank in range(W):
+        eng = EmuWaterworld(E, seed=6, env_id_base=rank * E, max_path_length=mpl, **cfg)
+        assert eng.lib.madrl_ww_set_peers(eng._h, 2, rank, t_max, arr('rew'), arr('done'), arr('info')) == 0
+        eng.reset()
+        got = eng.rollout(act[:, rank * E:(rank + 1) * E], auto_reset=mpl > 0)
+        for x, y in zip(got, want):
+            assert np.array_equal(x, y[:, rank * E:(rank + 1) * E])
+    for d in dests:
+        for rank in range(W):
+            s = slice(rank * E, (rank + 1) * E)
+            assert np.array_equal(d['rew'][rank, :, :T], want[1][:, s].transpose(1, 0, 2))
+            assert np.array_equal(d['done'][rank, :, :T], want[2][:, s].T)
+            assert np.array_equal(d['info'][rank, :, :T], want[3][:, s].transpose(1, 0, 2))
+        assert np.isnan(d['rew'][:, :, T:]).all() and (d['done'][:, :, T:] == 255).all() and (d['info'][:, :, T:] == -1).all()
+        assert np.isnan(d['rew'][W:]).all() and (d['done'][W:] == 255).all() and (d['info'][W:] == -1).all()
+
+
+def test_waterworld_launch_log():
+    """madrl_ww_launch_log records each launch's instantiation and grid while it is on, counts launches past the
+    buffer it is given, and records nothing while it is off."""
+    from emu.driver import EmuWaterworld
+    eng = EmuWaterworld(3, seed=4, **WW["c2"])
+    lib, recs = eng.lib, np.full((4, 10), -9, np.int32)
+    assert lib.madrl_ww_launch_log(1, None, 0) >= 0
+    eng.reset()
+    act = np.zeros((2, 3, 5, 2))
+    eng.rollout(act)
+    dests, arr = _peer_dests(1, 1, 3, 2, 5)
+    assert lib.madrl_ww_set_peers(eng._h, 1, 0, 2, arr('rew'), arr('done'), arr('info')) == 0
+    eng.rollout(act)
+    assert lib.madrl_ww_launch_log(1, _p(recs), 2) == 3
+    # fp64, OPL 1, compile-time K = 30; the emulated device has 2 SMs with one resident block each
+    assert recs[:2].tolist() == [[8, 8, 1, 1, 30, 0, 0, 0, 0, 2]] * 2 and (recs[2:] == -9).all()
+    eng.rollout(act)
+    assert lib.madrl_ww_launch_log(0, _p(recs), 4) == 1 and recs[0].tolist() == [8, 8, 1, 1, 30, 1, 0, 0, 0, 2]
+    eng.rollout(act)
+    assert lib.madrl_ww_launch_log(0, None, 0) == 0
+    assert lib.madrl_ww_launch_log(0, None, 1) == -1
+
+
+def test_waterworld_peer_exchange_refuses_host_rollout():
+    """The host-buffer rollout cuts a rollout into chunked launches, and each launch would write its peer rows from
+    step 0 of the gather buffers.  With peers set it is refused, with one chunk or several, and writes nothing; once
+    the peers are cleared it runs again."""
+    from emu.driver import EmuWaterworld
+    cfg = WW["c2"]
+    E, T, Np = 3, 13, 5
+    eng = EmuWaterworld(E, seed=4, max_path_length=7, fp64=False, **cfg)
+    eng.reset()
+    dests, arr = _peer_dests(1, 1, E, T, Np)
+    for d in dests:
+        d['rew'] = d['rew'].astype(np.float32)
+    assert eng.lib.madrl_ww_set_peers(eng._h, 1, 0, T, arr('rew'), arr('done'), arr('info')) == 0
+    act = np.ascontiguousarray(np.random.RandomState(2).randn(T, E, Np, 2).astype(np.float32))
+    f = eng.lib.madrl_ww_rollout_host2
+    step_bytes = E * Np * eng.obs_dim * 4
+    try:
+        for chunk in (0, 3 * step_bytes):                 # one chunk (the default size), ~3 steps per chunk
+            eng.lib.madrl_set_host_chunk_bytes(chunk)
+            for host in (f, eng.lib.madrl_ww_rollout_host):
+                bufs = [Guarded((T, E, Np, eng.obs_dim), np.float32, np.nan), Guarded((T, E, Np), np.float32, np.nan),
+                        Guarded((T, E), np.uint8, 255), Guarded((T, E, 2), np.int32, -1)]
+                args = (eng._h, T, _p(act), *[_p(b.arr) for b in bufs], 1) + ((0,) if host is f else ())
+                assert host(*args) == -1
+                assert b"set_peers" in eng.lib.madrl_last_error()
+                assert all(np.isnan(b.check("host").astype(np.float64)).all() for b in bufs[:2])
+                assert (bufs[2].arr == 255).all() and (bufs[3].arr == -1).all()
+        d = dests[0]
+        assert np.isnan(d['rew']).all() and (d['done'] == 255).all() and (d['info'] == -1).all()
+        assert eng.lib.madrl_ww_set_peers(eng._h, 0, 0, 0, None, None, None) == 0
+        ref = EmuWaterworld(E, seed=4, max_path_length=7, fp64=False, **cfg)
+        ref.reset()
+        for x, y in zip(eng.rollout(act, host=True), ref.rollout(act)):
+            assert np.array_equal(x, y)
+        assert np.isnan(d['rew']).all() and (d['done'] == 255).all() and (d['info'] == -1).all()
+    finally:
+        eng.lib.madrl_set_host_chunk_bytes(0)
+
+
 def _vec_executor_check(eng, oracles, act, mpl, exact, info_of):
     """VecEnvExecutor.step semantics (vec_env_executor.py:16-28) against per-env oracles: done at the
     env's own terminal state or at max_path_length, reset in place, obs slot = reset observation."""

@@ -1,5 +1,5 @@
-"""Fused NVLink peer-memory exchange (needs >= 2 GPUs; skipped on the single-GPU test box):
-the gather buffers every rank ends up with must equal the stacked per-rank rollouts."""
+"""Fused NVLink peer-memory exchange (needs >= 2 GPUs): the gather buffers every rank ends up with must equal the
+stacked per-rank rollouts.  tests/test_peer_exchange_edges_gpu.py runs the same worker as a one-rank group."""
 import os
 import socket
 
@@ -71,7 +71,8 @@ def _worker(rank, world, port, q):
                 got = ag.result(k)
                 if rank == 0:
                     ok = ok and torch.equal(got.reshape(-1), ref) and torch.equal(seen[-1].reshape(-1), ref)
-                    ok = ok and torch.equal(pk.view_of(got[1], 'obs'), pk.view_of(ref.view(world, -1)[1], 'obs'))
+                    last = world - 1               # the last rank's slot (rank 1 with two ranks)
+                    ok = ok and torch.equal(pk.view_of(got[last], 'obs'), pk.view_of(ref.view(world, -1)[last], 'obs'))
                 else:
                     ok = ok and got is None and not seen
             ag.close()

@@ -2,14 +2,10 @@
 (needs a GPU).  The cases are tests/ww_writer_edges.py's table.
 
 Every comparison of the writer with the one-warp kernel (set_obs_writer ON against OFF, bit for bit) also asserts,
-from the kernels torch.profiler records, which kernel each launch ran: were ww_use_writer to refuse the writer, ON
-would compare the one-warp kernel with itself.  The writer's float32 observations are checked against the float64
+from the library's launch log (madrl_ww_launch_log), which kernel each launch ran: were ww_use_writer to refuse the
+writer, ON would compare the one-warp kernel with itself.  The writer's float32 observations are checked against the float64
 oracle by teacher forcing, one writer launch per step, and the fp64 build checks each case's configuration against
 the oracle over whole trajectories."""
-import json
-import os
-import tempfile
-
 import numpy as np
 import pytest
 import torch
@@ -29,29 +25,24 @@ EDGE_CASES = [W.BY_NAME["c2"], W.BY_NAME["k64_plain"]]
 
 # ------------------------------------------------------------------------------------------------ kernel identity
 def launched(fn):
-    """fn() under torch.profiler -> (its result, [(name, grid)] of the ww_kernel launches, in launch order).  The
-    names are the demangled ones CUPTI reports (ww_writer_edges.writer_kernel), the grid is the launch's gridDim.x."""
-    from torch.profiler import ProfilerActivity, profile
-    # By default each session tears CUPTI down at its end and the next one re-initialises it.  That re-initialisation
-    # is unreliable in a process that has captured CUDA graphs, as the closed-loop and whole-path tests that run
-    # before this file do: torch.profiler applies these two settings for its own CUDA graphs ("CUDA Graph does not
-    # work well with CUPTI teardown"), and sessions here have recorded no kernel at all without them.  CUPTI then
-    # stays initialised for the rest of the process.  setdefault: a caller's own choice stands.
-    os.environ.setdefault("DISABLE_CUPTI_LAZY_REINIT", "1")
-    os.environ.setdefault("TEARDOWN_CUPTI", "0")
-    torch.cuda.synchronize()
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    """fn() with the library's launch log on -> (its result, [(name, grid)] of the ww_kernel launches, in launch order).
+    madrl_ww_launch_log records the template arguments of the instantiation each launch ran and its gridDim.x, as the
+    launch code passes them to the kernel; they are spelled as the demangled kernel name (ww_writer_edges.writer_kernel).
+    The log is read on the host, so unlike a profiler session it cannot lose a launch."""
+    L, fields, most = _lib.lib(), 10, 4096
+    assert L.madrl_ww_launch_log(1, None, 0) >= 0
+    try:
         out = fn()
-        torch.cuda.synchronize()
-    with tempfile.TemporaryDirectory() as d:
-        path = os.path.join(d, "trace.json")
-        prof.export_chrome_trace(path)
-        with open(path) as f:
-            events = json.load(f)["traceEvents"]
-    kernels = sorted((e["ts"], e["name"], int(e.get("args", {}).get("grid", [0])[0]))
-                     for e in events if e.get("cat") == "kernel")
-    assert kernels, "torch.profiler recorded no CUDA kernel: the kernel-identity checks cannot run (is CUPTI loadable?)"
-    return out, [(n, g) for _, n, g in kernels if W.is_ww_kernel(n)]
+    finally:
+        recs = np.zeros((most, fields), np.int32)
+        n = L.madrl_ww_launch_log(0, recs.ctypes.data, most)
+    assert 0 <= n <= most, n
+    real = {4: "float", 8: "double"}
+    obs = {2: "unsigned short", 4: "float", 8: "double"}
+    flag = ("false", "true")
+    return out, [("void madrl::ww_kernel<%s, %s, %d, %d, %d, %s, %d, %s, %s>(madrl::WWParams<%s, %s>)" % (
+        real[r], obs[o], opl, kch, kc, flag[peer], policy, flag[keep], flag[writer], real[r], obs[o]), int(grid))
+        for r, o, opl, kch, kc, peer, policy, keep, writer, grid in recs[:n].tolist()]
 
 
 def assert_writer(kernels, case, n=None):
@@ -187,8 +178,8 @@ def test_other_paths_never_take_writer():
         if callable(setup):
             setup(eng)
         if setup == "peers":
-            keep = ([torch.zeros(E * T * 5, device="cuda")], [torch.zeros(E * T, dtype=torch.uint8, device="cuda")],
-                    [torch.zeros(E * T * 2, dtype=torch.int32, device="cuda")])
+            keep = ([torch.zeros(1, E, T, 5, device="cuda")], [torch.zeros(1, E, T, dtype=torch.uint8, device="cuda")],
+                    [torch.zeros(1, E, T, 2, dtype=torch.int32, device="cuda")])
             eng.set_peers(0, T, *keep)
         if setup == "heuristic":
             _, k = launched(lambda: eng.rollout_heuristic(T, obs0))

@@ -86,8 +86,8 @@ assert BY_NAME["stage_max"].Np * BY_NAME["stage_max"].D <= STAGE_MAX_FLOATS < \
 
 
 def writer_kernel(case):
-    """The kernel name torch.profiler reports (CUPTI's demangling, as an H100 shows it) for the writer-warp kernel a
-    launch of `case` runs."""
+    """The demangled name of the writer-warp kernel a launch of `case` runs (as CUPTI spells it on an H100, and as
+    the GPU tests spell the records of madrl_ww_launch_log)."""
     return "void madrl::ww_kernel<float, float, 1, %d, %d, false, 0, false, true>(madrl::WWParams<float, float>)" % (
         case.kch, case.kc)
 
