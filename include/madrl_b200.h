@@ -284,6 +284,9 @@ int madrl_pursuit_destroy(madrl_pursuit* h);
 void* madrl_pursuit_state_ptr(madrl_pursuit* h);
 int madrl_pursuit_seed(madrl_pursuit* h, uint64_t seed, void* stream);
 int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_per_sm);
+/* Which kernel each Pursuit launch ran: madrl_ww_launch_log's contract for pe_kernel launches, with records of 8
+ * int32: sizeof(observation element), EPL, CPL, RC, POLICY, FLAT, KEEP and the launch's grid. */
+int madrl_pursuit_launch_log(int enable, int32_t* records, int max_records);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
  * terminal one.  After this call every `*_rollout` (device pointers) with auto_reset first copies the rows
@@ -360,6 +363,9 @@ int madrl_hostage_destroy(madrl_hostage* h);
 void* madrl_hostage_state_ptr(madrl_hostage* h);
 int madrl_hostage_seed(madrl_hostage* h, uint64_t seed, void* stream);
 int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, int blocks_per_sm);
+/* Which kernel each Hostage launch ran: madrl_ww_launch_log's contract for hw_kernel launches, with records of 7
+ * int32: sizeof(real), sizeof(observation element), OPL, KCH, KC, KEEP and the launch's grid. */
+int madrl_hostage_launch_log(int enable, int32_t* records, int max_records);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
  * terminal one.  After this call every `*_rollout` (device pointers) with auto_reset first copies the rows

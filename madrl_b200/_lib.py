@@ -154,6 +154,8 @@ def _signatures():
         "madrl_ww_set_heuristic_norm": (i32, [vp, i32]),
         "madrl_ww_set_peers": (i32, [vp, i32, i32, i32, P(vp), P(vp), P(vp)]),
         "madrl_ww_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, vp]),
+        "madrl_pursuit_launch_log": (i32, [i32, vp, i32]),
+        "madrl_hostage_launch_log": (i32, [i32, vp, i32]),
         "madrl_pursuit_set_params": (i32, [vp, f64, f64]),
         "madrl_pursuit_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
         # hand-written policies

@@ -7,6 +7,7 @@
 #pragma once
 #include <math.h>
 #include <cmath>
+#include <mutex>
 #include <new>
 
 #include "common.cuh"
@@ -139,6 +140,39 @@ int engine_launch(const EngineCore* h, Kernel kfn, size_t smem, int E, cudaStrea
   if (grid_out != nullptr) *grid_out = grid;
   return MADRL_OK;
 }
+
+// A family's launch log (madrl_ww_launch_log, madrl_pursuit_launch_log, madrl_hostage_launch_log): while it is on,
+// every launch of the family's kernel appends the template arguments of the instantiation it ran and its grid, so
+// that a test can check which kernel a launch path takes without a profiler.  Off, the default, it costs one
+// relaxed load per launch.  `Fields` int32 per record.
+template <int Fields>
+struct LaunchLog {
+  static constexpr int kMax = 4096;
+  std::atomic<bool> on{false};
+  std::mutex mu;
+  int32_t recs[kMax][Fields];
+  int n = 0;   // launches since the log was last read, including those past kMax
+
+  void add(const int32_t (&rec)[Fields]) {
+    if (!on.load(std::memory_order_relaxed)) return;
+    std::lock_guard<std::mutex> lock(mu);
+    if (n < kMax)
+      for (int i = 0; i < Fields; ++i) recs[n][i] = rec[i];
+    ++n;
+  }
+
+  // Copies the first min(n, max_records, kMax) records out, clears the log and turns it on or off -> n.
+  int read(int enable, int32_t* records, int max_records) {
+    MADRL_REQUIRE(max_records >= 0 && (max_records == 0 || records != nullptr), "bad launch-log buffer");
+    std::lock_guard<std::mutex> lock(mu);
+    const int got = n, keep = n < kMax ? n : kMax;
+    for (int r = 0; r < keep && r < max_records; ++r)
+      for (int i = 0; i < Fields; ++i) records[r * Fields + i] = recs[r][i];
+    n = 0;
+    on.store(enable != 0, std::memory_order_relaxed);
+    return got;
+  }
+};
 
 // `*_reset_host`: `reset(mask_dev, obs_dev)` is the family's device-pointer reset on the legacy default
 // stream; the mask and the observations go through the staging buffer.

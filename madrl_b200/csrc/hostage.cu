@@ -490,12 +490,27 @@ extern "C" int madrl_hostage_set_launch(madrl_hostage* h, int warps_per_block, i
   return engine_set_launch(h, warps_per_block, blocks_per_sm);
 }
 
+// The launch log (madrl_hostage_launch_log, see LaunchLog): one record per hw_kernel launch.
+static LaunchLog<7> g_hw_log;
+
+extern "C" int madrl_hostage_launch_log(int enable, int32_t* records, int max_records) {
+  return g_hw_log.read(enable, records, max_records);
+}
+
+template <typename real, typename O, int OPL, int KCH, int KC, bool KEEP>
+static int hw_launch_kernel(madrl_hostage* h, const HWParams<real, O>& p, cudaStream_t stream) {
+  int grid = 0;
+  const int rc = engine_launch(h, hw_kernel<real, O, OPL, KCH, KC, KEEP>, 0, p.E, stream, p, 0, &grid);
+  if (rc == MADRL_OK) g_hw_log.add({(int32_t)sizeof(real), (int32_t)sizeof(O), OPL, KCH, KC, KEEP, grid});
+  return rc;
+}
+
 template <typename real, typename O, int OPL, int KCH, int KC>
 static int hw_launch_inst(madrl_hostage* h, const HWParams<real, O>& p, cudaStream_t stream) {
   if constexpr (sizeof(real) == 4)   // set_obs_cache refuses KEEP on fp64 handles
     if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
-      return engine_launch(h, hw_kernel<real, O, OPL, KCH, KC, true>, 0, p.E, stream, p);
-  return engine_launch(h, hw_kernel<real, O, OPL, KCH, KC>, 0, p.E, stream, p);
+      return hw_launch_kernel<real, O, OPL, KCH, KC, true>(h, p, stream);
+  return hw_launch_kernel<real, O, OPL, KCH, KC, false>(h, p, stream);
 }
 
 template <typename real, typename O>

@@ -669,14 +669,29 @@ void pe_policy_table(int R, int c2, uint8_t* lut) {
   }
 }
 
+// The launch log (madrl_pursuit_launch_log, see LaunchLog): one record per pe_kernel launch.
+static LaunchLog<8> g_pe_log;
+
+extern "C" int madrl_pursuit_launch_log(int enable, int32_t* records, int max_records) {
+  return g_pe_log.read(enable, records, max_records);
+}
+
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP>
+static int pe_launch_kernel(madrl_pursuit* h, PEParams<O>& p, size_t smem, cudaStream_t stream) {
+  int grid = 0;
+  const int rc = engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT, KEEP>, smem, p.E, stream, p, 0, &grid);
+  if (rc == MADRL_OK) g_pe_log.add({(int32_t)sizeof(O), EPL, CPL, RC, POLICY, FLAT, KEEP, grid});
+  return rc;
+}
+
 template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
 static int pe_launch_inst3(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)p.smem_per_warp;   // block LUT + per-warp regions
   MADRL_REQUIRE(smem <= 200 * 1024, "map too large for shared memory (%zu B per block)", smem);
   if constexpr (!POLICY)   // the heuristic-policy rollouts always stream
     if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
-      return engine_launch(h, pe_kernel<O, EPL, CPL, RC, false, FLAT, true>, smem, p.E, stream, p);
-  return engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT>, smem, p.E, stream, p);
+      return pe_launch_kernel<O, EPL, CPL, RC, false, FLAT, true>(h, p, smem, stream);
+  return pe_launch_kernel<O, EPL, CPL, RC, POLICY, FLAT, false>(h, p, smem, stream);
 }
 
 template <typename O, int EPL, int CPL, int RC, bool POLICY>

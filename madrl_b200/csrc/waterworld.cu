@@ -986,37 +986,16 @@ extern "C" int madrl_ww_default_blocks_per_sm(madrl_ww* h, int T) {
   return ww_default_blocks_per_sm(h, T);
 }
 
-// The launch log (madrl_ww_launch_log): while it is on, every ww_kernel launch appends the template arguments of the
-// instantiation it ran and its grid, so that a test can check which kernel a launch path takes without a profiler.
-// Off, the default, it costs one relaxed load per launch.
-constexpr int kWwLogFields = 10, kWwLogMax = 4096;
-static std::atomic<bool> g_ww_log_on{false};
-static std::mutex g_ww_log_mu;
-static int32_t g_ww_log[kWwLogMax][kWwLogFields];
-static int g_ww_log_n = 0;   // launches since the log was last read, including those past kWwLogMax
+// The launch log (madrl_ww_launch_log, see LaunchLog): one record per ww_kernel launch.
+static LaunchLog<10> g_ww_log;
 
 template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY, bool KEEP, bool WRITER>
 static void ww_log_launch(int grid) {
-  if (!g_ww_log_on.load(std::memory_order_relaxed)) return;
-  std::lock_guard<std::mutex> lock(g_ww_log_mu);
-  if (g_ww_log_n < kWwLogMax) {
-    const int32_t rec[kWwLogFields] = {(int32_t)sizeof(real), (int32_t)sizeof(O), OPL, KCH, KC, PEER, POLICY, KEEP,
-                                       WRITER, grid};
-    for (int i = 0; i < kWwLogFields; ++i) g_ww_log[g_ww_log_n][i] = rec[i];
-  }
-  ++g_ww_log_n;
+  g_ww_log.add({(int32_t)sizeof(real), (int32_t)sizeof(O), OPL, KCH, KC, PEER, POLICY, KEEP, WRITER, grid});
 }
 
 extern "C" int madrl_ww_launch_log(int enable, int32_t* records, int max_records) {
-  MADRL_REQUIRE(max_records >= 0 && (max_records == 0 || records != nullptr), "bad launch-log buffer");
-  std::lock_guard<std::mutex> lock(g_ww_log_mu);
-  const int n = g_ww_log_n;
-  const int keep = n < kWwLogMax ? n : kWwLogMax;
-  for (int r = 0; r < keep && r < max_records; ++r)
-    for (int i = 0; i < kWwLogFields; ++i) records[r * kWwLogFields + i] = g_ww_log[r][i];
-  g_ww_log_n = 0;
-  g_ww_log_on.store(enable != 0, std::memory_order_relaxed);
-  return n;
+  return g_ww_log.read(enable, records, max_records);
 }
 
 template <typename real, typename O, int OPL, int KCH, int KC, bool PEER, int POLICY, bool KEEP = false>
