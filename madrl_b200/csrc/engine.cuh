@@ -216,16 +216,25 @@ int engine_rollout_host(H* h, int T, const void* act_h, void* obs_h, void* rew_h
   return rc;
 }
 
-// Largest representable t with correctly-rounded sqrt(t) <= thr: `sqrt(d2) <= thr` (what
-// scipy's cdist + `<=` computes in the reference) is then exactly `d2 <= t`.
+// Largest representable t with the double sqrt(t) <= thr_d: for a `real` d2, `sqrt(d2) <= thr_d` (what scipy's
+// cdist + `<=` computes in the reference, in double) is then exactly `d2 <= t`.  The search is in double against
+// the double threshold: a float sqrtf(t) against (float)thr_d rounds twice and admits up to two ulps more.
 template <typename real>
 real exact_sq_threshold(double thr_d) {
-  const real thr = (real)thr_d;
-  real t = thr * thr;
+  real t = (real)(thr_d * thr_d);
   const real up = (real)INFINITY, dn = -(real)INFINITY;
-  while (std::sqrt(t) <= thr) t = std::nextafter(t, up);
-  while (std::sqrt(t) > thr) t = std::nextafter(t, dn);
+  while (std::sqrt((double)t) <= thr_d) t = std::nextafter(t, up);
+  while (std::sqrt((double)t) > thr_d) t = std::nextafter(t, dn);
   return t;
+}
+
+// The largest `real` at or below thr_d: for a `real` x, `x > round_down(thr_d)` is exactly `x > thr_d` (and `<=`
+// likewise), the comparison the reference makes in double.  Rounding to nearest can land above thr_d
+// ((float)0.2 = 0.20000000298), and an operand equal to it would then be sensed where the reference rejects it.
+template <typename real>
+real round_down(double thr_d) {
+  const real t = (real)thr_d;
+  return (double)t > thr_d ? std::nextafter(t, -(real)INFINITY) : t;
 }
 
 // Sensor unit vectors of the continuous families (Waterworld, Hostage): angles = linspace(0, 2pi, K+1)[:-1]

@@ -525,8 +525,9 @@ static int hw_launch_t(madrl_hostage* h, int mode, int T, const void* actions, v
   p.T = T; p.mode = mode; p.auto_reset = auto_reset;
   p.obs_step = (size_t)p.E * p.Nr * p.D; p.agent_step = (size_t)p.E * p.Nr;
   const double r = c.radius;                         // rescuers & criminals; hostages 2r (hw:111-120)
-  p.r_r2 = (real)(r * r);
-  p.range = (real)c.sensor_range;
+  // the sensing thresholds rounded down, so that `x > thr` of a `real` x decides as the reference's double test
+  p.r_r2 = round_down<real>(r * r);
+  p.range = round_down<real>(c.sensor_range);
   p.cull2 = (real)((c.sensor_range * c.sensor_range + r * r) * (1.0 + 1e-4) + 1e-12);
   p.coll2_c = exact_sq_threshold<real>(r + r);
   p.coll2_h = exact_sq_threshold<real>(r + r * 2);

@@ -79,14 +79,13 @@ struct WWParams {
   int32_t* peer_info[8];
 };
 
-// 0 <= sv < best for best > 0, in one comparison for float: non-negative floats order like their bit patterns
-// and every negative one has the sign bit set, i.e. compares above any positive `best` as an unsigned integer.
-// Unlike the reference's `sv < 0` test, the float form also rejects sv = -0.0.  sx * jx + sy * jy is -0.0 when
-// the candidate sits exactly at the pursuer's position (jx = jy = +0) and neither sensor component is positive,
-// which happens when pursuers are clipped into the same corner.  Only the OPL >= 2 candidate-slot path uses it;
-// the OPL == 1 walk tests `!(sv < 0)` and matches the reference there.
-__device__ __forceinline__ bool in_zero_to(float sv, float best) { return __float_as_uint(sv) < __float_as_uint(best); }
-__device__ __forceinline__ bool in_zero_to(double sv, double best) { return !(sv < 0.0) && sv < best; }
+// 0 <= sv < best, zeros of both signs included, as the reference's `sv < 0` rejection leaves it: sx * jx + sy * jy
+// is -0.0 when the candidate sits exactly at the pursuer's position (jx = jy = +0) and neither sensor component is
+// positive, which happens when pursuers are clipped into the same corner, and the reference senses it there.  The
+// strict `<` keeps the first index among equal values (np.argmin), -0.0 against +0.0 included.  (A one-comparison
+// unsigned test of the bit patterns rejects -0.0, and once best = -0.0 would let a later +0.0 win.)
+template <typename real>
+__device__ __forceinline__ bool in_zero_to(real sv, real best) { return !(sv < (real)0) && sv < best; }
 
 template <typename real>
 struct Spawn { real x, y, vx, vy; uint64_t ctr; };
@@ -626,7 +625,7 @@ ww_kernel(const __grid_constant__ WWParams<real, O> p) {
               for (int kc = 0; kc < KCH; ++kc) {
                 const real sv = sx_l[kc] * jx + sy_l[kc] * jy;
                 // ww:64-72: 0 <= sv (<= range, through the initial best) and within the pursuer's radius of the ray.
-                // `!(sv < 0)` as in the reference, not in_zero_to: a candidate exactly at the pursuer's position
+                // `!(sv < 0)` as in the reference (and in_zero_to): a candidate exactly at the pursuer's position
                 // (pursuers clipped into the same corner) gives sv = -0.0 for sensors with no positive component,
                 // and the reference senses it at distance 0.
                 const bool ok = !(sv < (real)0) & !(jd - sv * sv > p.r_p2);
@@ -1076,8 +1075,9 @@ static int ww_launch_t(madrl_ww* h, int mode, int T, const void* actions, void* 
   p.obs_step = (size_t)p.E * p.Np * p.D; p.agent_step = (size_t)p.E * p.Np;
   // radii ww:108-118 (double arithmetic as in the reference, then narrowed once)
   const double r_p = c.radius, r_e = c.radius * 2, r_po = c.radius * 3 / 4;
-  p.r_p2 = (real)(r_p * r_p);
-  p.range = (real)c.sensor_range;
+  // the sensing thresholds rounded down, so that `x > thr` of a `real` x decides as the reference's double test
+  p.r_p2 = round_down<real>(r_p * r_p);
+  p.range = round_down<real>(c.sensor_range);
   p.range_up = std::nextafter(p.range, (real)INFINITY);
   // Exact conservative cull: sv <= range and d2 - sv^2 <= r^2 imply d2 <= range^2 + r^2.
   p.cull2 = (real)((c.sensor_range * c.sensor_range + r_p * r_p) * (1.0 + 1e-4) + 1e-12);
