@@ -580,9 +580,20 @@ int madrl_path_sums_f32(int T, int E, int A, int P, const float* rew_dev, const 
  *                             row env_off[e] + g for g <= end_e.  first != NULL: src is shifted by one step (step t
  *                             reads src[t-1], step 0 first [E][slab_bytes]), as the policy reads its observations.
  *                             16-byte vector copies when slab_bytes and the pointers allow them.
+ * Over the ranks of a sharded batch (each rank holding its own envs' carry and acc) the fold runs in two calls around
+ * a sum of the ranks' increments, so that t* is the whole batch's:
+ *   madrl_whole_paths_steps   inc int64 [T]: this rank's increment of the count at step t_base + t, the env-steps of
+ *                             its paths that end there (from carry's last done and the launch's own dones).  It
+ *                             does not write carry.  One CTA, no atomics.
+ *   madrl_whole_paths_fold_pooled  madrl_whole_paths_fold with the count advanced by inc[t], the increments summed
+ *                             over the ranks; the finished flag, N and P are this rank's.
  * MADRL_EINVAL for sizes < 1, batch_size < 1 or >= 2^62, or a NULL required buffer. */
 int madrl_whole_paths_fold(int T, int E, int t_base, size_t batch_size, const uint8_t* done_dev, int32_t* carry_dev,
                            int64_t* acc_dev, void* stream);
+int madrl_whole_paths_steps(int T, int E, int t_base, const uint8_t* done_dev, const int32_t* carry_dev,
+                            int64_t* inc_dev, void* stream);
+int madrl_whole_paths_fold_pooled(int T, int E, int t_base, size_t batch_size, const uint8_t* done_dev,
+                                  const int64_t* inc_dev, int32_t* carry_dev, int64_t* acc_dev, void* stream);
 int madrl_whole_paths_finish(int E, int S, const uint8_t* done_stage_dev, const int32_t* carry_dev,
                              int32_t* env_off_dev, int32_t* path_start_dev, uint8_t* done_flat_dev, void* stream);
 int madrl_whole_paths_gather(int T, int E, size_t slab_bytes, int t_base, const void* src_dev, const void* first_dev,

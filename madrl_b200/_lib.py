@@ -186,6 +186,8 @@ def _signatures():
         "madrl_path_sums_f32": (i32, [i32] * 4 + [vp] * 6),
         # whole-path sampling and the flat batch's path-parallel passes
         "madrl_whole_paths_fold": (i32, [i32] * 3 + [sz] + [vp] * 4),
+        "madrl_whole_paths_steps": (i32, [i32] * 3 + [vp] * 4),
+        "madrl_whole_paths_fold_pooled": (i32, [i32] * 3 + [sz] + [vp] * 5),
         "madrl_whole_paths_finish": (i32, [i32] * 2 + [vp] * 6),
         "madrl_whole_paths_gather": (i32, [i32, i32, sz, i32] + [vp] * 6),
         "madrl_paths_plan_flat": (i32, [i32] * 2 + [vp] * 6),

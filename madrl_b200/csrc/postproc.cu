@@ -676,7 +676,9 @@ __global__ void time_baseline_apply_kernel(int T, int E, int A, int G, int L, co
 // reaches batch_size, and env e keeps its steps [0, end_e], end_e its first done at or after t* (the paths finished
 // by t* and the one it was running at t*, run to its end).  One CTA folds each launch: thread j owns the envs
 // j, j + kWpThreads, ..., and a block reduction per step gives the step's count increment.  Integer sums, so the
-// result does not depend on the reduction order, and no atomics.
+// result does not depend on the reduction order, and no atomics.  Over the ranks of a sharded batch the fold splits
+// in two: each rank's steps kernel writes its increments, the ranks sum them, and the pooled fold advances the one
+// count by the sums.
 constexpr int kWpThreads = 256;
 
 __device__ __forceinline__ int64_t block_sum_i64(int64_t v, int64_t* sh) {
@@ -690,11 +692,16 @@ __device__ __forceinline__ int64_t block_sum_i64(int64_t v, int64_t* sh) {
   return t;
 }
 
-// carry [3][E] = (last done step, end_e, paths kept); acc [5] = (count, t*, finished, N, P).
+// carry [3][E] = (last done step, end_e, paths kept); acc [5] = (count, t*, finished, N, P).  kPooled: the count
+// advances by inc[t], the increment of step t_base + t pooled over the ranks that shard the batch
+// (whole_paths_steps_kernel on each rank, summed between the launches), instead of this launch's own block sums;
+// the envs, the finished flag, N and P stay this rank's.  (The unpooled instantiation never reads inc.)
+template <bool kPooled>
 __global__ void __launch_bounds__(kWpThreads) whole_paths_fold_kernel(int T, int E, int t_base, int64_t batch_size,
                                                                       const uint8_t* __restrict__ done,
                                                                       int32_t* __restrict__ carry,
-                                                                      int64_t* __restrict__ acc) {
+                                                                      int64_t* __restrict__ acc,
+                                                                      const int64_t* __restrict__ inc) {
   __shared__ int64_t sh[kWpThreads / 32];
   int32_t* last = carry;
   int32_t* end = carry + E;
@@ -708,7 +715,10 @@ __global__ void __launch_bounds__(kWpThreads) whole_paths_fold_kernel(int T, int
       int64_t add = 0;
       for (int e = threadIdx.x; e < E; e += kWpThreads)
         if (d[e]) { add += g - last[e]; last[e] = g; ++npaths[e]; }
-      count += block_sum_i64(add, sh);
+      if constexpr (kPooled)
+        count += inc[t];
+      else
+        count += block_sum_i64(add, sh);
       if (count >= batch_size) {
         tstar = g;
         for (int e = threadIdx.x; e < E; e += kWpThreads)
@@ -733,6 +743,29 @@ __global__ void __launch_bounds__(kWpThreads) whole_paths_fold_kernel(int T, int
     const bool fin = tstar >= 0 && open == 0;
     acc[0] = count; acc[1] = tstar; acc[2] = fin;
     acc[3] = fin ? n : 0; acc[4] = fin ? p : 0;
+  }
+}
+
+// inc [T]: this rank's increments of the count, the fold's block sums without its writes.  Env e's last done before
+// step g is its last done earlier in the launch, found by looking back along its own done column (the look-backs of
+// one column cover it at most once), or carry's last from the launches before.
+__global__ void __launch_bounds__(kWpThreads) whole_paths_steps_kernel(int T, int E, int t_base,
+                                                                       const uint8_t* __restrict__ done,
+                                                                       const int32_t* __restrict__ carry,
+                                                                       int64_t* __restrict__ inc) {
+  __shared__ int64_t sh[kWpThreads / 32];
+  for (int t = 0; t < T; ++t) {
+    const int g = t_base + t;
+    int64_t add = 0;
+    for (int e = threadIdx.x; e < E; e += kWpThreads) {
+      if (!done[(size_t)t * E + e]) continue;
+      int prev = carry[e];
+      for (int u = t - 1; u >= 0; --u)
+        if (done[(size_t)u * E + e]) { prev = t_base + u; break; }
+      add += g - prev;
+    }
+    add = block_sum_i64(add, sh);
+    if (threadIdx.x == 0) inc[t] = add;
   }
 }
 
@@ -1224,8 +1257,32 @@ extern "C" int madrl_whole_paths_fold(int T, int E, int t_base, size_t batch_siz
   MADRL_REQUIRE(T >= 1 && E >= 1 && t_base >= 0, "bad sizes");
   MADRL_REQUIRE(batch_size >= 1 && batch_size < ((size_t)1 << 62), "batch_size must be in [1, 2^62)");
   MADRL_REQUIRE(done_dev && carry_dev && acc_dev, "NULL buffer");
-  MADRL_LAUNCH(whole_paths_fold_kernel, 1, kWpThreads, 0, (cudaStream_t)stream, T, E, t_base, (int64_t)batch_size,
-               done_dev, carry_dev, acc_dev);
+  MADRL_LAUNCH(whole_paths_fold_kernel<false>, 1, kWpThreads, 0, (cudaStream_t)stream, T, E, t_base,
+               (int64_t)batch_size, done_dev, carry_dev, acc_dev, (const int64_t*)nullptr);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_whole_paths_steps(int T, int E, int t_base, const uint8_t* done_dev, const int32_t* carry_dev,
+                                       int64_t* inc_dev, void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && t_base >= 0, "bad sizes");
+  MADRL_REQUIRE(done_dev && carry_dev && inc_dev, "NULL buffer");
+  MADRL_LAUNCH(whole_paths_steps_kernel, 1, kWpThreads, 0, (cudaStream_t)stream, T, E, t_base, done_dev, carry_dev,
+               inc_dev);
+  g_launches.fetch_add(1);
+  MADRL_CUDA_CHECK(cudaGetLastError());
+  return MADRL_OK;
+}
+
+extern "C" int madrl_whole_paths_fold_pooled(int T, int E, int t_base, size_t batch_size, const uint8_t* done_dev,
+                                             const int64_t* inc_dev, int32_t* carry_dev, int64_t* acc_dev,
+                                             void* stream) {
+  MADRL_REQUIRE(T >= 1 && E >= 1 && t_base >= 0, "bad sizes");
+  MADRL_REQUIRE(batch_size >= 1 && batch_size < ((size_t)1 << 62), "batch_size must be in [1, 2^62)");
+  MADRL_REQUIRE(done_dev && inc_dev && carry_dev && acc_dev, "NULL buffer");
+  MADRL_LAUNCH(whole_paths_fold_kernel<true>, 1, kWpThreads, 0, (cudaStream_t)stream, T, E, t_base,
+               (int64_t)batch_size, done_dev, carry_dev, acc_dev, inc_dev);
   g_launches.fetch_add(1);
   MADRL_CUDA_CHECK(cudaGetLastError());
   return MADRL_OK;

@@ -41,22 +41,28 @@ from ._lib import _ptr
 MODES = ("centralized", "decentralized", "concurrent")
 
 
-def _global_envs(engine, group):
+def _global_envs(engine, group, same=()):
     """The envs of the whole batch: the engine's own, or with a group of several ranks the global size of the
     shards, once every rank has checked that they tile it.  The ranks exchange their (lo, hi, E_global) in one
-    collective and apply the same rule to what they gathered, so they all raise or all go on."""
+    collective and apply the same rule to what they gathered, so they all raise or all go on.  `same`: (name, int)
+    pairs that every rank must pass alike, exchanged and checked in the same collective."""
     from .dist import _world, pool_cat
     if group is None or _world(group) == 1:
         return engine.n_envs
     shard = getattr(engine, "shard", None)
     mine = (-1, -1, -1) if shard is None or int(shard[1]) - int(shard[0]) != engine.n_envs else shard
-    lo, hi, size = pool_cat(torch.tensor(mine, dtype=torch.int64, device=engine.device).view(3, 1),
-                            group).cpu().numpy()
+    mine = tuple(mine) + tuple(int(v) for _, v in same)
+    got = pool_cat(torch.tensor(mine, dtype=torch.int64, device=engine.device).view(len(mine), 1),
+                   group).cpu().numpy()
+    lo, hi, size = got[:3]
     E = int(size[0])
     if not (lo[0] == 0 and (lo[1:] == hi[:-1]).all() and (hi > lo).all() and hi[-1] == E and (size == E).all()):
         raise ValueError("an evaluation over several ranks needs engines built by dist.make_sharded whose shards "
                          "tile the batch in group-rank order; got (lo, hi, n_envs_global) = %s"
                          % [tuple(int(v) for v in c) for c in zip(lo, hi, size)])
+    for (name, _), v in zip(same, got[3:]):
+        if (v != v[0]).any():
+            raise ValueError("%s differs across the ranks: %s" % (name, [int(x) for x in v]))
     return E
 
 

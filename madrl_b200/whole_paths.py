@@ -14,6 +14,13 @@ the batch's path table, so ``postproc.gae``, the linear baselines, ``process_sam
 ``process_samples_recurrent`` / ``pad_paths``, ``path_statistics`` and ``rltools_sampler.process_samples`` cut its
 paths from ``path_start`` with one thread per path or row (``madrl_paths_plan_flat``, ``madrl_gae_paths_f32``)
 rather than walking the N rows of the view serially.  The results are the serial kernels' bit for bit.
+
+With ``group=`` (a ``torch.distributed`` group whose ranks each hold one shard of the env batch, built by
+``dist.make_sharded``) the selection is the whole batch's: each launch, ``madrl_whole_paths_steps`` writes the
+rank's count increment of every step, ``dist.pool_sum`` adds them over the ranks, and
+``madrl_whole_paths_fold_pooled`` advances the one count by the sums, so t* is the same on every rank and each rank
+keeps exactly the rows of its envs that the unsharded selection keeps.  The ranks' batches, concatenated in
+group-rank order (``path_start`` and ``env_rows`` shifted by the rows of the lower ranks), are the unsharded batch.
 """
 import collections
 
@@ -22,6 +29,7 @@ import torch
 from . import _lib
 from ._lib import _ptr
 from .closed_loop import PolicyRollout, _map_state
+from .dist import _world, pool_min, pool_sum
 
 
 class WholePathBatch(object):
@@ -94,15 +102,20 @@ _Launch = collections.namedtuple("_Launch", "first policy_obs actions rew info e
 class _Selection(object):
     """The device side of one batch: ``add`` folds each launch of T steps of E envs (madrl_whole_paths_fold) and
     keeps its outputs, ``batch`` gathers the kept rows (madrl_whole_paths_finish / _gather).  `max_steps`: the
-    capacity of the done columns kept for the path table."""
+    capacity of the done columns kept for the path table.  `group`: the ranks that shard the batch (None or one
+    rank: this rank holds all of it); every rank must add its launches in step."""
 
-    def __init__(self, E, T, batch_size, max_steps, device):
+    def __init__(self, E, T, batch_size, max_steps, device, group=None):
         self.E, self.T, self.batch_size, self.S, self.device = E, T, int(batch_size), int(max_steps), device
         self.carry = torch.tensor([-1, -1, 0], dtype=torch.int32, device=device).repeat_interleave(E)
         self.acc = torch.tensor([0, -1, 0, 0, 0], dtype=torch.int64, device=device)
         self.done_stage = torch.zeros((self.S, E), dtype=torch.uint8, device=device)
         self.launches = []
         self.status = None
+        self.group = group if group is not None and _world(group) > 1 else None
+        if self.group is not None:
+            self.inc = torch.empty(T, dtype=torch.int64, device=device)
+            self.pooled_inc = torch.zeros(T, dtype=torch.int64, device=device)
 
     @property
     def n_steps(self):
@@ -110,7 +123,9 @@ class _Selection(object):
 
     def add(self, first, policy_obs, actions, rew, done, info, extras):
         """Fold one launch ([T, E, ...] tensors, owned by the selection from now on; `first` [E, ...]: the policy's
-        input before its first step) -> True once the batch is complete.  One 40-byte device->host read."""
+        input before its first step) -> True once the batch is complete.  One 40-byte device->host read; over
+        several ranks, until t* is known, a sum of the T step increments over the ranks, and then the minimum of
+        their finished flags, so that every rank completes at the same launch."""
         T, E, t = self.T, self.E, self.n_steps
         if t + T > self.S:
             raise RuntimeError("no whole-path batch after %d steps: the engine's paths must end within its "
@@ -118,12 +133,22 @@ class _Selection(object):
         _lib.require_tensor(done, "done", torch.uint8, (T, E), self.device)
         self.launches.append(_Launch(first, policy_obs, actions, rew, info, extras))
         self.done_stage[t:t + T].copy_(done)
+        L, d = _lib.lib(), _ptr(self.done_stage[t:t + T])
         with torch.cuda.device(self.device):
-            _lib.check(_lib.lib().madrl_whole_paths_fold(T, E, t, self.batch_size, _ptr(self.done_stage[t:t + T]),
-                                                         _ptr(self.carry), _ptr(self.acc),
-                                                         _lib.stream(self.device)))
-        self.status = self.acc.cpu()
-        return bool(self.status[2])
+            stream = _lib.stream(self.device)
+            if self.group is None:
+                _lib.check(L.madrl_whole_paths_fold(T, E, t, self.batch_size, d, _ptr(self.carry), _ptr(self.acc),
+                                                    stream))
+                self.status = self.acc.cpu()
+                return bool(self.status[2])
+            if self.status is None or self.status[1] < 0:      # t* not known yet: pool this launch's increments
+                _lib.check(L.madrl_whole_paths_steps(T, E, t, d, _ptr(self.carry), _ptr(self.inc), stream))
+                self.pooled_inc = pool_sum(self.inc, self.group)
+            _lib.check(L.madrl_whole_paths_fold_pooled(T, E, t, self.batch_size, d, _ptr(self.pooled_inc),
+                                                       _ptr(self.carry), _ptr(self.acc), stream))
+            status = torch.cat([self.acc, pool_min(self.acc[2:3], self.group)]).cpu()
+        self.status = status[:5]
+        return bool(status[5])
 
     def batch(self):
         """The `WholePathBatch` of a complete selection."""
@@ -173,10 +198,19 @@ class WholePathSampler(object):
 
     ``sampler(state0=None)`` resets the engine (and zeroes a copy of the recurrent state `state0`, whose shapes it
     takes) and returns a `WholePathBatch`.  Each launch's outputs are copied aside before the next launch overwrites
-    them, so the memory held is about twice the rows the sampler ran."""
+    them, so the memory held is about twice the rows the sampler ran.
+
+    ``group``: a ``torch.distributed`` group whose ranks each hold one shard of the env batch (engines built by
+    ``dist.make_sharded`` with the group's rank and size).  The selection is then the whole batch's: one count of
+    finished env-steps over every rank's envs, one t* and one number of launches on every rank.  Each rank returns
+    its own envs' rows; concatenated in group-rank order, with ``path_start`` and ``env_rows`` shifted by the rows
+    of the lower ranks, they are the batch an unsharded sampler returns on the same envs.  Every rank must call the
+    sampler together.  At construction the ranks check, in one collective, that their shards tile the batch in
+    group-rank order and that they pass the same ``batch_size``, ``max_path_length`` and ``chunk``; otherwise every
+    rank raises ValueError.  ``group=None`` or a one-rank group: this rank holds the whole batch."""
 
     def __init__(self, engine, policy, batch_size, max_path_length, chunk=64, frame_stack=1, standardizer=None,
-                 graph=True):
+                 graph=True, group=None):
         if int(batch_size) != batch_size or batch_size < 1:
             raise ValueError("batch_size must be a positive int, got %r" % (batch_size,))
         if int(chunk) != chunk or chunk < 1:
@@ -185,8 +219,11 @@ class WholePathSampler(object):
         if int(max_path_length) != mpl or mpl < 1:
             raise ValueError("max_path_length (%r) must equal the engine's, which must be > 0 (got %d): the engine's "
                              "horizon cut ends the paths" % (max_path_length, mpl))
-        self.engine, self.policy = engine, policy
+        self.engine, self.policy, self.group = engine, policy, group
         self.batch_size, self.max_path_length, self.chunk = int(batch_size), mpl, int(chunk)
+        from .evaluate import _global_envs
+        self.n_envs_global = _global_envs(engine, group, (("batch_size", self.batch_size),
+                                                          ("max_path_length", mpl), ("chunk", self.chunk)))
         self.frame_stack, self.standardizer = frame_stack, standardizer
         self.loop = PolicyRollout(engine, policy, self.chunk, auto_reset=True, graph=graph, frame_stack=frame_stack,
                                   standardizer=standardizer)
@@ -194,8 +231,10 @@ class WholePathSampler(object):
     def max_steps(self):
         """The most lockstep steps a call can run: every path ends within max_path_length steps, so the finished
         paths reach batch_size by step ceil(batch_size / E) + max_path_length - 1, and the paths running then end
-        within max_path_length more; rounded up to whole launches."""
-        E, mpl, T = self.engine.n_envs, self.max_path_length, self.chunk
+        within max_path_length more; rounded up to whole launches.  E is the whole batch's env count, so every
+        rank of a group has the same capacity."""
+        E = getattr(self, "n_envs_global", self.engine.n_envs)
+        mpl, T = self.max_path_length, self.chunk
         steps = -(-self.batch_size // E) + 2 * mpl
         return -(-steps // T) * T
 
@@ -213,7 +252,7 @@ class WholePathSampler(object):
     def __call__(self, state0=None):
         eng = self.engine
         with torch.cuda.device(eng.device):
-            sel = _Selection(eng.n_envs, self.chunk, self.batch_size, self.max_steps(), eng.device)
+            sel = _Selection(eng.n_envs, self.chunk, self.batch_size, self.max_steps(), eng.device, self.group)
             obs0 = self._first_obs()
             state = _map_state(torch.zeros_like, state0)
             while True:
