@@ -158,6 +158,10 @@ def _signatures():
         "madrl_hostage_launch_log": (i32, [i32, vp, i32]),
         "madrl_pursuit_set_params": (i32, [vp, f64, f64]),
         "madrl_pursuit_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        # frames
+        "madrl_ww_render": (i32, [vp, i32, vp, i32, vp, vp, vp]),
+        "madrl_hostage_render": (i32, [vp, i32, vp, i32, vp, vp, vp]),
+        "madrl_pursuit_render": (i32, [vp, i32, vp, i32, vp, vp]),
         # hand-written policies
         "madrl_ww_heuristic_actions": (i32, [i32, sz, i32, i32, vp, vp, vp]),
         "madrl_pursuit_heuristic_actions": (i32, [sz, i32, i32, i32, i32, vp, vp, vp, vp, vp]),

@@ -29,6 +29,18 @@ struct EngineCore {
   size_t obs_elem_bytes(size_t native) const { return obs_format == MADRL_OBS_BF16 ? 2 : native; }
 };
 
+// What the frame kernels of render.cu read of a family handle, which only its own source file can see into:
+// the config, the state layout and the state blob.  Defined next to each family's handle.
+template <class Cfg, class Layout>
+struct HandleView {
+  const Cfg* cfg;
+  const Layout* lay;
+  const char* state;
+};
+HandleView<madrl_ww_config, madrl_ww_layout> handle_view(const madrl_ww* h);
+HandleView<madrl_pursuit_config, madrl_pursuit_layout> handle_view(const madrl_pursuit* h);
+HandleView<madrl_hostage_config, madrl_hostage_layout> handle_view(const madrl_hostage* h);
+
 template <class H>
 int engine_destroy(H* h) {
   if (!h) return MADRL_OK;

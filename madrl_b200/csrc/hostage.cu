@@ -472,6 +472,10 @@ extern "C" int madrl_hostage_destroy(madrl_hostage* h) { return engine_destroy(h
 
 extern "C" void* madrl_hostage_state_ptr(madrl_hostage* h) { return h ? h->state : nullptr; }
 
+HandleView<madrl_hostage_config, madrl_hostage_layout> madrl::handle_view(const madrl_hostage* h) {
+  return {&h->cfg, &h->lay, h->state};
+}
+
 extern "C" int madrl_hostage_seed(madrl_hostage* h, uint64_t seed, void* stream) { return engine_seed(h, seed, stream); }
 
 extern "C" int madrl_hostage_set_terminal_obs(madrl_hostage* h, void* term_obs_dev) {

@@ -620,6 +620,10 @@ extern "C" int madrl_pursuit_destroy(madrl_pursuit* h) { return engine_destroy(h
 
 extern "C" void* madrl_pursuit_state_ptr(madrl_pursuit* h) { return h ? h->state : nullptr; }
 
+HandleView<madrl_pursuit_config, madrl_pursuit_layout> madrl::handle_view(const madrl_pursuit* h) {
+  return {&h->cfg, &h->lay, h->state};
+}
+
 extern "C" int madrl_pursuit_seed(madrl_pursuit* h, uint64_t seed, void* stream) { return engine_seed(h, seed, stream); }
 
 extern "C" int madrl_pursuit_set_terminal_obs(madrl_pursuit* h, void* term_obs_dev) {

@@ -905,6 +905,10 @@ extern "C" int madrl_ww_destroy(madrl_ww* h) { return engine_destroy(h); }
 
 extern "C" void* madrl_ww_state_ptr(madrl_ww* h) { return h ? h->state : nullptr; }
 
+HandleView<madrl_ww_config, madrl_ww_layout> madrl::handle_view(const madrl_ww* h) {
+  return {&h->cfg, &h->lay, h->state};
+}
+
 extern "C" int madrl_ww_seed(madrl_ww* h, uint64_t seed, void* stream) { return engine_seed(h, seed, stream); }
 
 extern "C" int madrl_ww_set_peers(madrl_ww* h, int n_peers, int rank, int t_max, void* const* rew_peers,

@@ -182,6 +182,54 @@ class BatchedEngine(object):
             return obs[0], rew[0], done[0], {self._info_keys[0]: info[0]}
         return obs[0], rew[0], done[0], {k: info[0, :, i] for i, k in enumerate(self._info_keys)}
 
+    RENDER_MAX_SIZE = 32768   # largest frame edge of madrl_*_render
+
+    def _frame_ids(self, env_ids):
+        """`env_ids` as the int32 device tensor the frame kernels read.  A sequence or a host tensor is checked here
+        (ValueError for an id outside [0, n_envs)); a CUDA tensor is not read back, which would synchronise with
+        the device, and the frame of an id outside the range comes back all zero (DESIGN §4.10)."""
+        if isinstance(env_ids, torch.Tensor) and env_ids.device.type == "cuda":
+            if env_ids.dtype not in (torch.int32, torch.int64) or env_ids.dim() != 1:
+                raise TypeError("env_ids must be a 1-D int32 or int64 tensor, got %s of shape %s"
+                                % (env_ids.dtype, tuple(env_ids.shape)))
+            ids = env_ids.to(device=self.device, dtype=torch.int32).contiguous()
+        else:
+            a = np.asarray(env_ids.numpy() if isinstance(env_ids, torch.Tensor) else env_ids)
+            if a.ndim != 1 or not (a.size == 0 or np.issubdtype(a.dtype, np.integer)):
+                raise TypeError("env_ids must be a 1-D sequence of ints, got %r" % (env_ids,))
+            if a.size and (a.min() < 0 or a.max() >= self.n_envs):
+                raise ValueError("env_ids must lie in [0, %d), got %d .. %d" % (self.n_envs, a.min(), a.max()))
+            ids = torch.as_tensor(a.astype(np.int32), device=self.device)
+        if ids.numel() < 1:
+            raise ValueError("env_ids must name at least one env")
+        return ids
+
+    def _render(self, env_ids, shape, out, *args):
+        """madrl_<abi>_render of `env_ids` into `out` (or a new tensor) of shape [n, *shape]; `args`: the family's
+        arguments between the ids and the output."""
+        if any(s < 1 or s > self.RENDER_MAX_SIZE for s in shape[:2]):
+            raise ValueError("a frame must be 1 to %d pixels a side, got %d x %d" % (self.RENDER_MAX_SIZE, shape[1],
+                                                                                   shape[0]))
+        ids = self._frame_ids(env_ids)
+        shape = (ids.numel(),) + tuple(shape)
+        if out is None:
+            out = torch.empty(shape, dtype=torch.uint8, device=self.device)
+        _lib.require_tensor(out, "out", torch.uint8, shape, self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self._fn("render")(self._h, ids.numel(), _ptr(ids), *args, _ptr(out), _lib.stream(self.device)))
+        return out
+
+    def _render_sensor_frames(self, env_ids, screen_size, out):
+        """Waterworld's and Hostage's render_frames: S x S frames drawn with the float64 sensor direction table."""
+        S = int(screen_size)
+        if S != screen_size:
+            raise TypeError("screen_size must be an int, got %r" % (screen_size,))
+        dirs = getattr(self, "_sensor_dirs", None)
+        if dirs is None:   # built once on the host, as the reference builds its sensors (waterworld.py:29-30)
+            ang = np.linspace(0., 2. * np.pi, self.cfg.n_sensors + 1)[:-1]
+            dirs = self._sensor_dirs = torch.as_tensor(np.stack([np.cos(ang), np.sin(ang)]), device=self.device)
+        return self._render(env_ids, (S, S, 3), out, S, _ptr(dirs))
+
     def rollout_host(self, actions, obs, rew, done, info, auto_reset=True, obs_last=False):
         """rollout() with HOST tensors (pinned for full PCIe speed); the copies are inside the call,
         chunked and overlapped with the compute (csrc/host_pipeline.cuh).  `obs_last=True`: only the last
@@ -221,6 +269,10 @@ class DropInEnv(AbstractMAEnv, EzPickle):
         self._seed_value = 0 if seed is None else int(seed)
         self._engine.seed(self._seed_value)
         return [seed]
+
+    def _frame(self, **kw):
+        """Env 0's frame (render_frames of the engine) as a NumPy RGB uint8 array; no window is opened."""
+        return self._engine.render_frames([0], **kw)[0].cpu().numpy()
 
     def vec_env_executor(self, n_envs, max_path_length):
         from .vec_executor import BatchedVecExecutor

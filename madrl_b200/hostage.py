@@ -89,6 +89,13 @@ class BatchedHostageWorld(BatchedEngine):
                     rng_counter=self._view(L.rng_counter, torch.int64, (E,)))
 
 
+    def render_frames(self, env_ids, screen_size=800, out=None):
+        """Frames of the listed envs as the reference's render draws them (hostage.py:431-478, with 8-connected
+        lines and circles in place of the anti-aliased ones; DESIGN §4.10): uint8 [n, screen_size, screen_size, 3],
+        RGB.  Arguments as BatchedMAWaterWorld.render_frames."""
+        return self._render_sensor_frames(env_ids, screen_size, out)
+
+
 class ContinuousHostageWorld(DropInEnv):
     """Drop-in for the reference class (same constructor, hostage.py:75-79)."""
 
@@ -114,6 +121,12 @@ class ContinuousHostageWorld(DropInEnv):
         self._rescuers = [CircAgent(i + 1, radius, n_sensors, sensor_range, addid) for i in range(n_good)]
         self._done = False
         self.setup()
+
+    def render(self, screen_size=800, rate=10, mode='human'):
+        """The frame the reference's render draws (hostage.py:431-478) as a NumPy RGB uint8 array
+        [screen_size, screen_size, 3]; the reference shows it in a window and returns None.  No window is opened:
+        `rate` and `mode` are accepted for the drop-ins' common signature and unused."""
+        return self._frame(screen_size=screen_size)
 
     def _make_engine(self, n_envs, **kw):
         # looks up the module-level class at call time, so that a test double can stand in for it

@@ -101,6 +101,18 @@ class BatchedPursuitEvade(BatchedEngine):
                     rng_counter=self._view(L.rng_counter, torch.int64, (E,)),
                     stale=self._view(L.stale, torch.int16, (E, Np, RR)))
 
+    def render_frames(self, env_ids, cell=16, out=None):
+        """Frames of the listed envs (a sequence or an int tensor; repeats allowed; a sharded engine's local ids):
+        uint8 [n, ys * cell, xs * cell, 3], RGB, on the engine's device -- the picture of the reference's render
+        (pursuit_evade.py:274-295) under the integer rule of DESIGN §4.10: pixel (row, col) shows cell
+        (col // cell, row // cell); free cells white, buildings (64, 64, 64); each pursuer's observation window
+        blended with #FF9848 as (v + o + 1) >> 1; then pursuer markers (255, 0, 0) and live evader markers
+        (0, 0, 255) over the cell's [cell/4, cell - cell/4) square.  `out` as BatchedMAWaterWorld.render_frames."""
+        c = int(cell)
+        if c != cell or c < 1:
+            raise ValueError("cell must be an int >= 1, got %r" % (cell,))
+        return self._render(env_ids, (self.map_pool.shape[2] * c, self.map_pool.shape[1] * c, 3), out, c)
+
     def set_params(self, catchr=None, constraint_window=None):
         """Curriculum updates (pursuit_evade.py:264-272)."""
         if catchr is not None:
@@ -224,6 +236,12 @@ class PursuitEvade(DropInEnv):
         if self._reward_mech == 'global':
             return obslist, [rew[0]] * self.n_pursuers, bool(done[0].item()), {'removed': removed}
         return obslist, rew, bool(done[0].item()), {'removed': removed}
+
+    def render(self, plt_delay=1.0, cell=16):
+        """Env 0's frame (BatchedPursuitEvade.render_frames) as a NumPy RGB uint8 array [ys * cell, xs * cell, 3],
+        where the reference plots it with matplotlib.  No window is opened: `plt_delay` is accepted for the
+        reference's signature and unused."""
+        return self._frame(cell=cell)
 
     def update_curriculum(self, itr):
         self.constraint_window += self.curriculum_constrain_rate

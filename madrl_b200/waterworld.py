@@ -109,6 +109,14 @@ class BatchedMAWaterWorld(BatchedEngine):
             rng_counter=self._view(L.rng_counter, torch.int64, (E,)),
             sensors=self._view(L.sensors, dt, (2, self.n_sensors)))
 
+    def render_frames(self, env_ids, screen_size=800, out=None):
+        """Frames of the listed envs (a sequence or an int tensor; repeats allowed; a sharded engine's local ids)
+        as the reference's render draws them (waterworld.py:438-479, with 8-connected lines and circles in place
+        of the anti-aliased ones; DESIGN §4.10): uint8 [n, screen_size, screen_size, 3], RGB, on the engine's
+        device.  `out`: a tensor of that shape to draw into; with it and a CUDA tensor of ids the call makes no
+        host synchronisation and no allocation after its first call, and may be captured in a CUDA graph."""
+        return self._render_sensor_frames(env_ids, screen_size, out)
+
     def set_peers(self, rank, t_max, rew_peers, done_peers, info_peers):
         """Enable the fused exchange: `*_peers` are lists (one per DESTINATION rank) of tensors
         aliasing the destination gather buffers; this rank writes slot `rank` of each
@@ -226,6 +234,12 @@ class MAWaterWorld(DropInEnv):
     @property
     def is_terminal(self):
         return self._timesteps >= self.timestep_limit
+
+    def render(self, screen_size=800, rate=10, mode='human'):
+        """The frame the reference's render draws (waterworld.py:438-479), as a NumPy RGB uint8 array
+        [screen_size, screen_size, 3] (BatchedMAWaterWorld.render_frames).  No window is opened: `rate` and `mode`
+        are accepted for the reference's signature and unused."""
+        return self._frame(screen_size=screen_size)
 
     def step(self, action_Np2):
         a = np.asarray(action_Np2, dtype=np.float64).reshape((self.n_pursuers, 2))  # waterworld.py:221-222
