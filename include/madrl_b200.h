@@ -396,7 +396,8 @@ int madrl_hostage_rollout_host2(madrl_hostage* h, int T, const void* actions_hos
  * Frames of n chosen envs drawn on the device from the state blob (csrc/render.cu, DESIGN §4.10), RGB uint8.
  * env_ids_dev int32 [n] (repeats allowed).  The kernels only read the state, and make no host synchronisation or
  * allocation, so a render may be captured into a CUDA graph.  The ids are not read on the host: the frame of an id
- * outside [0, n_envs) is written all zero, which no drawn frame is.
+ * outside [0, n_envs) is written all zero, which no drawn frame is.  An object with a non-finite coordinate draws
+ * nothing.
  *   madrl_ww_render       out [n][S][S][3]: the reference's MAWaterWorld.render (waterworld.py:438-479) drawn with
  *                         8-connected lines and circles (LINE_8) and its background blend; S = screen_size.
  *                         sensor_dirs_dev float64 [2][n_sensors]: the cos and sin rows of the sensor angles
@@ -405,7 +406,8 @@ int madrl_hostage_rollout_host2(madrl_hostage* h, int T, const void* actions_hos
  *   madrl_hostage_render  the same for ContinuousHostageWorld.render (hostage.py:431-478).
  *   madrl_pursuit_render  out [n][ys * cell][xs * cell][3]: the integer Pursuit picture of DESIGN §4.10.
  * MADRL_EINVAL for a NULL handle or buffer, n < 1, screen_size or cell outside [1, 32768], a Pursuit frame more
- * than 32768 pixels a side, or a radius of 2^30 pixels or more. */
+ * than 32768 pixels a side, a radius of 2^29 pixels or more, or a sensor_range that is not finite or reaches
+ * |sensor_range| * screen_size >= 2^29 pixels. */
 int madrl_ww_render(madrl_ww* h, int n, const int32_t* env_ids_dev, int screen_size, const double* sensor_dirs_dev,
                     uint8_t* out_dev, void* stream);
 int madrl_hostage_render(madrl_hostage* h, int n, const int32_t* env_ids_dev, int screen_size,

@@ -19,8 +19,10 @@ constexpr int RT = 32;         // tile edge (pixels)
 constexpr int RTHREADS = 256;  // 8 warps; warp w draws rows w, w + 8, w + 16 and w + 24 of its tile
 constexpr int R_ROWS = RT * RT / RTHREADS;
 constexpr int RENDER_MAX_SIZE = 32768;   // largest frame edge: every clipped coordinate and Bresenham term fits int32
-constexpr long long RENDER_MAX_RADIUS = 1ll << 30;
-constexpr long long RENDER_COORD_LIMIT = 1ll << 30;   // coordinates are clamped here, far outside any frame
+// Radii and sensor reaches (|sensor_range| S) stay below 2^29 pixels, so a coordinate the 2^30 clamp moves belongs to
+// a primitive that misses the frame both before and after the clamp (a NaN coordinate clamps to -2^30 and misses).
+constexpr double RENDER_MAX_REACH = (double)(1ll << 29);
+constexpr long long RENDER_COORD_LIMIT = 1ll << 30;
 constexpr size_t RENDER_MAX_GRID = 1u << 20;   // blocks per launch; larger batches loop over work items
 constexpr unsigned KIND_CIRCLE = 1u << 24, KIND_LINE = 2u << 24, RGB_MASK = 0xffffffu;
 
@@ -342,11 +344,18 @@ __global__ void __launch_bounds__(PE_THREADS) render_pursuit_kernel(PEScene sc, 
   }
 }
 
-// A radius in pixels, int(radius * S) as the reference computes it; MADRL_EINVAL past RENDER_MAX_RADIUS
+// A radius in pixels, int(radius * S) as the reference computes it; MADRL_EINVAL from RENDER_MAX_REACH up
 static int radius_px(double radius, int S, int* out) {
   const double v = radius * (double)S;
-  MADRL_REQUIRE(v >= 0.0 && v < (double)RENDER_MAX_RADIUS, "a radius of %g at screen_size %d is out of range", radius, S);
+  MADRL_REQUIRE(v >= 0.0 && v < RENDER_MAX_REACH, "a radius of %g at screen_size %d is out of range", radius, S);
   *out = (int)v;
+  return MADRL_OK;
+}
+
+// MADRL_EINVAL unless |sensor_range| S < RENDER_MAX_REACH (a NaN or infinite range fails it)
+static int check_sensor_reach(double range, int S) {
+  MADRL_REQUIRE(fabs(range) * (double)S < RENDER_MAX_REACH,
+                "a sensor_range of %g at screen_size %d reaches 2^29 pixels or more", range, S);
   return MADRL_OK;
 }
 
@@ -384,7 +393,8 @@ extern "C" int madrl_ww_render(madrl_ww* h, int n, const int32_t* env_ids_dev, i
   const int S = screen_size;
   WWScene sc{v.state, v.lay->objs, v.lay->obst, v.lay->n_obj, c.n_pursuers, c.n_evaders, c.n_sensors,
              0, 0, 0, 0, c.sensor_range, sensor_dirs_dev};
-  if ((rc = radius_px(c.obstacle_radius, S, &sc.r_obst)) || (rc = radius_px(c.radius, S, &sc.r_pur)) ||
+  if ((rc = check_sensor_reach(c.sensor_range, S)) || (rc = radius_px(c.obstacle_radius, S, &sc.r_obst)) ||
+      (rc = radius_px(c.radius, S, &sc.r_pur)) ||
       (rc = radius_px(c.radius * 2, S, &sc.r_ev)) || (rc = radius_px(c.radius * 3 / 4, S, &sc.r_po)))
     return rc;   // ww:109-117: evaders radius * 2, poison radius * 3 / 4
   return launch_tiles(c.fp64 != 0, sc, c.n_envs, n, env_ids_dev, S, out_dev, stream);
@@ -400,7 +410,8 @@ extern "C" int madrl_hostage_render(madrl_hostage* h, int n, const int32_t* env_
   const int S = screen_size;
   HWScene sc{v.state, v.lay->objs, v.lay->fixed, v.lay->saved, v.lay->flags, v.lay->n_obj, c.n_good, c.n_bad,
              c.n_hostages, c.n_sensors, 0, 0, 0, c.sensor_range, sensor_dirs_dev};
-  if ((rc = radius_px(c.radius, S, &sc.r_body)) || (rc = radius_px(c.radius * 2, S, &sc.r_hostage)) ||
+  if ((rc = check_sensor_reach(c.sensor_range, S)) || (rc = radius_px(c.radius, S, &sc.r_body)) ||
+      (rc = radius_px(c.radius * 2, S, &sc.r_hostage)) ||
       (rc = radius_px(c.bomb_radius, S, &sc.r_bomb)))
     return rc;   // hostage.py:122-129: hostages radius * 2; the key is drawn with `radius` (hr:447)
   return launch_tiles(c.fp64 != 0, sc, c.n_envs, n, env_ids_dev, S, out_dev, stream);

@@ -183,16 +183,21 @@ class BatchedEngine(object):
         return obs[0], rew[0], done[0], {k: info[0, :, i] for i, k in enumerate(self._info_keys)}
 
     RENDER_MAX_SIZE = 32768   # largest frame edge of madrl_*_render
+    RENDER_MAX_REACH = float(1 << 29)   # radii and |sensor_range| * screen_size must stay below it (pixels)
 
     def _frame_ids(self, env_ids):
         """`env_ids` as the int32 device tensor the frame kernels read.  A sequence or a host tensor is checked here
         (ValueError for an id outside [0, n_envs)); a CUDA tensor is not read back, which would synchronise with
-        the device, and the frame of an id outside the range comes back all zero (DESIGN §4.10)."""
+        the device, and the frame of an id outside the range comes back all zero (DESIGN §4.10).  An int64 id
+        outside the range is made -1 on the device first, so that the int32 cast cannot wrap it onto an env."""
         if isinstance(env_ids, torch.Tensor) and env_ids.device.type == "cuda":
             if env_ids.dtype not in (torch.int32, torch.int64) or env_ids.dim() != 1:
                 raise TypeError("env_ids must be a 1-D int32 or int64 tensor, got %s of shape %s"
                                 % (env_ids.dtype, tuple(env_ids.shape)))
-            ids = env_ids.to(device=self.device, dtype=torch.int32).contiguous()
+            ids = env_ids.to(device=self.device)
+            if ids.dtype == torch.int64:
+                ids = ids.masked_fill((ids < 0) | (ids >= self.n_envs), -1)
+            ids = ids.to(dtype=torch.int32).contiguous()
         else:
             a = np.asarray(env_ids.numpy() if isinstance(env_ids, torch.Tensor) else env_ids)
             if a.ndim != 1 or not (a.size == 0 or np.issubdtype(a.dtype, np.integer)):
@@ -224,6 +229,9 @@ class BatchedEngine(object):
         S = int(screen_size)
         if S != screen_size:
             raise TypeError("screen_size must be an int, got %r" % (screen_size,))
+        r = float(self.cfg.sensor_range)
+        if not abs(r) * S < self.RENDER_MAX_REACH:   # NaN fails it too
+            raise ValueError("a sensor_range of %r at screen_size %d reaches 2^29 pixels or more" % (r, S))
         dirs = getattr(self, "_sensor_dirs", None)
         if dirs is None:   # built once on the host, as the reference builds its sensors (waterworld.py:29-30)
             ang = np.linspace(0., 2. * np.pi, self.cfg.n_sensors + 1)[:-1]

@@ -53,15 +53,16 @@ def circle_half_widths(r):
     return h
 
 
-def fill_circle(img, cx, cy, r, color):
+def fill_circle(img, cx, cy, r, color, y0=0):
+    """`img` holds the frame's rows y0 .. y0 + len(img) - 1 (all of it when y0 = 0 and it is H rows)."""
     H, W = img.shape[:2]
     h = circle_half_widths(r)
-    for oy in range(-r, r + 1):
+    for oy in range(max(-r, y0 - cy), min(r, y0 + H - 1 - cy) + 1):
         y, w = cy + oy, h[abs(oy)]
-        if 0 <= y < H and w >= 0:
+        if w >= 0:
             x0, x1 = max(cx - w, 0), min(cx + w, W - 1)
             if x0 <= x1:
-                img[y, x0:x1 + 1] = color
+                img[y - y0, x0:x1 + 1] = color
 
 
 def clip_line(W, H, x1, y1, x2, y2):
@@ -140,68 +141,123 @@ def blend_background(img):
 
 
 # ------------------------------------------------------------------------------------------ frames
-def _sensor_lines(img, x, y, sensor_range, dirs, size, body_r, body_color):
+# A frame is built as its primitives in painter's order -- ("circle", cx, cy, r, color), ("pixels", xs, ys, color)
+# for a line walked once into its pixels, or None for a primitive that draws nothing -- then painted.  The list is
+# indexed as the kernels index their primitives, and painting it in row bands lets a 32768 x 32768 frame be checked
+# without holding it whole.
+def _finite(*v):
+    return all(math.isfinite(float(x)) for x in v)
+
+
+def circle_prim(x, y, size, r, color):
+    """A filled circle at the stored coordinate (x, y); None if a coordinate is not finite (such an object
+    draws nothing, DESIGN §4.10)."""
+    return ("circle", to_px(x, size), to_px(y, size), r, color) if _finite(x, y) else None
+
+
+def line_prim(W, H, x1, y1, x2, y2, color):
+    a = np.array(line_pixels(W, H, x1, y1, x2, y2), np.int64).reshape(-1, 2)
+    return ("pixels", a[:, 0], a[:, 1], color)
+
+
+def paint(prims, W, H, rows=None):
+    """The RGB frame [H, W, 3] the primitives draw, background blend included; `rows` = (y0, y1): only its rows
+    y0 .. y1 - 1, as a [y1 - y0, W, 3] band."""
+    y0, y1 = (0, H) if rows is None else rows
+    img = np.full((y1 - y0, W, 3), 255, np.uint8)
+    for q in prims:
+        if q is None:
+            continue
+        if q[0] == "circle":
+            fill_circle(img, q[1], q[2], q[3], q[4], y0=y0)
+        else:
+            xs, ys, color = q[1], q[2], q[3]
+            m = (ys >= y0) & (ys < y1)
+            img[ys[m] - y0, xs[m]] = color
+    return blend_background(img)
+
+
+def _sensor_prims(x, y, sensor_range, dirs, size, body_r, body_color):
     """A pursuer / rescuer: each sensor line, then its body (the reference redraws the body after every line,
     which leaves the body over all of them)."""
+    K = dirs.shape[1]
+    if not _finite(x, y):
+        return [None] * (K + 1)
     p = (to_px(x, size), to_px(y, size))
-    for k in range(dirs.shape[1]):
+    out = []
+    for k in range(K):
         ex = int((np.float64(x) + sensor_range * dirs[0, k]) * size)
         ey = int((np.float64(y) + sensor_range * dirs[1, k]) * size)
-        draw_line(img, p[0], p[1], ex, ey, SENSOR_LINE)
-    if dirs.shape[1]:
-        fill_circle(img, p[0], p[1], int(body_r * size), body_color)
+        out.append(line_prim(size, size, p[0], p[1], ex, ey, SENSOR_LINE))
+    return out + [circle_prim(x, y, size, int(body_r * size), body_color)]
 
 
-def ww_frame(px, py, obst, Np, Ne, size, radius, obstacle_radius, sensor_range, dirs):
-    """The reference MAWaterWorld.render frame of one env: px, py [n_obj] (pursuers, evaders, poisons),
-    obst [2]; RGB uint8 [size, size, 3]."""
-    img = np.full((size, size, 3), 255, np.uint8)
-    fill_circle(img, to_px(obst[0], size), to_px(obst[1], size), int(obstacle_radius * size), WW_OBSTACLE)
+def ww_prims(px, py, obst, Np, Ne, size, radius, obstacle_radius, sensor_range, dirs):
+    """The primitives of ww_frame, in the kernels' order: the obstacle, each pursuer's lines and body, evaders,
+    poison."""
+    out = [circle_prim(obst[0], obst[1], size, int(obstacle_radius * size), WW_OBSTACLE)]
     for i in range(Np):
-        _sensor_lines(img, px[i], py[i], sensor_range, dirs, size, radius, WW_PURSUER)
+        out += _sensor_prims(px[i], py[i], sensor_range, dirs, size, radius, WW_PURSUER)
     for i in range(Np, Np + Ne):
-        fill_circle(img, to_px(px[i], size), to_px(py[i], size), int(radius * 2 * size), WW_EVADER)
+        out.append(circle_prim(px[i], py[i], size, int(radius * 2 * size), WW_EVADER))
     for i in range(Np + Ne, len(px)):
-        fill_circle(img, to_px(px[i], size), to_px(py[i], size), int(radius * 3 / 4 * size), WW_POISON)
-    return blend_background(img)
+        out.append(circle_prim(px[i], py[i], size, int(radius * 3 / 4 * size), WW_POISON))
+    return out
 
 
-def hw_frame(px, py, fixed, saved, flags, n_good, n_bad, size, radius, bomb_radius, sensor_range, dirs):
-    """The reference ContinuousHostageWorld.render frame of one env: px, py [n_obj] (rescuers, criminals,
-    hostages), fixed [4] = key x, y, bomb x, y, saved [n_hostages], flags (bit 0: gate open); RGB."""
-    img = np.full((size, size, 3), 255, np.uint8)
+def ww_frame(px, py, obst, Np, Ne, size, radius, obstacle_radius, sensor_range, dirs, rows=None):
+    """The reference MAWaterWorld.render frame of one env: px, py [n_obj] (pursuers, evaders, poisons),
+    obst [2]; RGB uint8 [size, size, 3] (`rows`: a band of it, as paint)."""
+    return paint(ww_prims(px, py, obst, Np, Ne, size, radius, obstacle_radius, sensor_range, dirs), size, size, rows)
+
+
+def hw_prims(px, py, fixed, saved, flags, n_good, n_bad, size, radius, bomb_radius, sensor_range, dirs):
+    """The primitives of hw_frame, in the kernels' order: gate line and key (None while the gate is open), bomb,
+    hostages (None once saved), criminals, each rescuer's lines and body."""
+    out = [None, None]
     if not int(flags) & 1:
-        draw_line(img, 0, int(0.5 * size), int(1 * size), int(0.5 * size), HW_GATE)
-        fill_circle(img, to_px(fixed[0], size), to_px(fixed[1], size), int(radius * size), HW_KEY)
-    fill_circle(img, to_px(fixed[2], size), to_px(fixed[3], size), int(bomb_radius * size), HW_BOMB)
+        out = [line_prim(size, size, 0, int(0.5 * size), int(1 * size), int(0.5 * size), HW_GATE),
+               circle_prim(fixed[0], fixed[1], size, int(radius * size), HW_KEY)]
+    out.append(circle_prim(fixed[2], fixed[3], size, int(bomb_radius * size), HW_BOMB))
     for j in range(len(saved)):
-        if not saved[j]:
-            i = n_good + n_bad + j
-            fill_circle(img, to_px(px[i], size), to_px(py[i], size), int(radius * 2 * size), HW_HOSTAGE)
+        i = n_good + n_bad + j
+        out.append(None if saved[j] else circle_prim(px[i], py[i], size, int(radius * 2 * size), HW_HOSTAGE))
     for i in range(n_good, n_good + n_bad):
-        fill_circle(img, to_px(px[i], size), to_px(py[i], size), int(radius * size), HW_CRIMINAL)
+        out.append(circle_prim(px[i], py[i], size, int(radius * size), HW_CRIMINAL))
     for i in range(n_good):
-        _sensor_lines(img, px[i], py[i], sensor_range, dirs, size, radius, HW_RESCUER)
-    return blend_background(img)
+        out += _sensor_prims(px[i], py[i], sensor_range, dirs, size, radius, HW_RESCUER)
+    return out
 
 
-def pe_frame(building, pur_x, pur_y, ev_x, ev_y, gone, obs_range, cell):
+def hw_frame(px, py, fixed, saved, flags, n_good, n_bad, size, radius, bomb_radius, sensor_range, dirs, rows=None):
+    """The reference ContinuousHostageWorld.render frame of one env: px, py [n_obj] (rescuers, criminals,
+    hostages), fixed [4] = key x, y, bomb x, y, saved [n_hostages], flags (bit 0: gate open); RGB (`rows`: a
+    band, as paint)."""
+    return paint(hw_prims(px, py, fixed, saved, flags, n_good, n_bad, size, radius, bomb_radius, sensor_range, dirs),
+                 size, size, rows)
+
+
+def pe_frame(building, pur_x, pur_y, ev_x, ev_y, gone, obs_range, cell, rows=None):
     """The Pursuit frame of one env: building bool [xs, ys]; pursuer and evader cells; gone = the evaders_gone
     bits (set for evaders removed and for those a random_opponents episode never spawned); RGB uint8
-    [ys * cell, xs * cell, 3], pixel (row, col) in cell (col // cell, row // cell)."""
+    [ys * cell, xs * cell, 3], pixel (row, col) in cell (col // cell, row // cell).  `rows` = (y0, y1): only
+    rows y0 .. y1 - 1."""
     xs, ys = building.shape
+    y0, y1 = (0, ys * cell) if rows is None else rows
     grid = np.where(building.T[..., None], np.array(PE_BUILDING, np.int64), np.array(PE_FREE, np.int64))
     off = (obs_range - 1) // 2
     win = np.array(PE_WINDOW, np.int64)
     for x, y in zip(pur_x, pur_y):
-        x0, y0 = max(int(x) - off, 0), max(int(y) - off, 0)
-        x1, y1 = min(int(x) - off + obs_range, xs), min(int(y) - off + obs_range, ys)
-        grid[y0:y1, x0:x1] = (grid[y0:y1, x0:x1] + win + 1) >> 1
-    img = np.repeat(np.repeat(grid, cell, axis=0), cell, axis=1).astype(np.uint8)
+        wx0, wy0 = max(int(x) - off, 0), max(int(y) - off, 0)
+        wx1, wy1 = min(int(x) - off + obs_range, xs), min(int(y) - off + obs_range, ys)
+        grid[wy0:wy1, wx0:wx1] = (grid[wy0:wy1, wx0:wx1] + win + 1) >> 1
+    img = grid.astype(np.uint8)[np.arange(y0, y1) // cell][:, np.arange(xs * cell) // cell]
     lo, hi = cell // 4, cell - cell // 4
 
     def mark(x, y, color):
-        img[int(y) * cell + lo:int(y) * cell + hi, int(x) * cell + lo:int(x) * cell + hi] = color
+        r0, r1 = max(int(y) * cell + lo, y0), min(int(y) * cell + hi, y1)
+        if r0 < r1:
+            img[r0 - y0:r1 - y0, int(x) * cell + lo:int(x) * cell + hi] = color
 
     for x, y in zip(pur_x, pur_y):
         mark(x, y, PE_PURSUER)
@@ -212,28 +268,28 @@ def pe_frame(building, pur_x, pur_y, ev_x, ev_y, gone, obs_range, cell):
 
 
 # ------------------------------------------------------------------------------------------ engine state
-def ww_frames(state, env_ids, size, cfg, Np, Ne):
+def ww_frames(state, env_ids, size, cfg, Np, Ne, rows=None):
     """Frames of the listed envs of a BatchedMAWaterWorld state dict (tensors or arrays); `cfg` its
-    madrl_ww_config."""
+    madrl_ww_config; `rows`: a band of each, as paint."""
     g = {k: np.asarray(v.cpu() if hasattr(v, "cpu") else v) for k, v in state.items()}
     dirs = sensor_dirs(cfg.n_sensors)
     return np.stack([ww_frame(g["pos_x"][e], g["pos_y"][e], (g["obst_x"][e], g["obst_y"][e]), Np, Ne, size,
-                              cfg.radius, cfg.obstacle_radius, cfg.sensor_range, dirs) for e in env_ids])
+                              cfg.radius, cfg.obstacle_radius, cfg.sensor_range, dirs, rows) for e in env_ids])
 
 
-def hw_frames(state, env_ids, size, cfg):
+def hw_frames(state, env_ids, size, cfg, rows=None):
     """Frames of the listed envs of a BatchedHostageWorld state dict; `cfg` its madrl_hostage_config."""
     g = {k: np.asarray(v.cpu() if hasattr(v, "cpu") else v) for k, v in state.items()}
     dirs = sensor_dirs(cfg.n_sensors)
     fixed = np.concatenate([g["key"], g["bomb"]], axis=1)
     return np.stack([hw_frame(g["pos_x"][e], g["pos_y"][e], fixed[e], g["saved"][e], g["flags"][e], cfg.n_good,
-                              cfg.n_bad, size, cfg.radius, cfg.bomb_radius, cfg.sensor_range, dirs)
+                              cfg.n_bad, size, cfg.radius, cfg.bomb_radius, cfg.sensor_range, dirs, rows)
                      for e in env_ids])
 
 
-def pe_frames(state, map_pool, env_ids, obs_range, cell):
+def pe_frames(state, map_pool, env_ids, obs_range, cell, rows=None):
     """Frames of the listed envs of a BatchedPursuitEvade state dict; map_pool int32 [n_maps, xs, ys]."""
     g = {k: np.asarray(v.cpu() if hasattr(v, "cpu") else v) for k, v in state.items()}
     return np.stack([pe_frame(map_pool[g["map_id"][e]] == -1, g["pursuer_x"][e], g["pursuer_y"][e],
-                              g["evader_x"][e], g["evader_y"][e], int(g["gone"][e]), obs_range, cell)
+                              g["evader_x"][e], g["evader_y"][e], int(g["gone"][e]), obs_range, cell, rows)
                      for e in env_ids])
