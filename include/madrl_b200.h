@@ -285,7 +285,8 @@ void* madrl_pursuit_state_ptr(madrl_pursuit* h);
 int madrl_pursuit_seed(madrl_pursuit* h, uint64_t seed, void* stream);
 int madrl_pursuit_set_launch(madrl_pursuit* h, int warps_per_block, int blocks_per_sm);
 /* Which kernel each Pursuit launch ran: madrl_ww_launch_log's contract for pe_kernel launches, with records of 8
- * int32: sizeof(observation element), EPL, CPL, RC, POLICY, FLAT, KEEP and the launch's grid. */
+ * int32: sizeof(observation element), EPL, CPL, RC, POLICY, FLAT, KEEP and the launch's grid.  POLICY's bit 0 is the
+ * in-kernel heuristic, bit 1 the evader-control instantiation (madrl_pursuit_set_evader_control). */
 int madrl_pursuit_launch_log(int enable, int32_t* records, int max_records);
 /* Terminal observations: with auto_reset the obs slot of a done step holds the RESET observation
  * (VecEnvExecutor semantics); StandardizedEnv (madrl_environments/__init__.py:283-291) also sees the
@@ -323,6 +324,34 @@ int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const void* obs0_de
                                     int auto_reset, int floor_centre, void* stream);
 int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, void* obs_dev, float* rew_dev,
                        uint8_t* done_dev, int32_t* info_dev, int auto_reset, void* stream);
+/* The evaders' controller (pursuit_evade.py:87 evader_controller, called once per live evader per step, :237-241).
+ * set_evader_control sets the handle's default, used by every launch that is given no evader actions:
+ * MADRL_PURSUIT_EVADERS_RANDOM (the default) moves each live evader by one draw of the env's stream (RandomPolicy);
+ * MADRL_PURSUIT_EVADERS_FIXED moves every evader by `action` (SingleActionPolicy(action)).
+ * The *_evaders entries take the evaders' actions of this launch instead: evader j of env e at step t moves by
+ * ev_act_dev[t * ev_st + e * ev_se + j] (int32, j its ORIGINAL index; strides 0 and 0 make one int a fixed
+ * controller); entries of removed evaders and of evaders that do not exist this episode are not read.
+ * A caller's action outside 0..3 means stay.  Whatever the controller, the env's draw counter advances by the live
+ * evader count each step, so the reset draws and the heuristic policy's fallback draws use the words they would
+ * under the random controller.  Other arguments as madrl_pursuit_rollout / madrl_pursuit_rollout_heuristic. */
+#define MADRL_PURSUIT_EVADERS_RANDOM 0
+#define MADRL_PURSUIT_EVADERS_FIXED 1
+int madrl_pursuit_set_evader_control(madrl_pursuit* h, int mode, int action);
+int madrl_pursuit_rollout_evaders(madrl_pursuit* h, int T, const int32_t* actions_dev, const int32_t* ev_act_dev,
+                                  size_t ev_st, size_t ev_se, void* obs_dev, float* rew_dev, uint8_t* done_dev,
+                                  int32_t* info_dev, int auto_reset, void* stream);
+int madrl_pursuit_rollout_heuristic_evaders(madrl_pursuit* h, int T, const void* obs0_dev, int32_t* actions_out_dev,
+                                            const int32_t* ev_act_dev, size_t ev_st, size_t ev_se, void* obs_dev,
+                                            float* rew_dev, uint8_t* done_dev, int32_t* info_dev, int auto_reset,
+                                            int floor_centre, void* stream);
+/* model_state (pursuit_evade.py:152): after this call reset() and every rollout (device pointers) write
+ * model_state_dev float [E][4][xs][ys] of the envs they touch, as the env stands after the launch's last step:
+ * channel 0 the map (-1 building, 0 free: what the map pool holds for pools of 0 / -1), 1 the pursuer count,
+ * 2 the evader count, 3 zero.  Like the reference (pursuit_evade.py:244-249) it is the occupancy before that
+ * step's removals, so an evader caught at the last step is still counted; after an auto-reset it is the reset's.
+ * The launch log marks such launches (and those with caller-controlled evaders) with bit 1 of its POLICY field.
+ * NULL switches it off. */
+int madrl_pursuit_set_model_state(madrl_pursuit* h, float* model_state_dev);
 int madrl_pursuit_reset_host(madrl_pursuit* h, const uint8_t* mask_host, void* obs_host);
 int madrl_pursuit_rollout_host(madrl_pursuit* h, int T, const int32_t* actions_host, void* obs_host,
                                float* rew_host, uint8_t* done_host, int32_t* info_host,

@@ -10,7 +10,7 @@ from ._lib import EngineError, launch_count  # noqa: F401
 from .core import Agent, AbstractMAEnv, EzPickle  # noqa: F401
 from .spaces import Box, Discrete  # noqa: F401
 from .waterworld import BatchedMAWaterWorld, MAWaterWorld, Archea  # noqa: F401
-from .pursuit import BatchedPursuitEvade, PursuitEvade, DiscreteAgent  # noqa: F401
+from .pursuit import BatchedPursuitEvade, PursuitEvade, DiscreteAgent, RandomPolicy, SingleActionPolicy  # noqa: F401
 from .hostage import BatchedHostageWorld, ContinuousHostageWorld, CircAgent  # noqa: F401
 from .closed_loop import PolicyRollout  # noqa: F401
 from .replay import ReplayPool  # noqa: F401
@@ -20,6 +20,6 @@ from .whole_paths import WholePathBatch, WholePathSampler  # noqa: F401
 __all__ = [
     "EngineError", "launch_count", "Agent", "AbstractMAEnv", "EzPickle", "Box", "Discrete",
     "BatchedMAWaterWorld", "MAWaterWorld", "Archea", "BatchedPursuitEvade", "PursuitEvade",
-    "DiscreteAgent", "BatchedHostageWorld", "ContinuousHostageWorld", "CircAgent", "PolicyRollout",
+    "DiscreteAgent", "RandomPolicy", "SingleActionPolicy", "BatchedHostageWorld", "ContinuousHostageWorld", "CircAgent", "PolicyRollout",
     "ReplayPool", "evaluate_policy", "evaluate_heuristic", "WholePathSampler", "WholePathBatch",
 ]

@@ -25,6 +25,8 @@ OBS_CACHE_STREAM, OBS_CACHE_KEEP = 0, 1
 WW_OBS_WRITER_AUTO, WW_OBS_WRITER_OFF, WW_OBS_WRITER_ON = 0, 1, 2
 # norm of Waterworld's in-kernel heuristic actions (madrl_ww_set_heuristic_norm)
 HEURISTIC_NORM_AGENT, HEURISTIC_NORM_ENV = 0, 1
+# the evaders' controller of a Pursuit handle (madrl_pursuit_set_evader_control)
+PURSUIT_EVADERS_RANDOM, PURSUIT_EVADERS_FIXED = 0, 1
 # evaluation records (madrl_eval_episodes_*): 8-byte carry words per (env, agent), most info columns
 EVAL_CARRY_WORDS, EVAL_INFO_MAX = 8, 2
 
@@ -158,6 +160,11 @@ def _signatures():
         "madrl_hostage_launch_log": (i32, [i32, vp, i32]),
         "madrl_pursuit_set_params": (i32, [vp, f64, f64]),
         "madrl_pursuit_rollout_heuristic": (i32, [vp, i32, vp, vp, vp, vp, vp, vp, i32, i32, vp]),
+        "madrl_pursuit_set_evader_control": (i32, [vp, i32, i32]),
+        "madrl_pursuit_rollout_evaders": (i32, [vp, i32, vp, vp, sz, sz, vp, vp, vp, vp, i32, vp]),
+        "madrl_pursuit_rollout_heuristic_evaders": (i32, [vp, i32, vp, vp, vp, sz, sz, vp, vp, vp, vp,
+                                                          i32, i32, vp]),
+        "madrl_pursuit_set_model_state": (i32, [vp, vp]),
         # frames
         "madrl_ww_render": (i32, [vp, i32, vp, i32, vp, vp, vp]),
         "madrl_hostage_render": (i32, [vp, i32, vp, i32, vp, vp, vp]),

@@ -21,7 +21,10 @@ import torch
 from . import _lib
 from ._lib import _ptr
 
-Rollout = collections.namedtuple("Rollout", "actions obs rew done info extras state policy_obs")
+class Rollout(collections.namedtuple("Rollout", "actions obs rew done info extras state policy_obs")):
+    """PolicyRollout's result.  `evader_actions` (an attribute, not a field, so that the tuple keeps its length):
+    with an `evader_policy`, the Pursuit evaders' actions int32 [T, E, Ne]; otherwise None."""
+    evader_actions = None
 
 
 def _map_state(fn, state):
@@ -116,15 +119,32 @@ class PolicyRollout(object):
     and each later call takes the previous call's ``policy_obs[-1]``.  The wrappers need float32 or bfloat16
     observations, ``auto_reset`` and, for Pursuit, ``flatten=True`` (ObservationBuffer takes 1-D observations).
 
+    Evaders in the loop (Pursuit engines only): ``evader_policy(model_state [E, 4, xs, ys]) -> [E, Ne]`` actions
+    (anything ``copy_`` can write into int32; a value outside 0..3 stays) is called at every step before the
+    engine's launch, on the model_state that the previous launch wrote -- what the reference's evader controller
+    sees at that point of ``step`` (pursuit_evade.py:237-241) -- and evader j of env e moves by its [e, j] (j the
+    original index).  It reads the engine's ``set_model_state`` tensor, which must be set before the ``reset()``
+    that produced ``obs0``: reset writes the model_state matching ``obs0``, and each call's last launch leaves the
+    one matching its ``obs[-1]`` for the next call::
+
+        ms = torch.zeros((E, 4, xs, ys), device=dev)
+        engine.set_model_state(ms)
+        obs0 = engine.reset()
+        out = PolicyRollout(engine, policy, T, evader_policy=ev_policy)(obs0)   # out.evader_actions [T, E, Ne]
+
     ``__call__(obs0, state0=None)`` returns a ``Rollout`` (actions, obs, rew, done, info, extras, state, policy_obs)
     of VIEWS of the rollout's buffers: the next call overwrites them, so clone what must outlive it.
     """
 
     def __init__(self, engine, policy, T, auto_reset=True, record=None, graph=True, obs_cache=None, frame_stack=1,
-                 standardizer=None):
+                 standardizer=None, evader_policy=None):
         self.engine, self.policy, self.T = engine, policy, T
         self.auto_reset, self.record, self.graph, self.obs_cache = auto_reset, record, graph, obs_cache
         self.frame_stack, self.standardizer = frame_stack, standardizer
+        if evader_policy is not None and not hasattr(engine, "set_evader_controller"):
+            raise ValueError("evader_policy needs a Pursuit engine; %s has no evaders to control"
+                             % type(engine).__name__)
+        self.evader_policy = evader_policy
         self._key = None
         self._graph = None
         self._check_wrappers()
@@ -172,7 +192,8 @@ class PolicyRollout(object):
             bool(std.enable_rewnorm), float(std.scale_reward))
         return (self.T, id(eng), eng.obs_dtype, None if term is None else (term.data_ptr(), tuple(term.shape)),
                 eng.launch_settings, self.auto_reset, self.graph, self._obs_cache(), self.record,
-                tuple((tuple(s.shape), s.dtype) for s in _flat(state0)), state0 is None, self.frame_stack, wrap)
+                tuple((tuple(s.shape), s.dtype) for s in _flat(state0)), state0 is None, self.frame_stack, wrap,
+                self.evader_policy is not None)
 
     def _obs_cache(self):
         if self.obs_cache is not None:
@@ -203,6 +224,12 @@ class PolicyRollout(object):
         if self.frame_stack > 1:
             self._policy_obs = torch.zeros((T,) + self._obs0_shape(), dtype=eng.obs_dtype, device=dev)
         self._extras = None   # allocated at the first policy call: shapes and dtypes are the policy's
+        self._ev = None
+        if self.evader_policy is not None:
+            if eng.model_state is None:
+                raise ValueError("evader_policy reads the engine's model_state: call engine.set_model_state(...) "
+                                 "before the reset() that produced obs0")
+            self._ev = torch.zeros((T, E, eng.n_evaders), dtype=torch.int32, device=dev)
         self._graph = None
 
     def _wrap_step(self, t):
@@ -245,8 +272,12 @@ class PolicyRollout(object):
                 buf[t].copy_(extras[k])
             if self._term is not None:
                 eng.set_terminal_obs(self._term[t:t + 1])
+            ev = {}
+            if self._ev is not None:
+                self._ev[t].copy_(self.evader_policy(eng.model_state))
+                ev = dict(evader_actions=self._ev[t:t + 1])
             eng.rollout(self._act[t:t + 1], auto_reset=self.auto_reset,
-                        out=(obs[t:t + 1], rew[t:t + 1], done[t:t + 1], info[t:t + 1]))
+                        out=(obs[t:t + 1], rew[t:t + 1], done[t:t + 1], info[t:t + 1]), **ev)
             if wrapped:
                 self._wrap_step(t)
             state = reset_state(state, done[t])
@@ -279,6 +310,8 @@ class PolicyRollout(object):
         with torch.cuda.stream(side):
             for _ in range(2):
                 self.policy(self._obs0, self._state0)
+                if self.evader_policy is not None:
+                    self.evader_policy(self.engine.model_state)
         torch.cuda.current_stream(dev).wait_stream(side)
         g = torch.cuda.CUDAGraph()
         with self._engine_settings(), torch.cuda.graph(g):
@@ -308,7 +341,9 @@ class PolicyRollout(object):
                 with self._engine_settings():
                     state = self._loop()
         obs, rew, done, info = self._traj
-        return Rollout(self._act, obs, rew, done, info, dict(self._extras), state, self._policy_obs)
+        r = Rollout(self._act, obs, rew, done, info, dict(self._extras), state, self._policy_obs)
+        r.evader_actions = self._ev
+        return r
 
 
 def _flat(state):

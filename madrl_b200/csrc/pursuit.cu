@@ -69,6 +69,13 @@ struct PEParams {
   int32_t* actions_out;           // [T][E][Np] the actions taken (NULL = not recorded)
   int policy_c2;                  // twice the policy's window centre: R (x = R/2) or 2*(R//2) (Python 2 `/`)
   uint8_t policy_lut[128];        // window cell of the nearest visible evader -> action (host-computed, see pe_policy_table)
+  // EVC instantiations only (the fields sit last so that the other instantiations keep their parameter offsets):
+  // the evaders' action source and the model_state output
+  int ev_random;                  // 1 = the env's Philox stream (the default controller), 0 = ev_act / ev_fixed
+  int ev_fixed;                   // every evader's action when ev_act is NULL (SingleActionPolicy)
+  const int32_t* ev_act;          // evader j of env e at step t: ev_act[t ev_st + e ev_se + j] (original index j)
+  size_t ev_st, ev_se;
+  float* model_state;             // optional [E][4][xs][ys]: the reference's model_state after the launch's last step
 };
 
 // Stream family of the policy's own draws (heuristics/pursuit.py:48,50 `action_space.sample()`): pursuer q
@@ -104,7 +111,10 @@ __device__ __forceinline__ double numpy_mean(const double* a, int n) {
 // FLAT = flatten=True layout (3R^2 [+1]); false = the (R, R, 4) conv layout: compile-time, so the window loop has no
 // layout branch.
 // KEEP = observation rows are stored at normal L2 priority instead of evict-first (store_obs).
-template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP = false>
+// EVC = "evader control": the evaders' actions come from p.ev_act / p.ev_fixed unless p.ev_random, and the launch
+// writes p.model_state.  The draw counter advances by the live count per step whatever the source, so the words of
+// the reset draws and of the heuristic's fallback are those of the random controller (DESIGN §4.2).
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP = false, bool EVC = false>
 __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEParams<O> p) {
   extern __shared__ __align__(16) uint32_t smem_u32[];
   const int lane = threadIdx.x, wib = 0;
@@ -294,8 +304,11 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
             }
           }
           // ---- move live evaders, one stream draw each in index order: pe:238-241, ct:16 -------
+          // (EVC and not ev_random: the caller's action of each live evader instead; its draw is skipped, not
+          // taken back)
+          const bool ev_random = !EVC || p.ev_random;
           int base_rank = 0;
-          {
+          if (ev_random) {
             int n_draws = 0;
 #pragma unroll
             for (int c = 0; c < EPL; ++c) n_draws += __popc(live[c]);
@@ -316,12 +329,19 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
             const bool alive = (live[c] >> lane) & 1u;
             const int rank = base_rank + __popc(live[c] & lanemask_lt());
             if (alive) {
-              const uint32_t word = lds_u32(wcache_a + 4u * (uint32_t)(coff + rank));
-              const int a = u32_to_range(word, 0, 5);
+              int a;
+              if constexpr (EVC) {
+                a = ev_random ? u32_to_range(lds_u32(wcache_a + 4u * (uint32_t)(coff + rank)), 0, 5)
+                    : p.ev_act == nullptr ? p.ev_fixed
+                                          : p.ev_act[(size_t)t * p.ev_st + (size_t)e * p.ev_se + (size_t)(lane + 32 * c)];
+              } else {
+                a = u32_to_range(lds_u32(wcache_a + 4u * (uint32_t)(coff + rank)), 0, 5);
+              }
               const int dx = (a == 0) ? -1 : (a == 1 ? 1 : 0), dy = (a == 2) ? 1 : (a == 3 ? -1 : 0);
               const int nx = ex[c] + dx, ny = ey[c] + dy;
               const uint32_t cur = cell0 + 4u * (ex[c] * ysP + ey[c]), nxt = cell0 + 4u * (nx * ysP + ny);
-              if (a < 4 && lds_low_byte(cur) == 0u && lds_low_byte(nxt) == 0u) {
+              // a caller's action outside 0..3 stays, as the pursuers' do
+              if ((EVC ? (unsigned)a < 4u : a < 4) && lds_low_byte(cur) == 0u && lds_low_byte(nxt) == 0u) {
                 reds_add_u32(cur, 0u - (1u << 16));
                 reds_add_u32(nxt, 1u << 16);
                 ex[c] = nx; ey[c] = ny;
@@ -438,6 +458,21 @@ __global__ void __launch_bounds__(32, 28) pe_kernel(const __grid_constant__ PEPa
           }
           if (FLAT && n_tail && lane < Np) store_obs<KEEP>(obs_t + (size_t)lane * p.D + 3 * RR, obs_cvt<O>(my_idv));   // pe:444-445
         }
+        if constexpr (EVC) {
+          // ---- model_state (pe:152, 201-203, 244-246) of the last step: the occupancy this observation was built
+          // from, before the removals below (pe:244-249).  An auto-reset pass that follows overwrites it.
+          if (p.model_state != nullptr && t == p.T - 1) {
+            float* ms = p.model_state + (size_t)e * 4 * xs * ys;
+            const int nc = xs * ys;
+            for (int i = lane; i < nc; i += 32) {
+              const uint32_t w = lds_u32(cell0 + 4u * (uint32_t)((i / ys) * ysP + i % ys));
+              ms[i] = (w & 1u) ? -1.0f : 0.0f;                        // the map: buildings -1
+              ms[nc + i] = (float)((w >> 8) & 0xffu);                  // pursuers
+              ms[2 * nc + i] = (float)((w >> 16) & 0xffu);             // evaders
+              ms[3 * nc + i] = 0.0f;
+            }
+          }
+        }
         need_reset = false;
         if (!pass) {
           // ---- rewards (float64 like the reference, narrowed once): pe:254-262 ------------------
@@ -510,6 +545,9 @@ using namespace madrl;
 struct madrl_pursuit : EngineCore {
   madrl_pursuit_config cfg;
   madrl_pursuit_layout lay;
+  int ev_mode = MADRL_PURSUIT_EVADERS_RANDOM;   // set_evader_control: the evaders' controller of launches without
+  int ev_action = 4;                            // an action tensor
+  float* model_state = nullptr;                 // set_model_state (NULL = off)
 
   StepBytes step_bytes() const {
     const size_t E = cfg.n_envs, Np = cfg.n_pursuers;
@@ -680,22 +718,29 @@ extern "C" int madrl_pursuit_launch_log(int enable, int32_t* records, int max_re
   return g_pe_log.read(enable, records, max_records);
 }
 
-template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP>
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool KEEP, bool EVC>
 static int pe_launch_kernel(madrl_pursuit* h, PEParams<O>& p, size_t smem, cudaStream_t stream) {
   int grid = 0;
-  const int rc = engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT, KEEP>, smem, p.E, stream, p, 0, &grid);
-  if (rc == MADRL_OK) g_pe_log.add({(int32_t)sizeof(O), EPL, CPL, RC, POLICY, FLAT, KEEP, grid});
+  const int rc = engine_launch(h, pe_kernel<O, EPL, CPL, RC, POLICY, FLAT, KEEP, EVC>, smem, p.E, stream, p, 0, &grid);
+  if (rc == MADRL_OK) g_pe_log.add({(int32_t)sizeof(O), EPL, CPL, RC, POLICY | (EVC << 1), FLAT, KEEP, grid});
   return rc;
 }
 
-template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
-static int pe_launch_inst3(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT, bool EVC>
+static int pe_launch_inst4(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
   const size_t smem = 1024 + (size_t)p.smem_per_warp;   // block LUT + per-warp regions
   MADRL_REQUIRE(smem <= 200 * 1024, "map too large for shared memory (%zu B per block)", smem);
   if constexpr (!POLICY)   // the heuristic-policy rollouts always stream
     if (p.mode == 0 && h->obs_cache == MADRL_OBS_CACHE_KEEP)
-      return pe_launch_kernel<O, EPL, CPL, RC, false, FLAT, true>(h, p, smem, stream);
-  return pe_launch_kernel<O, EPL, CPL, RC, POLICY, FLAT, false>(h, p, smem, stream);
+      return pe_launch_kernel<O, EPL, CPL, RC, false, FLAT, true, EVC>(h, p, smem, stream);
+  return pe_launch_kernel<O, EPL, CPL, RC, POLICY, FLAT, false, EVC>(h, p, smem, stream);
+}
+
+template <typename O, int EPL, int CPL, int RC, bool POLICY, bool FLAT>
+static int pe_launch_inst3(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream) {
+  // the EVC instantiation runs whenever the evaders are not the random controller's or model_state is wanted
+  return (p.ev_random && p.model_state == nullptr) ? pe_launch_inst4<O, EPL, CPL, RC, POLICY, FLAT, false>(h, p, stream)
+                                                   : pe_launch_inst4<O, EPL, CPL, RC, POLICY, FLAT, true>(h, p, stream);
 }
 
 template <typename O, int EPL, int CPL, int RC, bool POLICY>
@@ -713,10 +758,16 @@ static int pe_launch_inst(madrl_pursuit* h, PEParams<O>& p, cudaStream_t stream)
 template <typename O>
 static int pe_launch_t(madrl_pursuit* h, int mode, int T, const int32_t* actions, void* obs, float* rew,
                        uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream,
-                       const void* policy_obs0, int32_t* actions_out, int policy_c2) {
+                       const void* policy_obs0, int32_t* actions_out, int policy_c2, const int32_t* ev_act,
+                       size_t ev_st, size_t ev_se) {
   const madrl_pursuit_config& c = h->cfg;
   PEParams<O> p;
   p.policy_obs0 = (const O*)policy_obs0; p.actions_out = actions_out; p.policy_c2 = policy_c2;
+  // the evaders' controller: the caller's action tensor, else the handle's (set_evader_control)
+  p.ev_act = ev_act; p.ev_st = ev_st; p.ev_se = ev_se;
+  p.ev_random = (ev_act == nullptr && h->ev_mode == MADRL_PURSUIT_EVADERS_RANDOM) ? 1 : 0;
+  p.ev_fixed = h->ev_action;
+  p.model_state = h->model_state;
   memset(p.policy_lut, 4, sizeof(p.policy_lut));
   if (policy_obs0 != nullptr) pe_policy_table(c.obs_range, policy_c2, p.policy_lut);
   p.E = c.n_envs; p.env_id_base = c.env_id_base; p.Np = c.n_pursuers; p.Ne = c.n_evaders;
@@ -758,10 +809,13 @@ static int pe_launch_t(madrl_pursuit* h, int mode, int T, const int32_t* actions
 
 static int pe_launch(madrl_pursuit* h, int mode, int T, const int32_t* actions, void* obs, float* rew,
                      uint8_t* done, int32_t* info, const uint8_t* mask, int auto_reset, cudaStream_t stream,
-                     const void* policy_obs0 = nullptr, int32_t* actions_out = nullptr, int policy_c2 = 0) {
+                     const void* policy_obs0 = nullptr, int32_t* actions_out = nullptr, int policy_c2 = 0,
+                     const int32_t* ev_act = nullptr, size_t ev_st = 0, size_t ev_se = 0) {
   return h->obs_format == MADRL_OBS_BF16
-             ? pe_launch_t<uint16_t>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out, policy_c2)
-             : pe_launch_t<float>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0, actions_out, policy_c2);
+             ? pe_launch_t<uint16_t>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0,
+                                     actions_out, policy_c2, ev_act, ev_st, ev_se)
+             : pe_launch_t<float>(h, mode, T, actions, obs, rew, done, info, mask, auto_reset, stream, policy_obs0,
+                                  actions_out, policy_c2, ev_act, ev_st, ev_se);
 }
 
 extern "C" int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, void* obs_dev, void* stream) {
@@ -769,25 +823,58 @@ extern "C" int madrl_pursuit_reset(madrl_pursuit* h, const uint8_t* mask_dev, vo
   return pe_launch(h, 1, 1, nullptr, obs_dev, nullptr, nullptr, nullptr, mask_dev, 0, (cudaStream_t)stream);
 }
 
-extern "C" int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, void* obs_dev,
-                                     float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
-                                     int auto_reset, void* stream) {
+extern "C" int madrl_pursuit_rollout_evaders(madrl_pursuit* h, int T, const int32_t* actions_dev,
+                                             const int32_t* ev_act_dev, size_t ev_st, size_t ev_se, void* obs_dev,
+                                             float* rew_dev, uint8_t* done_dev, int32_t* info_dev, int auto_reset,
+                                             void* stream) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
   MADRL_REQUIRE(T >= 1, "T must be >= 1");
   MADRL_REQUIRE(actions_dev && obs_dev && rew_dev && done_dev && info_dev, "NULL trajectory buffer");
-  return pe_launch(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream);
+  return pe_launch(h, 0, T, actions_dev, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream,
+                   nullptr, nullptr, 0, ev_act_dev, ev_st, ev_se);
 }
 
-extern "C" int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const void* obs0_dev, int32_t* actions_out_dev,
-                                               void* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
-                                               int auto_reset, int floor_centre, void* stream) {
+extern "C" int madrl_pursuit_rollout(madrl_pursuit* h, int T, const int32_t* actions_dev, void* obs_dev,
+                                     float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
+                                     int auto_reset, void* stream) {
+  return madrl_pursuit_rollout_evaders(h, T, actions_dev, nullptr, 0, 0, obs_dev, rew_dev, done_dev, info_dev,
+                                       auto_reset, stream);
+}
+
+extern "C" int madrl_pursuit_rollout_heuristic_evaders(madrl_pursuit* h, int T, const void* obs0_dev,
+                                                       int32_t* actions_out_dev, const int32_t* ev_act_dev,
+                                                       size_t ev_st, size_t ev_se, void* obs_dev, float* rew_dev,
+                                                       uint8_t* done_dev, int32_t* info_dev, int auto_reset,
+                                                       int floor_centre, void* stream) {
   MADRL_REQUIRE(h != nullptr, "handle is NULL");
   MADRL_REQUIRE(T >= 1, "T must be >= 1");
   MADRL_REQUIRE(obs0_dev && obs_dev && rew_dev && done_dev && info_dev, "NULL trajectory buffer");
   MADRL_REQUIRE(h->cfg.layer_norm > 0.0, "the heuristic policy tests `evader channel > 0`: layer_norm must be positive");
   const int R = h->cfg.obs_range;
   return pe_launch(h, 0, T, nullptr, obs_dev, rew_dev, done_dev, info_dev, nullptr, auto_reset, (cudaStream_t)stream,
-                   obs0_dev, actions_out_dev, floor_centre ? 2 * (R / 2) : R);
+                   obs0_dev, actions_out_dev, floor_centre ? 2 * (R / 2) : R, ev_act_dev, ev_st, ev_se);
+}
+
+extern "C" int madrl_pursuit_rollout_heuristic(madrl_pursuit* h, int T, const void* obs0_dev, int32_t* actions_out_dev,
+                                               void* obs_dev, float* rew_dev, uint8_t* done_dev, int32_t* info_dev,
+                                               int auto_reset, int floor_centre, void* stream) {
+  return madrl_pursuit_rollout_heuristic_evaders(h, T, obs0_dev, actions_out_dev, nullptr, 0, 0, obs_dev, rew_dev,
+                                                 done_dev, info_dev, auto_reset, floor_centre, stream);
+}
+
+extern "C" int madrl_pursuit_set_evader_control(madrl_pursuit* h, int mode, int action) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  MADRL_REQUIRE(mode == MADRL_PURSUIT_EVADERS_RANDOM || mode == MADRL_PURSUIT_EVADERS_FIXED,
+                "evader control mode must be MADRL_PURSUIT_EVADERS_RANDOM or _FIXED, got %d", mode);
+  h->ev_mode = mode;
+  h->ev_action = action;
+  return MADRL_OK;
+}
+
+extern "C" int madrl_pursuit_set_model_state(madrl_pursuit* h, float* model_state_dev) {
+  MADRL_REQUIRE(h != nullptr, "handle is NULL");
+  h->model_state = model_state_dev;
+  return MADRL_OK;
 }
 
 extern "C" int madrl_pursuit_step(madrl_pursuit* h, const int32_t* actions_dev, void* obs_dev, float* rew_dev,

@@ -144,8 +144,10 @@ class BatchedEngine(object):
                                            _ptr(done), _ptr(info), int(auto_reset), _lib.stream(self.device)))
         return obs, rew, done, info
 
-    def _rollout_heuristic(self, T, obs0, auto_reset, out, record_actions, actions_out, *extra):
-        """madrl_<abi>_rollout_heuristic; `extra`: the family's arguments before the stream."""
+    def _rollout_heuristic(self, T, obs0, auto_reset, out, record_actions, actions_out, *extra, fn="rollout_heuristic",
+                           mid=()):
+        """madrl_<abi>_<fn>; `mid`: the family's arguments after the actions buffer, `extra`: those before the
+        stream."""
         E, A = self.n_envs, self._n_acting
         _lib.require_tensor(obs0, "obs0", self.obs_dtype, (E, A, self.obs_dim), self.device)
         obs, rew, done, info = self._outputs(T, out, auto_reset)
@@ -155,9 +157,8 @@ class BatchedEngine(object):
         else:
             act = torch.empty(act_shape, dtype=self._act_dtype, device=self.device) if record_actions else None
         with torch.cuda.device(self.device):
-            _lib.check(self._fn("rollout_heuristic")(self._h, T, _ptr(obs0), _ptr(act), _ptr(obs), _ptr(rew),
-                                                     _ptr(done), _ptr(info), int(auto_reset), *extra,
-                                                     _lib.stream(self.device)))
+            _lib.check(self._fn(fn)(self._h, T, _ptr(obs0), _ptr(act), *mid, _ptr(obs), _ptr(rew), _ptr(done),
+                                    _ptr(info), int(auto_reset), *extra, _lib.stream(self.device)))
         return act, obs, rew, done, info
 
     def set_obs_cache(self, mode):
@@ -169,15 +170,15 @@ class BatchedEngine(object):
 
     obs_cache = _lib.OBS_CACHE_STREAM
 
-    def step(self, actions, auto_reset=False, out=None):
+    def step(self, actions, auto_reset=False, out=None, **rollout_kw):
         """One lockstep step.  actions [E, A, *act_tail] (or anything reshapeable to it).  `out`: caller buffers
         (obs [E, A, D], rew [E, A], done [E], info [E, *info_tail]) written instead of new tensors; the
-        returned values are then views of them."""
+        returned values are then views of them.  `rollout_kw`: the family's further rollout() arguments."""
         a = torch.as_tensor(actions, device=self.device, dtype=self._act_dtype).reshape(
             (1, self.n_envs, self._n_acting) + self._act_tail)
         if out is not None:
             out = tuple(t.unsqueeze(0) if isinstance(t, torch.Tensor) else t for t in out)
-        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset, out=out)
+        obs, rew, done, info = self.rollout(a, auto_reset=auto_reset, out=out, **rollout_kw)
         if len(self._info_keys) == 1:
             return obs[0], rew[0], done[0], {self._info_keys[0]: info[0]}
         return obs[0], rew[0], done[0], {k: info[0, :, i] for i, k in enumerate(self._info_keys)}

@@ -11,6 +11,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from ._lib import _ptr
 from .core import Agent, EzPickle
 from .engine import BatchedEngine, DropInEnv
 from .spaces import Box, Discrete
@@ -123,15 +124,129 @@ class BatchedPursuitEvade(BatchedEngine):
         self._launch_settings_changed()
 
     def rollout_heuristic(self, T, obs0, auto_reset=True, out=None, record_actions=True, py2_division=True,
-                          actions_out=None):
+                          actions_out=None, evader_actions=None):
         """T lockstep steps in one launch with the reference's hand-written policy
         (heuristics/pursuit.py:18-50: walk towards the nearest visible evader, a random move when none is
         visible) evaluated inside the kernel: closed loop, no action tensor, no per-step launch.
         obs0 [E, Np, D] = the observation the first action is computed from (`reset()`'s, or `obs[-1]` of
         the previous rollout).  `py2_division`: the window centre `xs / 2` (heuristics/pursuit.py:23) as
         Python 2 -- the reference's language -- computes it (R // 2); False = Python 3 true division.
+        `evader_actions`: as rollout()'s.
         Returns (actions int32 [T,E,Np] or None, obs, rew, done, removed)."""
-        return self._rollout_heuristic(T, obs0, auto_reset, out, record_actions, actions_out, int(bool(py2_division)))
+        if evader_actions is None:
+            return self._rollout_heuristic(T, obs0, auto_reset, out, record_actions, actions_out,
+                                           int(bool(py2_division)))
+        st, se = self._evader_strides(evader_actions, T)
+        return self._rollout_heuristic(T, obs0, auto_reset, out, record_actions, actions_out, int(bool(py2_division)),
+                                       fn="rollout_heuristic_evaders", mid=(_ptr(evader_actions), st, se))
+
+    # ---- the evaders' controller (pursuit_evade.py:87 evader_controller, DESIGN §4.2) ----
+    evader_controller = None   # set_evader_controller's argument
+    model_state = None         # set_model_state's tensor
+
+    def set_evader_controller(self, action=None):
+        """The evaders' controller of every launch that is given no `evader_actions`: None = the reference's
+        default RandomPolicy(5), one draw of the env's stream per live evader per step; an int `a` =
+        SingleActionPolicy(a), every evader takes action a each step (4 = stay: the stationary evaluation;
+        a value outside 0..3 stays too).  evaluate_heuristic / evaluate_policy on this engine then run against
+        those evaders.  A launch setting: a PolicyRollout graph is re-captured after it."""
+        if action is None:
+            mode, a = _lib.PURSUIT_EVADERS_RANDOM, 4
+        else:
+            if isinstance(action, bool) or not isinstance(action, (int, np.integer)):
+                raise TypeError("the evader controller must be None (random) or an int action, got %r" % (action,))
+            if not -2 ** 31 <= int(action) < 2 ** 31:
+                raise ValueError("the evader action must fit in int32, got %d" % action)
+            mode, a = _lib.PURSUIT_EVADERS_FIXED, int(action)
+        _lib.check(self._L.madrl_pursuit_set_evader_control(self._h, mode, a))
+        self.evader_controller = None if action is None else a
+        self._launch_settings_changed()
+
+    def set_model_state(self, out):
+        """After this call reset() and every rollout write `out`, float32 [E, 4, xs, ys] on the engine's device: the
+        reference's model_state (pursuit_evade.py:152) of each env they touch as it stands after the launch's last
+        step -- channel 0 the map (-1 building, 0 free), 1 pursuer counts, 2 evader counts, 3 zeros -- taken, like
+        the reference, before that step's removals (an evader caught at the last step is still counted).  It is
+        what the reference hands the evader controller at the next step.  None switches it off."""
+        E, xs, ys = self.n_envs, self.map_pool.shape[1], self.map_pool.shape[2]
+        _lib.require_tensor(out, "model_state", torch.float32, (E, 4, xs, ys), self.device, optional=True)
+        _lib.check(self._L.madrl_pursuit_set_model_state(self._h, _ptr(out)))
+        self.model_state = out
+        self._launch_settings_changed()
+
+    def _evader_strides(self, ev, T):
+        """Check a caller's evader actions int32 [T, E, Ne] -> the element strides (step, env) the kernel indexes
+        with.  Any strides >= 0 are taken as long as the evader axis is dense, so an expanded view (one row of
+        Ne actions for every env and step: stride 0 and 0) is read without a copy."""
+        _lib.require_tensor(ev, "evader_actions", torch.int32, (T, self.n_envs, self.n_evaders), self.device,
+                            contiguous=False)
+        if self.n_evaders > 1 and ev.stride(2) != 1:
+            raise ValueError("evader_actions must be dense along the evader axis (stride 1), got strides %s"
+                             % (ev.stride(),))
+        return ev.stride(0), ev.stride(1)
+
+    def rollout(self, actions, auto_reset=True, out=None, evader_actions=None):
+        """BatchedEngine.rollout.  `evader_actions` int32 [T, E, Ne] on the engine's device moves evader j of env
+        e at step t by evader_actions[t, e, j] (j its original index; entries of removed evaders and of evaders
+        that do not exist this episode are not read; a value outside 0..3 stays) instead of the controller of
+        set_evader_controller."""
+        if evader_actions is None:
+            return super().rollout(actions, auto_reset, out)
+        actions = actions.to(device=self.device, dtype=self._act_dtype).contiguous()
+        T = _lib.require_tensor(actions, "actions", self._act_dtype, (None, self.n_envs, self._n_acting),
+                                self.device).shape[0]
+        st, se = self._evader_strides(evader_actions, T)
+        obs, rew, done, info = self._outputs(T, out, auto_reset)
+        with torch.cuda.device(self.device):
+            _lib.check(self._L.madrl_pursuit_rollout_evaders(self._h, T, _ptr(actions), _ptr(evader_actions), st, se,
+                                                             _ptr(obs), _ptr(rew), _ptr(done), _ptr(info),
+                                                             int(auto_reset), _lib.stream(self.device)))
+        return obs, rew, done, info
+
+    def step(self, actions, auto_reset=False, out=None, evader_actions=None):
+        """BatchedEngine.step.  `evader_actions`: int32 [E, Ne], rollout()'s for one step."""
+        if evader_actions is None:
+            return super().step(actions, auto_reset, out)
+        _lib.require_tensor(evader_actions, "evader_actions", torch.int32, (self.n_envs, self.n_evaders), self.device,
+                            contiguous=False)
+        return super().step(actions, auto_reset, out, evader_actions=evader_actions.unsqueeze(0))
+
+
+class RandomPolicy(object):
+    """The reference's default evader controller (utils/Controllers.py:8-16): a uniform action of
+    `n_actions`.  PursuitEvade runs RandomPolicy(5) on the device, from the env's own stream."""
+
+    def __init__(self, n_actions, rng=np.random.RandomState()):
+        self.rng = rng
+        self.n_actions = n_actions
+
+    def act(self, state):
+        return self.rng.randint(self.n_actions)
+
+
+class SingleActionPolicy(object):
+    """The reference's constant controller (utils/Controllers.py:19-26): SingleActionPolicy(4) keeps the evaders
+    where they spawned (the stationary evaluation)."""
+
+    def __init__(self, a):
+        self.action = a
+
+    def act(self, state):
+        return self.action
+
+
+def _controller_kind(c):
+    """(fixed action or None, host controller?) of a drop-in's evader_controller: None and RandomPolicy(5) are the
+    device's random controller; a SingleActionPolicy (this module's or any class of that name with `.action`) is
+    the fixed one; any other object with act(model_state) is called on the host."""
+    name = type(c).__name__
+    if c is None or (name == 'RandomPolicy' and getattr(c, 'n_actions', None) == 5):
+        return None, False
+    if name == 'SingleActionPolicy' and hasattr(c, 'action'):
+        return int(c.action), False
+    if not callable(getattr(c, 'act', None)):
+        raise TypeError("evader_controller must have act(model_state), got %r" % (c,))
+    return None, True
 
 
 class PursuitEvade(DropInEnv):
@@ -160,7 +275,7 @@ class PursuitEvade(DropInEnv):
         self.term_evade = kw.pop('term_evade', -5.0)
         self.urgency_reward = kw.pop('urgency_reward', 0.0)
         self.include_id = kw.pop('include_id', True)
-        if not kw.pop('train_pursuit', True):
+        if not kw.pop('train_pursuit', True):   # DESIGN §8: the reference's evader-training mode does not hold together
             raise NotImplementedError("train_pursuit=False is not supported by the batched engine")
         self.surround = kw.pop('surround', True)
         self.constraint_window = kw.pop('constraint_window', 1.0)
@@ -170,9 +285,11 @@ class PursuitEvade(DropInEnv):
         self._engine_kwargs = dict(device=kw.pop('device', None))
         self._seed_value = kw.pop('seed', 0)
         self._env_id = kw.pop('env_id', 0)
-        for k in ('ally_layer', 'opponent_layer', 'evader_controller', 'pursuer_controller', 'initial_config'):
+        for k in ('ally_layer', 'opponent_layer', 'pursuer_controller', 'initial_config'):
             if kw.pop(k, None) is not None:
                 raise NotImplementedError("%s cannot be injected into the batched engine" % k)
+        self.evader_controller = kw.pop('evader_controller', None)
+        self._ev_fixed, self._ev_host = _controller_kind(self.evader_controller)
         n = 3 * self.obs_range ** 2 + (1 if self.include_id else 0)
         self.low, self.high = np.zeros(n), np.ones(n)
         self.action_space = Discrete(5)
@@ -185,7 +302,7 @@ class PursuitEvade(DropInEnv):
 
     def _make_engine(self, n_envs, **kw):
         # looks up the module-level class at call time, so that a test double can stand in for it
-        return BatchedPursuitEvade(n_envs, self.map_pool, n_evaders=self.n_evaders, n_pursuers=self.n_pursuers,
+        eng = BatchedPursuitEvade(n_envs, self.map_pool, n_evaders=self.n_evaders, n_pursuers=self.n_pursuers,
                                    obs_range=self.obs_range, flatten=self.flatten, layer_norm=self.layer_norm,
                                    n_catch=self.n_catch, catchr=self.catchr, term_pursuit=self.term_pursuit,
                                    urgency_reward=self.urgency_reward, include_id=self.include_id,
@@ -193,11 +310,23 @@ class PursuitEvade(DropInEnv):
                                    sample_maps=self.sample_maps, reward_mech=self._reward_mech,
                                    random_opponents=self.random_opponents, max_opponents=self.max_opponents,
                                    seed=self._seed_value, **self._engine_kwargs, **kw)
+        if self._ev_fixed is not None:
+            eng.set_evader_controller(self._ev_fixed)
+        return eng
 
     def setup(self):
         self.pursuers = [DiscreteAgent(self.obs_range, flatten=self.flatten) for _ in range(self.n_pursuers)]
         super().setup()
         self._n_live = self.n_evaders
+        if self._ev_host:
+            self._model_state = torch.zeros((1, 4, self.xs, self.ys), dtype=torch.float32, device=self._engine.device)
+            self._engine.set_model_state(self._model_state)
+
+    def vec_env_executor(self, n_envs, max_path_length):
+        if self._ev_host:
+            raise NotImplementedError("a host evader_controller steps one env at a time; the batched executor "
+                                      "takes None, RandomPolicy(5) or SingleActionPolicy")
+        return super().vec_env_executor(n_envs, max_path_length)
 
     @property
     def agents(self):
@@ -227,7 +356,16 @@ class PursuitEvade(DropInEnv):
             acts = np.asarray(actions).reshape(-1)[:self.n_pursuers]
         else:  # one joint action, pursuit_evade.py:233
             acts = np.array(np.unravel_index(actions, self.act_dims))
-        obs, rew, done, info = self._engine.step(acts.astype(np.int32)[None], auto_reset=False)
+        kw = {}
+        if self._ev_host:   # pe:237-241: act(model_state) once per live evader, in index order
+            ms = self._model_state[0].cpu().numpy()
+            gone = int(self._engine.state['gone'][0].item())
+            a = np.full(self.n_evaders, 4, np.int32)
+            for j in range(self.n_evaders):
+                if not (gone >> j) & 1:
+                    a[j] = self.evader_controller.act(ms)
+            kw['evader_actions'] = torch.as_tensor(a[None], device=self._engine.device)
+        obs, rew, done, info = self._engine.step(acts.astype(np.int32)[None], auto_reset=False, **kw)
         obs = obs.cpu().numpy().astype(np.float64)
         rew = rew[0].cpu().numpy().astype(np.float64)
         removed = int(info['removed'][0].item())
